@@ -2,7 +2,7 @@
 """Benchmark of the DeepSpeech2 train step (BASELINE.json metric: utterances/sec, 161x1000 synthetic
 spectrograms).  One JSON line on stdout (rank 0).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--workload NAME] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = forward + CTC + backward (+ one gradient all-reduce for N>1) + fused clip/AdamW step on one
@@ -11,6 +11,10 @@ batch of B=32 utterances per GPU (weak scaling).  `value` is timed with the batc
 read back D2H inside the timed region.  `--impl reference` times the reference's own CPU path (the
 oracle port issuing the same ATen calls: oneDNN conv, packed `_VF.lstm`, `ctc_loss`, autograd) on the
 host cores of the box, on a bounded sample of the same workload.
+
+`--dump-outputs DIR` writes what the last timed step computed, as float32 / float64 .npy files: `loss.npy` and
+`params_sample.npy` (a fixed, seeded sample of 2^21 entries of the updated flat parameter vector).  Inputs and
+initial weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -75,11 +79,11 @@ def load_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))), "measured"
-    return 6650.0, 1590.0, "fallback"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region"""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -194,7 +198,7 @@ def _oracle_cfg(workload):
 def stock_cuda_baseline(workload, P0, batch, steps=10, warmup=3):
     """north_star's denominator: the reference's stock PyTorch CUDA path — the ATen calls of reference model.py
     (cuDNN conv / packed cuDNN RNN, ATen CTC, clip_grad_norm_, torch AdamW) issued by the oracle port on the GPU,
-    starting from the SAME weights and the SAME batch as the B200 arm.  Three variants so that the comparison is
+    starting from the SAME weights and the SAME batch as the CUDA arm.  Three variants so that the comparison is
     not against a handicapped baseline (SURVEY.md §8d):
       default      torch's default flags (cudnn.allow_tf32=True, matmul.allow_tf32=False, cudnn.benchmark=False —
                    reference lightning_config.py:59), fp32
@@ -259,7 +263,7 @@ def stock_cuda_baseline(workload, P0, batch, steps=10, warmup=3):
              torch.backends.cuda.matmul.allow_tf32) = saved
         torch.cuda.empty_cache()
     res["kind"] = ("stock torch CUDA ops (cuDNN conv/RNN, ATen CTC, clip_grad_norm_, torch AdamW) issued by the "
-                   "oracle port; same initial weights and batch as the B200 arm")
+                   "oracle port; same initial weights and batch as the CUDA arm")
     return res
 
 
@@ -278,7 +282,7 @@ def _group_of(name):
 
 def parity_fullsize(workload, model, flat, P0, batch):
     """The benchmarked configuration against the fp32 reference arithmetic, at full size and with the same weights:
-    the B200 arm (current precision mode) vs the reference's own ATen calls on the GPU with every TF32 switch OFF
+    the CUDA arm (current precision mode) vs the reference's own ATen calls on the GPU with every TF32 switch OFF
     (cuDNN fp32 conv/RNN, fp32 matmul) and the CTC lattice in float64.  `oracle/` is the checker here, nothing of
     it is timed.  Reports logits / loss / per-parameter-group gradient errors (rel = max|a-b| / max|b|,
     rel_l2 = ||a-b|| / ||b||)."""
@@ -336,7 +340,7 @@ def parity_fullsize(workload, model, flat, P0, batch):
         del stock_logits, stock_grads
     finally:
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.benchmark = saved
-    # ---- B200 arm, same weights
+    # ---- CUDA arm, same weights
     model.load_state_dict(P0)
     flat.zero_grad()
     got_logits, _, _ = model(x, sizes)
@@ -362,6 +366,18 @@ def parity_fullsize(workload, model, flat, P0, batch):
     del ref_grads, ref_logits, got_logits
     torch.cuda.empty_cache()
     return res
+
+
+def dump_outputs(out_dir, loss, flat, n_sample=1 << 21):
+    """the last timed step's results: its loss and a fixed, seeded sample of the updated flat parameter vector"""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([loss], dtype=np.float64))
+    data = flat.data.detach().reshape(-1)
+    g = torch.Generator().manual_seed(20240611)
+    idx = torch.randperm(data.numel(), generator=g)[:min(n_sample, data.numel())].sort().values
+    np.save(os.path.join(out_dir, "params_sample.npy"), data[idx.to(data.device)].float().cpu().numpy())
 
 
 def run_b200(args):
@@ -390,7 +406,7 @@ def run_b200(args):
     flat = FlatParams(model, direct_grads=True)   # backward kernels write straight into the flat gradient buffer
     if not args.no_defer:
         # the step runs on a high-priority stream; the weight-gradient GEMMs of each recurrent layer are queued on a
-        # normal-priority side stream and fill the SMs / pipes the next layer's latency-bound sweep leaves idle
+        # normal-priority side stream and use the pipes the next layer's latency-bound sweep leaves idle
         main_stream = torch.cuda.Stream(device=dev, priority=-1)
         main_stream.wait_stream(torch.cuda.current_stream(dev))
         torch.cuda.set_stream(main_stream)
@@ -398,7 +414,7 @@ def run_b200(args):
     opt = FusedOptimizer(flat, model.optim_cfg, max_norm=400.0)
     n_params = sum(p.numel() for p in model.parameters())
 
-    # the weights every arm of this run starts from (B200 timing, full-size parity check, stock CUDA baseline)
+    # the weights every arm of this run starts from (CUDA timing, full-size parity check, stock CUDA baseline)
     P0 = {k: v.detach().clone() for k, v in model.state_dict().items()}
     x, targets, pct, tsz = synth_batch(B, T, L, seed=1234 + rank)
     x_pinned = x.pin_memory()
@@ -466,9 +482,11 @@ def run_b200(args):
         sampler.start()
     ms_dev, launches, loss_val = timed(args.steps, e2e=False)
     log(f"device-resident: {ms_dev:.2f} ms/step")
-    ms_e2e, _, _ = timed(args.steps, e2e=True)
+    ms_e2e, _, loss_e2e = timed(args.steps, e2e=True)
     log(f"e2e: {ms_e2e:.2f} ms/step")
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss_e2e, flat)
 
     # ---- per-block device times (cudaEvent ranges inside the library) for the roofline of the dominant kernel
     prof = {}
@@ -499,19 +517,13 @@ def run_b200(args):
     fwd_bytes = (G * tbh + G * H * H * 4 + tbh * (2 if rnn == "lstm" else 1)) * D_ * layers
     bwd_bytes = ((2 * G + 3) * tbh + G * H * H * 4) * D_ * layers
     roofs = {}
-    traffic_db = {}
-    try:   # DRAM bytes per launch from the committed ncu --set full captures (librispeech workload only)
-        if args.workload == "librispeech" and B == 32:
-            traffic_db = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-    except Exception:
-        traffic_db = {}
     for tag, nbytes in (("rnn_fwd_sweep", fwd_bytes), ("rnn_bwd_sweep", bwd_bytes)):
         if tag in prof and prof[tag]["ms_per_step"] > 0:
             nl = max(1, prof[tag]["ranges_per_step"])          # launches per step (one per layer)
             ms_launch = prof[tag]["ms_per_step"] / nl
             ach = (nbytes / nl) / (ms_launch * 1e-3) / 1e9
             roofs[tag] = {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak,
-                          "traffic": traffic_db.get(tag, {}).get("dram_bytes_per_launch"), "peak_source": which,
+                          "peak_source": which,
                           "algorithmic_bytes_per_launch": nbytes / nl, "launches_per_step": nl,
                           "ms_per_launch": ms_launch, "ms_per_step": prof[tag]["ms_per_step"],
                           "note": "latency-bound: T' serial steps of (grid barrier + MMA issue chain + epilogue); "
@@ -523,7 +535,7 @@ def run_b200(args):
         ctc_bytes = 2 * Tp * B * Cn * 4 + B * L * 8 + 2 * B * 4
         ach = ctc_bytes / (prof["ctc"]["ms_per_step"] * 1e-3) / 1e9
         roofs["ctc"] = {"bound": "hbm", "achieved": ach, "peak": hbm_peak, "unit": "GB/s", "frac": ach / hbm_peak,
-                        "traffic": traffic_db.get("ctc", {}).get("dram_bytes_per_launch"), "peak_source": which,
+                        "peak_source": which,
                         "algorithmic_bytes_per_launch": ctc_bytes, "launches_per_step": 1,
                         "ms_per_launch": prof["ctc"]["ms_per_step"], "ms_per_step": prof["ctc"]["ms_per_step"],
                         "note": "latency-bound: T' dependent lattice steps per utterance, B*2 CTAs; the HBM fraction "
@@ -544,7 +556,7 @@ def run_b200(args):
         "data": "synthetic",
         "dtype_note": ("dense GEMMs / conv2: TF32 operands (TMA rounds to nearest); recurrent products: fp16 operands "
                        "(10-bit mantissa like TF32; backward gate gradients scaled per step by a power of two); fp32 "
-                       "accumulation in TMEM, fp32 state / activations / gradients / optimizer"
+                       "accumulation in registers, fp32 state / activations / gradients / optimizer"
                        if args.precision == "tf32" else
                        "the reference's `precision: 16`: recurrent-stack GEMMs (input projection, dW_ih, dW_hh, dX) on "
                        "fp16 operand copies (gradients scaled by a power of two per tensor), recurrent products fp16, "
@@ -553,7 +565,7 @@ def run_b200(args):
         "config": {"workload": args.workload, "rnn": f"{layers}x{'bi' if bidir else 'uni'}-{rnn}-{H}",
                    "batch_per_gpu": B, "global_batch": B * world, "frames": T, "target_len": L, "params": n_params,
                    "parallelism": f"dp{world}", "optimizer": "fused clip(400)+AdamW inside the step",
-                   "l2": "per-step working set (activations 3+ GB) exceeds the 126 MB L2; no explicit flush"},
+                   "l2": "per-step working set (activations 3+ GB) exceeds the 50 MB L2; no explicit flush"},
         "e2e": {"value": e2e, "unit": "utt/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": h2d,
                 "d2h_bytes_per_step": 4},
         "gpu_launches": launches, "ffma_fallback_sweeps": int(lib.ds2_fallback_count(0)), "clocks": clocks,
@@ -603,6 +615,8 @@ def main():
     ap.add_argument("--no-stock-cuda", action="store_true", help="skip the stock torch CUDA baseline legs")
     ap.add_argument("--no-parity", action="store_true", help="skip the full-size parity check against fp32 ATen")
     ap.add_argument("--no-defer", action="store_true", help="weight-gradient GEMMs on the compute stream (no side stream)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's loss and a fixed sample of the updated parameters as .npy files")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-"""deepspeech.pytorch_b200 — B200-native DeepSpeech2 train-step path (import as
+"""deepspeech.pytorch_b200 — H100-native DeepSpeech2 train-step path (import as
 `deepspeech_pytorch_b200`; the directory name carries a dot, so a one-file shim at the repo root
 registers the package under that importable name)."""
 from . import _lib
@@ -10,7 +10,7 @@ from .labels import LABELS
 
 
 def set_precision(name: str):
-    """'fp32' (FFMA everywhere), 'tf32' (tcgen05 tensor cores, TF32 operands for the dense GEMMs) or 'fp16' (the
+    """'fp32' (FFMA everywhere), 'tf32' (wgmma tensor cores, TF32 operands for the dense GEMMs) or 'fp16' (the
     reference's `precision: 16`: fp16 operand copies for the recurrent stack's GEMMs, everything else as 'tf32').
     A `DeepSpeech(precision=16)` model selects 'fp16' by itself for its own calls."""
     code = {"fp32": _lib.PREC_FP32, "tf32": _lib.PREC_TF32, "fp16": _lib.PREC_F16}[name]

@@ -71,7 +71,7 @@ void note_fallback(const char* what, int rnn, int T, int B, int H, int D) {
   snprintf(key, sizeof(key), "%s rnn=%d B=%d H=%d D=%d", what, rnn, B, H, D);
   std::lock_guard<std::mutex> lk(mu);
   if (seen[key]++ == 0)
-    fprintf(stderr, "ds2_b200: WARNING tensor-core mode: %s (T=%d) is not eligible for the persistent tcgen05 sweep; "
+    fprintf(stderr, "ds2_b200: WARNING tensor-core mode: %s (T=%d) is not eligible for the persistent tensor-core sweep; "
                     "using one FFMA launch per time step (slow). ds2_fallback_count() counts these.\n", key, T);
 }
 
@@ -103,7 +103,7 @@ void prof_end(cudaStream_t st) {
 
 extern "C" {
 
-const char* ds2_version(void) { return "ds2_b200 0.1.0 (sm_100a)"; }
+const char* ds2_version(void) { return "ds2_b200 0.1.0 (sm_90a)"; }
 const char* ds2_last_error(void) { return ds2::g_err; }
 
 int ds2_device_check(int* sm_count, int* cc_major, int* cc_minor) {
@@ -120,8 +120,8 @@ int ds2_device_check(int* sm_count, int* cc_major, int* cc_minor) {
   if (sm_count) *sm_count = p.multiProcessorCount;
   if (cc_major) *cc_major = p.major;
   if (cc_minor) *cc_minor = p.minor;
-  if (p.major != 10) {
-    ds2::set_error("device %s is sm_%d%d; this library is built for sm_100a only", p.name, p.major, p.minor);
+  if (p.major != 9 || p.minor != 0) {
+    ds2::set_error("device %s is sm_%d%d; this library is built for sm_90a (H100) only", p.name, p.major, p.minor);
     return DS2_ERR_CUDA;
   }
   return DS2_OK;
@@ -140,7 +140,7 @@ int64_t ds2_launch_count(int reset) {
 }
 
 // ---- side stream for deferred work (weight-gradient GEMMs of a recurrent layer run in the shadow of the NEXT layer's
-// latency-bound sweep, which leaves 20 of the 148 SMs and most of every pipe idle) ---------------------------------
+// latency-bound sweep, which leaves most of every pipe idle; DESIGN.md §5.6 has the measured gain) ------------------
 int ds2_set_side_stream(void* stream) {
   ds2::g_side_stream.store(stream);
   return DS2_OK;

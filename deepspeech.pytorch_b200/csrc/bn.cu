@@ -112,7 +112,7 @@ int bn_rows_fwd(int rows, int F, const float* x, const float* gamma, const float
              eps, mean_invstd);
   size_t total = (size_t)rows * F;
   int blocks = (int)((total + 1023) / 1024);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   DS2_LAUNCH(bn_apply_kernel, blocks, 256, 0, st, total, F, x, gamma, beta, mean_invstd, y, xhat);
   return DS2_OK;
@@ -122,7 +122,7 @@ int bn_rows_reapply(int rows, int F, const float* x, const float* gamma, const f
                     const float* mean_invstd, float* y, float* xhat, cudaStream_t st) {
   size_t total = (size_t)rows * F;
   int blocks = (int)((total + 1023) / 1024);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   DS2_LAUNCH(bn_apply_kernel, blocks, 256, 0, st, total, F, x, gamma, beta, mean_invstd, y, xhat);
   return DS2_OK;
@@ -136,7 +136,7 @@ int bn_rows_bwd(int rows, int F, const float* xhat, const float* gamma, const fl
   DS2_LAUNCH(bn_bwd_params_kernel, cdiv(F, 128), 128, 0, st, F, ws_sums, dgamma, dbeta);
   size_t total = (size_t)rows * F;
   int blocks = (int)((total + 1023) / 1024);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   DS2_LAUNCH(bn_bwd_apply_kernel, blocks, 256, 0, st, total, F, 1.0 / (double)rows, xhat, gamma, mean_invstd, dy,
              ws_sums, dx);

@@ -1,4 +1,4 @@
-// Shared host/device helpers for libds2_b200.so (sm_100a only).
+// Shared host/device helpers for libds2_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -13,7 +13,7 @@ namespace ds2 {
 void set_error(const char* fmt, ...);
 extern std::atomic<long long> g_launches;
 int precision();
-inline bool tensor_core_mode() { return precision() != DS2_PREC_FP32; }   // TF32 or precision-16: tcgen05 kernels
+inline bool tensor_core_mode() { return precision() != DS2_PREC_FP32; }   // TF32 or precision-16: wgmma kernels
 inline bool f16_gemm_mode() { return precision() == DS2_PREC_F16; }       // fp16 operands for the dense RNN GEMMs
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
@@ -116,9 +116,11 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 
 // ---- internal cross-file entry points -------------------------------------------------------
 // C[M,N] = alpha*op(A)op(B) + beta*C (row-major, fp32 FFMA kernel; any shape/stride)
+// (ws: room for the split-K partial slabs, gemm_simt_workspace_bytes; without it the kernel makes one pass over K)
 int gemm_simt(int transA, int transB, int M, int N, int K, float alpha, const float* A, int lda, const float* B,
-              int ldb, float beta, float* C, int ldc, cudaStream_t st);
-// tcgen05 TF32 kernel.  Returns 1 if the shape is not eligible (caller falls back to gemm_simt).
+              int ldb, float beta, float* C, int ldc, cudaStream_t st, void* ws = nullptr, size_t ws_bytes = 0);
+size_t gemm_simt_workspace_bytes(int M, int N, int K);
+// wgmma TF32 kernel.  Returns 1 if the shape is not eligible (caller falls back to gemm_simt).
 int gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const float* A, int lda, const float* B,
             int ldb, float beta, float* C, int ldc, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t gemm_tc_workspace_bytes(int transA, int transB, int M, int N, int K);

@@ -280,8 +280,10 @@ __global__ void bn_bwd_reduce_kernel(int B, int D, int T, const float* __restric
 __global__ void bn_bwd_apply_kernel(int B, int D, int T, double inv_count, const float* __restrict__ z,
                                     const float* __restrict__ mi, const float* __restrict__ gamma,
                                     const int32_t* __restrict__ len, const double* __restrict__ sums,
-                                    float* __restrict__ du_dz, float* __restrict__ dbias) {
-  // grid (ceil(T*D/256), CO, B)
+                                    float* __restrict__ du_dz, float* __restrict__ dbias_part) {
+  // grid (ceil(T*D/256), CO, B); the bias gradient of a block goes to dbias_part[c][b][block] (summed in a fixed order
+  // by ordered_sum_kernel: the sum is ~0 after the BatchNorm, and a run-order-dependent rounding of it would change
+  // what the optimizer makes of it)
   const int c = blockIdx.y, b = blockIdx.z;
   const size_t base = ((size_t)b * CO + c) * D * T;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -303,8 +305,23 @@ __global__ void bn_bwd_apply_kernel(int B, int D, int T, double inv_count, const
   if (threadIdx.x == 0) {
     float tot = 0.f;
     for (int w = 0; w < (int)blockDim.x / 32; ++w) tot += red[w];
-    atomicAdd(&dbias[c], tot);
+    dbias_part[((size_t)c * B + b) * gridDim.x + blockIdx.x] = tot;
   }
+}
+
+// out[r] = sum_i part[r * n + i], always in the same order (block r: strided per-thread sums, fixed tree)
+__global__ void ordered_sum_kernel(int n, const float* __restrict__ part, float* __restrict__ out) {
+  __shared__ float red[256];
+  const float* p = part + (size_t)blockIdx.x * n;
+  float s = 0.f;
+  for (int i = threadIdx.x; i < n; i += 256) s += p[i];
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) out[blockIdx.x] = red[0];
 }
 
 __global__ void bn_bwd_params2d_kernel(const double* __restrict__ sums, float* __restrict__ dgamma,
@@ -448,13 +465,18 @@ int conv_tc_run(const float* in_cl, int B, int T, int R_in, int R_out, const flo
                 double* stat_sums, cudaStream_t st);
 int nchw_to_cl(int B, int R, int T, const float* in, float* out, cudaStream_t st);
 int pack_conv2_tc(const float* w2, float* wn_fwd, float* wd_bwd, cudaStream_t st);
-int conv2_wgrad_tc(const float* dz2, const float* a1, float* a1_shifted, int B, int T, float* dw2, cudaStream_t st);
-int conv1_wgrad_tc(const float* dz1, const float* x, float* xs, int B, int T, int Tp, float* dw1, cudaStream_t st);
+int conv2_wgrad_tc(const float* dz2, const float* a1, float* a1_shifted, float* part, int B, int T, float* dw2,
+                   cudaStream_t st);
+int conv1_wgrad_tc(const float* dz1, const float* x, float* xs, float* part, int B, int T, int Tp, float* dw1,
+                   cudaStream_t st);
+size_t conv_wgrad_tc_partial_floats();
 
 struct ConvWs {
   float *wpk1, *wpk2, *wTe, *wTo, *du2, *da1;
   float *taps_f, *taps_b, *cl;     // tensor-core path: packed taps (21x352x32 each), channels-last staging
   float* shifted;                  // tensor-core weight gradient: a1 delayed by 0,1,2,3 time steps
+  float* wg_part;                  // tensor-core weight gradients: per-CTA partial tiles (conv_tc.cu)
+  float* db_part;                  // conv bias gradients: per-block partial sums
   double* sums;   // 4 x 64 doubles: fwd stats 1, fwd stats 2, bwd sums 2, bwd sums 1
 };
 static size_t conv_ws_carve(int B, int T, void* base, ConvWs* w) {
@@ -473,6 +495,8 @@ static size_t conv_ws_carve(int B, int T, void* base, ConvWs* w) {
   p = (float*)take((size_t)21 * 352 * 32 * 4); if (w) w->taps_b = p;
   p = (float*)take((size_t)B * CO * DS2_CONV1_D * Tp * 4); if (w) w->cl = p;
   p = (float*)take((size_t)4 * B * CO * DS2_CONV1_D * (Tp + 4) * 4); if (w) w->shifted = p;
+  p = (float*)take(conv_wgrad_tc_partial_floats() * 4); if (w) w->wg_part = p;
+  p = (float*)take((size_t)CO * B * cdiv((long long)DS2_CONV1_D * Tp, 256) * 4); if (w) w->db_part = p;
   return off;
 }
 
@@ -506,9 +530,9 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
   if (rc) return rc;
   DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D1 * Tp, W.sums, g1, be1, rm1, rv1, training, momentum,
              eps, stats);
-  DS2_LAUNCH(bn_act_kernel, 148 * 8, 256, 0, st, B, D1, Tp, z1, stats, g1, be1, out_len, a1);
+  DS2_LAUNCH(bn_act_kernel, 132 * 8, 256, 0, st, B, D1, Tp, z1, stats, g1, be1, out_len, a1);
   if (tensor_core_mode() && !getenv("DS2_NO_CONV_TC") && !getenv("DS2_NO_CONV_TC_FWD")) {
-    // conv2 on tcgen05: channels-last copy of a1, packed taps, implicit GEMM with the kw taps folded into N
+    // conv2 on wgmma: channels-last copy of a1, packed taps, implicit GEMM with the kw taps folded into N
     rc = nchw_to_cl(B, D1, Tp, a1, W.cl, st);
     if (rc) return rc;
     rc = pack_conv2_tc(w2, W.taps_f, nullptr, st);
@@ -553,7 +577,8 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
              stats + 64, g2, be2, out_len, dy, W.du2, s2);
   DS2_LAUNCH(bn_bwd_params2d_kernel, 1, 32, 0, st, s2, dg2, dbe2);
   DS2_LAUNCH(bn_bwd_apply_kernel, dim3(cdiv(D2 * Tp, 256), CO, B), 256, 0, st, B, D2, Tp, 1.0 / ((double)B * D2 * Tp),
-             z2, stats + 64, g2, out_len, s2, W.du2, db2);
+             z2, stats + 64, g2, out_len, s2, W.du2, W.db_part);
+  DS2_LAUNCH(ordered_sum_kernel, CO, 256, 0, st, B * cdiv(D2 * Tp, 256), W.db_part, db2);
   // ---- conv2 gradients.  Nobody needs dW2 before the optimizer: with a side stream set the weight gradient runs there,
   // next to the data gradient and the (elementwise, HBM-bound) BN1 backward of the main stream, and is joined before
   // the conv1 weight gradient reuses its staging buffer.
@@ -569,7 +594,7 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
         wst = side;
         forked = true;
       }
-      wrc = conv2_wgrad_tc(W.du2, a1, W.shifted, B, Tp, dw2, wst);
+      wrc = conv2_wgrad_tc(W.du2, a1, W.shifted, W.wg_part, B, Tp, dw2, wst);
       if (wrc < 0) return wrc;
       if (forked) {
         int mrc = side_mark_workspace(ws, side);
@@ -584,7 +609,7 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
   const size_t ob = (size_t)CO * D1 * Tp, oc = (size_t)D1 * Tp;
   int rc;
   if (tensor_core_mode() && !getenv("DS2_NO_CONV_TC") && !getenv("DS2_NO_CONV_TC_DGRAD")) {
-    // data gradient on tcgen05: rows y=2i use taps kh=2m (d = i+5-m), rows y=2i+1 taps kh=2m+1
+    // data gradient on wgmma: rows y=2i use taps kh=2m (d = i+5-m), rows y=2i+1 taps kh=2m+1
     rc = nchw_to_cl(B, D2, Tp, W.du2, W.cl, st);
     if (rc) return rc;
     rc = pack_conv2_tc(w2, nullptr, W.taps_b, st);
@@ -608,16 +633,17 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
              z1, stats, g1, be1, out_len, W.da1, W.da1, s1);
   DS2_LAUNCH(bn_bwd_params2d_kernel, 1, 32, 0, st, s1, dg1, dbe1);
   DS2_LAUNCH(bn_bwd_apply_kernel, dim3(cdiv(D1 * Tp, 256), CO, B), 256, 0, st, B, D1, Tp, 1.0 / ((double)B * D1 * Tp),
-             z1, stats, g1, out_len, s1, W.da1, db1);
+             z1, stats, g1, out_len, s1, W.da1, W.db_part);
+  DS2_LAUNCH(ordered_sum_kernel, CO, 256, 0, st, B * cdiv(D1 * Tp, 256), W.db_part, db1);
   if (forked) {   // dW2 done (and its staging buffer free) before this call returns
     int jrc = side_wait_for_workspace(ws, st);
     if (jrc) return jrc;
   }
   {
-    // conv1 weight gradient on tcgen05 (reuses the conv2 weight gradient's staging buffer, which is free by now)
+    // conv1 weight gradient on wgmma (reuses the conv2 weight gradient's staging buffer, which is free by now)
     int wrc = 1;
     if (tensor_core_mode() && !getenv("DS2_NO_CONV_TC") && !getenv("DS2_NO_CONV1_TC_WGRAD")) {
-      wrc = conv1_wgrad_tc(W.da1, x, W.shifted, B, T, Tp, dw1, st);
+      wrc = conv1_wgrad_tc(W.da1, x, W.shifted, W.wg_part, B, T, Tp, dw1, st);
       if (wrc < 0) return wrc;
     }
     if (wrc == 1) DS2_LAUNCH(conv1_dw_kernel, dim3(3, B, C1_DSPLIT), 128, 0, st, B, T, Tp, W.da1, x, dw1);

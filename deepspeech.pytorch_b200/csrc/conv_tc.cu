@@ -1,17 +1,17 @@
-// 32->32 channel convolution (conv2 forward and its data gradient) on tcgen05 tensor cores as an
+// 32->32 channel convolution (conv2 forward and its data gradient) on wgmma tensor cores as an
 // im2col-free implicit GEMM with the horizontal taps folded into N ("tap-in-N"):
 //
 //   for an output row and one vertical tap j, with the input row r_j in channels-last layout (t, ci):
-//       D[p, (kw, co)] += sum_ci  X[r_j][p][ci] * Wn[j][(kw, co)][ci]          (M = 128 positions p,
+//       D[p, (kw, co)] += sum_ci  X[r_j][p][ci] * Wn[j][(kw, co)][ci]          (M = 64 positions p,
 //                                                                               N = 11*32 = 352, K = 32)
 //   and after all vertical taps   out[t][co] = sum_kw D[t + kw - 5][(kw, co)]   (shifted sum, epilogue)
 //
-// The A tile of a tap is ONE contiguous TMA box (128 positions x 32 channels = 128-byte rows, 128B
+// The A tile of a tap is ONE contiguous TMA box (64 positions x 32 channels = 128-byte rows, 128B
 // swizzle, out-of-range rows / positions zero-filled by TMA = the convolution padding), the B tile is
-// the packed tap matrix (352 x 32); no descriptor tricks, no im2col buffer.  A tile produces 118
-// outputs (128 positions minus the 10-position halo).  Accumulators: 352 TMEM columns (two N=176 MMAs
-// per K=8 step).  Epilogue: per kw the 32-column block is read from TMEM and added into a shared-memory
-// output tile at row p-kw; then bias, length mask, NCHW store and the BatchNorm sum / sum-of-squares
+// the packed tap matrix (352 x 32); no descriptor tricks, no im2col buffer.  A tile produces 54
+// outputs (64 positions minus the 10-position halo).  Two MMA warpgroups own one N = 176 half each
+// (88 accumulator registers per thread); their epilogue adds every accumulator at row p-kw into a
+// shared-memory output tile, then bias, length mask, NCHW store and the BatchNorm sum / sum-of-squares
 // partials of the forward pass.
 //
 // The data gradient of the stride-(2,1) convolution is the same kernel run twice (even / odd output
@@ -27,13 +27,13 @@ int make_tmap_nd_f32(CUtensorMap* out, const float* base, int rank, const unsign
 
 namespace cv {
 constexpr int CH = 32, KW = 11, NN = KW * CH;      // 352
-constexpr int MP = 128, TO = MP - (KW - 1);         // positions per tile, outputs per tile (118)
-constexpr int A_BYTES = MP * 128;                   // 16 KB
+constexpr int MP = 64, TO = MP - (KW - 1);          // positions per tile, outputs per tile (54)
+constexpr int A_BYTES = MP * 128;                   // 8 KB
 constexpr int W_HALF = (NN / 2) * 128;              // 176 rows x 128 B = 22528
-constexpr int STAGE_BYTES = A_BYTES + 2 * W_HALF;   // 61440
+constexpr int STAGE_BYTES = A_BYTES + 2 * W_HALF;   // 53248
 constexpr int STAGES = 3;
 constexpr int OUT_LD = 33;
-constexpr int THREADS = 192;
+constexpr int THREADS = 384;                        // warp 0 TMA producer, warps 4..11 two MMA warpgroups
 constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + (TO + 10) * OUT_LD * 4 + 256;
 }  // namespace cv
 
@@ -78,10 +78,8 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* out_s = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);       // [TO+10][33]
-  uint64_t* full = reinterpret_cast<uint64_t*>(out_s + (TO + 10) * OUT_LD);   // 128*33 floats: 8-byte aligned
+  uint64_t* full = reinterpret_cast<uint64_t*>(out_s + (TO + 10) * OUT_LD);   // 64*33 floats: 8-byte aligned
   uint64_t* empty = full + STAGES;
-  uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int t0 = blockIdx.x * TO, d = blockIdx.y, b = blockIdx.z;
@@ -98,16 +96,11 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmW);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(accum_bar, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // two MMA warpgroups
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < (TO + 10) * OUT_LD; i += THREADS) out_s[i] = 0.f;
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     int s = 0;
@@ -119,58 +112,54 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
       mbar_wait(&empty[s], ph ^ 1);
       mbar_arrive_expect_tx_w(&full[s], (uint32_t)STAGE_BYTES);
       uint8_t* st = smem + s * STAGE_BYTES;
-      // A: 128 positions starting at t0-5 (negative / beyond-T coordinates are zero-filled = padding)
+      // A: 64 positions starting at t0-5 (negative / beyond-T coordinates are zero-filled = padding)
       tma_load_4d_w(st, &p.tmA, &full[s], 0, t0 - 5, r, b);
       tma_load_3d_w(st + A_BYTES, &p.tmW, &full[s], 0, 0, wi);
       tma_load_3d_w(st + A_BYTES + W_HALF, &p.tmW, &full[s], 0, NN / 2, wi);
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-  } else if (warp == 1) {
-    // the whole warp runs the loop, one elected lane issues (a single divergent lane pays ~76 cycles per MMA
-    // in uniform-register round trips; see tc_common.cuh)
-    const uint32_t idesc = instr_desc(FMT_TF32, MP, NN / 2);
+  } else if (warp >= 4 && nj > 0) {
+    const int wg = warp / 4 - 1;                      // N half: columns 176 wg .. 176 wg + 175
+    float acc[NN / 4];
+#pragma unroll
+    for (int i = 0; i < NN / 4; ++i) acc[i] = 0.f;
     int s = 0;
     uint32_t ph = 0;
     for (int jj = 0; jj < nj; ++jj) {
       mbar_wait(&full[s], ph);
-      tc_fence_after();
       const uint64_t ad = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES));
-      const uint64_t b0 = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES));
-      const uint64_t b1 = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES + W_HALF));
+      const uint64_t bd = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES + wg * W_HALF));
+      wg_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        mma_tf32_w(tmem_base, ad + (uint64_t)(2 * k), b0 + (uint64_t)(2 * k), idesc, (jj | k) != 0);
-        mma_tf32_w(tmem_base + (uint32_t)(NN / 2), ad + (uint64_t)(2 * k), b1 + (uint64_t)(2 * k), idesc, (jj | k) != 0);
-      }
-      mma_commit_w(&empty[s]);
+      for (int k = 0; k < 4; ++k) Wgmma<NN / 2, false>::mma(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1u);
+      wg_release(&empty[s]);
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-    mma_commit_w(accum_bar);
-  } else {
-    const int q = warp % 4, e = threadIdx.x - 64;
-    const int pl = q * 32 + lane;                     // position inside the tile (TMEM lane)
-    if (nj > 0) {
-      mbar_wait(accum_bar, 0);
-      tc_fence_after();
-      for (int kw = 0; kw < KW; ++kw) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(kw * CH), v);
-        const int to = pl - kw;                       // output this position feeds through tap kw
-        if (to >= 0 && to < TO) {
-          float* row = out_s + to * OUT_LD;
+    // accumulator (position pl, column (kw, co)) feeds output pl - kw.  One kw at a time (the two warpgroups hold
+    // different column blocks; inside a block every output has one contributor): the sum over kw always runs in the
+    // same order, so the result is bit-repeatable.
+    const int w = warp % 4;
+    for (int kw = 0; kw < KW; ++kw) {
 #pragma unroll
-          for (int c = 0; c < CH; ++c) row[c] += v[c];
+      for (int i = 0; i < NN / 16; ++i) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int pl = 16 * w + (lane >> 2) + 8 * (e >> 1);
+          const int n = NN / 2 * wg + 8 * i + 2 * (lane & 3) + (e & 1);
+          const int to = pl - kw;
+          if (n / CH == kw && to >= 0 && to < TO) out_s[to * OUT_LD + n % CH] += acc[4 * i + e];
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
       }
-    } else {
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+      asm volatile("bar.sync 1, 256;" ::: "memory");
     }
-    // bias, mask, NCHW store: warp q owns channels 8q..8q+7, lanes run along time (128-byte stores);
+  }
+  __syncthreads();
+  if (warp >= 4 && warp < 8) {
+    // bias, mask, NCHW store: warp q owns channels 8q..8q+7, lanes run along time;
     // per-channel sum / sum of squares for the BatchNorm of the forward pass
+    const int q = warp % 4;
     const int L = p.out_len ? p.out_len[b] : p.T;
     const int orow_idx = p.out_row_mul * d + p.out_row_off;
-    (void)e;
     for (int cc = 0; cc < 8; ++cc) {
       const int c = q * 8 + cc;
       const float bv = p.bias ? p.bias[c] : 0.f;
@@ -195,9 +184,6 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<512>(tmem_base);
 }
 
 // ---- packing ----------------------------------------------------------------------------------------
@@ -276,24 +262,22 @@ int conv_tc_run(const float* in_cl, int B, int T, int R_in, int R_out, const flo
 //   dW[co][ci][kh][kw] = sum_{b,d,t} dz2[b,co,d,t] * a1[b,ci,2d+kh-10,t+kw-5]
 // GEMM over time (K = t), organised around the INPUT row r = 2d+kh-10: one fetch of the row's eleven shifted tiles
 // (B operand, N = (kw,ci) = 352) serves every vertical tap kh of r's parity, whose dz2 rows d = (r+10-kh)/2 are
-// stacked in M: a CTA owns a group of 4 taps (M = 4 x 32 co = 128) and a slice of the (b, r) pairs, accumulates them
-// all in TMEM (352 columns) and finally adds its 128 x 352 tile into dW with fp32 atomics.  Rows d outside the output
-// are zero-filled by TMA.  (The first version looped over (b, d) for one kh with M = 32 of 64: every input row was
-// fetched once per tap, 19 GB of L2 -> shared-memory traffic per launch = 11 TB/s, the limit; stacking the taps cuts
-// it to 7.6 GB and fills the M = 128 data path.)
-// The producer needs ~110 cycles per TMA instruction, so the eleven shifted 4 KB tiles are fetched with four boxes
-// that span the "shift copy" dimension of a 4-copy tensor (see shift_copies_kernel); the N blocks then sit in the
-// order KW_OF_BLOCK.
+// stacked in M: a CTA owns a group of 2 taps (M = 2 x 32 co = 64) and a slice of the (b, r) pairs, accumulates them
+// all in the registers of two MMA warpgroups (one N = 176 half each) and finally stores its 64 x 352 tile; a second
+// kernel sums the tiles of the slices in a fixed order (bit-repeatable, no float atomics).  Rows d outside the output
+// are zero-filled by TMA.
+// The eleven shifted 4 KB tiles are fetched with four boxes that span the "shift copy" dimension of a 4-copy tensor
+// (see shift_copies_kernel); the N blocks then sit in the order KW_OF_BLOCK.
 namespace wg {
 constexpr int KT = 32;                               // time steps per K chunk (128 bytes)
 constexpr int KH = 21;                               // vertical taps of conv2
-constexpr int KH_PER = 4;                            // vertical taps stacked in M
-constexpr int GROUPS = 3;                            // tap groups per parity: kh = parity + 2 * (4 * g + i)
-constexpr int A_BYTES = KH_PER * 32 * 128;           // 128 M rows
+constexpr int KH_PER = 2;                            // vertical taps stacked in M
+constexpr int GROUPS = 6;                            // tap groups per parity: kh = parity + 2 * (2 * g + i)
+constexpr int A_BYTES = KH_PER * 32 * 128;           // 64 M rows
 constexpr int B_BYTES = cv::NN * 128;                // 352 rows
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;       // 61440
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;       // 53248
 constexpr int STAGES = 3;
-constexpr int THREADS = 192;
+constexpr int THREADS = 384;                         // warp 0 TMA producer, warps 4..11 two MMA warpgroups
 constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 256;
 }  // namespace wg
 
@@ -303,7 +287,7 @@ struct WgradParams {
   CUtensorMap tmS2;   // same tensor, box = 2 copies
   CUtensorMap tmS1;   // same tensor, box = 1 copy
   int B, T, slices;
-  float* dw2;
+  float* part;        // [2 GROUPS][slices][64 rows][352 columns] accumulator tiles, summed by conv2_wgrad_reduce_kernel
 };
 // shared-memory N block j (32 ci rows each) holds tap kw = KW_OF_BLOCK[j]:
 //   box (t0-4, copies 0,1) -> kw 1,0 | (t0, copies 0..3) -> kw 5,4,3,2 | (t0+4, copies 0..3) -> kw 9,8,7,6 | (t0+8, copy 3) -> kw 10
@@ -334,10 +318,9 @@ __global__ void __launch_bounds__(wg::THREADS, 1) conv2_wgrad_tc_kernel(const __
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int parity = blockIdx.x / GROUPS, kh0 = parity + 2 * KH_PER * (blockIdx.x % GROUPS);   // taps kh0 + 2 i
+  if (kh0 >= KH) return;                                // parity 1 has one group fewer (uniform over the CTA)
   const int nkh = min(KH_PER, (KH - 1 - kh0) / 2 + 1);
   const int nr = (DS2_CONV1_D - parity + 1) / 2;        // input rows of this parity: r = 2 r' + parity
   const int pairs = p.B * nr;
@@ -353,15 +336,10 @@ __global__ void __launch_bounds__(wg::THREADS, 1) conv2_wgrad_tc_kernel(const __
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmDz);
     tma_prefetch_desc(&p.tmS4);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(accum_bar, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // two MMA warpgroups
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   int nchunks = 0;
   for (int pi = p0; pi < p1; ++pi)
@@ -387,57 +365,63 @@ __global__ void __launch_bounds__(wg::THREADS, 1) conv2_wgrad_tc_kernel(const __
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // warp-converged issue (one elected lane), as in conv_tc_kernel
-    const uint32_t idesc = instr_desc(FMT_TF32, 128, cv::NN / 2);
+  } else if (warp >= 4) {                             // (no chunks: the tile is stored as zeros)
+    const int wg = warp / 4 - 1;                      // N half: columns 176 wg .. 176 wg + 175
+    float acc[cv::NN / 4];
+#pragma unroll
+    for (int i = 0; i < cv::NN / 4; ++i) acc[i] = 0.f;
     int s = 0;
     uint32_t ph = 0;
     for (int c = 0; c < nchunks; ++c) {
       mbar_wait(&full[s], ph);
-      tc_fence_after();
       const uint64_t ad = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES));
-      const uint64_t b0 = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES));
-      const uint64_t b1 = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES + cv::W_HALF));
+      const uint64_t bd = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES + wg * cv::W_HALF));
+      wg_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        mma_tf32_w(tmem_base, ad + (uint64_t)(2 * k), b0 + (uint64_t)(2 * k), idesc, (c | k) != 0);
-        mma_tf32_w(tmem_base + (uint32_t)(cv::NN / 2), ad + (uint64_t)(2 * k), b1 + (uint64_t)(2 * k), idesc, (c | k) != 0);
-      }
-      mma_commit_w(&empty[s]);
+      for (int k = 0; k < 4; ++k) Wgmma<cv::NN / 2, false>::mma(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1u);
+      wg_release(&empty[s]);
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-    if (nchunks > 0) mma_commit_w(accum_bar);
-  } else if (nchunks > 0) {
-    // M = 128: row m = 32 i + co lives in TMEM lane m; warp quadrant q reads tap i = q, lane = co
-    const int q = warp % 4;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    if (q < nkh) {      // rows of taps beyond the last one were never loaded
-      const int kh = kh0 + 2 * q, co = lane;
-      for (int blk = 0; blk < cv::KW; ++blk) {
-        const int kw = KW_OF_BLOCK[blk];
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(blk * 32), v);
+    // accumulator row m = 32 i + co (tap kh0 + 2 i), column (N block, ci); rows of taps beyond nkh are never read
+    const int w = warp % 4;
+    float* tile = p.part + ((size_t)blockIdx.x * gridDim.y + blockIdx.y) * 64 * cv::NN;
 #pragma unroll
-        for (int ci = 0; ci < 32; ++ci)
-          atomicAdd(&p.dw2[(((size_t)co * 32 + ci) * KH + kh) * 11 + kw], v[ci]);
+    for (int i = 0; i < cv::NN / 16; ++i) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = 16 * w + (lane >> 2) + 8 * hh;
+        const int n = cv::NN / 2 * wg + 8 * i + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(tile + (size_t)m * cv::NN + n) = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<512>(tmem_base);
 }
 
-// dz2: (B,32,41,T) NCHW gate... conv2 output gradient; a1: (B,32,81,T) NCHW; dw2 (32,32,21,11) must be zeroed.
-// Returns 1 when the shape is not eligible (row pitch T*4 bytes must be a multiple of 16).
-int conv2_wgrad_tc(const float* dz2, const float* a1, float* a1_shifted /* 4*B*32*81*(T+4) floats */, int B, int T,
-                   float* dw2, cudaStream_t st) {
+// dW2[co][ci][kh][kw] = sum over the slices (in order) of the tile entries that hold it
+__global__ void conv2_wgrad_reduce_kernel(int slices, const float* __restrict__ part, float* __restrict__ dw2) {
+  using namespace wg;
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= 32 * 32 * KH * cv::KW) return;
+  const int kw = idx % cv::KW, kh = (idx / cv::KW) % KH, ci = (idx / (cv::KW * KH)) % 32, co = idx / (cv::KW * KH * 32);
+  const int parity = kh & 1, q = (kh - parity) / 2, x = parity * GROUPS + q / KH_PER, m = 32 * (q % KH_PER) + co;
+  int blk = 0;
+  while (KW_OF_BLOCK[blk] != kw) ++blk;
+  const float* src = part + (size_t)x * slices * 64 * cv::NN + (size_t)m * cv::NN + blk * 32 + ci;
+  float s = 0.f;
+  for (int y = 0; y < slices; ++y) s += src[(size_t)y * 64 * cv::NN];
+  dw2[idx] = s;
+}
+
+// dz2: (B,32,41,T) NCHW gate... conv2 output gradient; a1: (B,32,81,T) NCHW; dw2 (32,32,21,11) is overwritten;
+// part: conv_wgrad_tc_partial_floats() floats.  Returns 1 when the shape is not eligible (row pitch T*4 bytes must be
+// a multiple of 16).
+int conv2_wgrad_tc(const float* dz2, const float* a1, float* a1_shifted /* 4*B*32*81*(T+4) floats */, float* part,
+                   int B, int T, float* dw2, cudaStream_t st) {
   if (T % 4 != 0) return 1;
   WgradParams p{};
   {
     const size_t rows = (size_t)B * 32 * 81;
-    DS2_LAUNCH(shift_copies_kernel, 148 * 8, 256, 0, st, rows, T, a1, a1_shifted);
+    DS2_LAUNCH(shift_copies_kernel, device_sm_count() * 8, 256, 0, st, rows, T, a1, a1_shifted);
     const unsigned long long Tq = (unsigned long long)T + 4;
     unsigned long long dims[5] = {Tq, 81ull, 32ull, (unsigned long long)B, 4ull};
     unsigned long long str[4] = {Tq * 4, 81ull * Tq * 4, 32ull * 81 * Tq * 4, (unsigned long long)rows * Tq * 4};
@@ -458,13 +442,14 @@ int conv2_wgrad_tc(const float* dz2, const float* a1, float* a1_shifted /* 4*B*3
     int rc = make_tmap_4d_f32(&p.tmDz, dz2, dims, str, box);
     if (rc) return rc;
   }
-  p.B = B; p.T = T; p.slices = 24; p.dw2 = dw2;   // 2 parities x 3 tap groups x 24 slices = 144 CTAs
+  p.B = B; p.T = T; p.slices = 12; p.part = part;   // 2 parities x 6 tap groups x 12 slices = 144 CTAs
   static DeviceOnce attr_once;
   if (attr_once.first()) {
     DS2_CHECK_CUDA(cudaFuncSetAttribute(conv2_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, wg::SMEM_BYTES));
     attr_once.done();
   }
   DS2_LAUNCH(conv2_wgrad_tc_kernel, dim3(2 * wg::GROUPS, p.slices), wg::THREADS, wg::SMEM_BYTES, st, p);
+  DS2_LAUNCH(conv2_wgrad_reduce_kernel, cdiv(32 * 32 * wg::KH * cv::KW, 256), 256, 0, st, p.slices, part, dw2);
   return DS2_OK;
 }
 
@@ -488,7 +473,7 @@ constexpr int A_BYTES = 32 * DI * 128;               // 128 M rows
 constexpr int B_BYTES = NROWS * 128;                 // 12 KB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;       // 28672
 constexpr int STAGES = 6;
-constexpr int THREADS = 192;
+constexpr int THREADS = 384;                         // warp 0 TMA producer, warps 4..11 two MMA warpgroups
 constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 256;
 }  // namespace w1
 __constant__ int KW1_OF_GROUP[12] = {5, 6, 3, 4, 1, 2, -1, 0, 9, 10, 7, 8};
@@ -498,7 +483,7 @@ struct Wgrad1Params {
   CUtensorMap tmX8;   // 5-D (T'+4, 161, B, 2 q, 4 s), box (32, 8, 1, 2, 4)
   CUtensorMap tmX4;   // same tensor, box (32, 8, 1, 2, 2)
   int B, Tp;
-  float* dw1;
+  float* part;        // [CLASSES][slices][128 rows][96 columns] accumulator tiles, summed by conv1_wgrad_reduce_kernel
 };
 
 __global__ void conv1_shift_copies_kernel(int B, int T, int Tp, const float* __restrict__ x, float* __restrict__ xs) {
@@ -520,8 +505,6 @@ __global__ void __launch_bounds__(w1::THREADS, 1) conv1_wgrad_tc_kernel(const __
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int cls = blockIdx.x;
   const int ndb = (DS2_CONV1_D + DI - 1) / DI;              // 21 blocks of output rows
@@ -538,15 +521,10 @@ __global__ void __launch_bounds__(w1::THREADS, 1) conv1_wgrad_tc_kernel(const __
     tma_prefetch_desc(&p.tmDz);
     tma_prefetch_desc(&p.tmX8);
     tma_prefetch_desc(&p.tmX4);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(accum_bar, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // two MMA warpgroups
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<128>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   int nchunks = 0;
   for (int pi = p0; pi < p1; ++pi)
@@ -569,48 +547,72 @@ __global__ void __launch_bounds__(w1::THREADS, 1) conv1_wgrad_tc_kernel(const __
         if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = instr_desc(FMT_TF32, 128, NROWS);
+  } else if (warp >= 4) {                             // (no chunks: the tile is stored as zeros)
+    const int wg = warp / 4 - 1;                      // M half: accumulator rows 64 wg .. 64 wg + 63
+    float acc[NROWS / 2];
+#pragma unroll
+    for (int i = 0; i < NROWS / 2; ++i) acc[i] = 0.f;
     int s = 0;
     uint32_t ph = 0;
     for (int c = 0; c < nchunks; ++c) {
       mbar_wait(&full[s], ph);
-      tc_fence_after();
-      const uint64_t ad = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES));
+      const uint64_t ad = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES)) + (uint64_t)(512 * wg);
       const uint64_t bd = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES));
+      wg_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) mma_tf32_w(tmem_base, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), idesc, (c | k) != 0);
-      mma_commit_w(&empty[s]);
+      for (int k = 0; k < 4; ++k) Wgmma<NROWS, false>::mma(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1u);
+      wg_release(&empty[s]);
       if (++s == STAGES) { s = 0; ph ^= 1; }
     }
-    if (nchunks > 0) mma_commit_w(accum_bar);
-  } else if (nchunks > 0) {
-    // accumulator row m = co * 4 + i sits in TMEM lane m
-    const int q = warp % 4, m = q * 32 + lane, co = m / DI, i = m % DI;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    for (int blk = 0; blk < NROWS / 32; ++blk) {
-      float v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(blk * 32), v);
+    // accumulator row m = co * 4 + i, column n = (tap column group, j)
+    const int w = warp % 4;
+    float* tile = p.part + ((size_t)cls * gridDim.y + blockIdx.y) * 128 * NROWS;
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        const int n = blk * 32 + c, kw = KW1_OF_GROUP[n / RJ], kh = RJ * cls + (n % RJ) - 2 * i;
-        if (kw >= 0 && kh >= 0 && kh < 41) atomicAdd(&p.dw1[((size_t)co * 41 + kh) * 11 + kw], v[c]);
+    for (int i = 0; i < NROWS / 8; ++i) {
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int m = 64 * wg + 16 * w + (lane >> 2) + 8 * hh, n = 8 * i + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(tile + (size_t)m * NROWS + n) = make_float2(acc[4 * i + 2 * hh], acc[4 * i + 2 * hh + 1]);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<128>(tmem_base);
+}
+
+// dW1[co][kh][kw] = sum, in a fixed order (class, output row i, slice), of the tile entries (m = 4 co + i,
+// n = 8 group + j) with kh = 8 class + j - 2 i and KW1_OF_GROUP[group] = kw
+__global__ void conv1_wgrad_reduce_kernel(int slices, const float* __restrict__ part, float* __restrict__ dw1) {
+  using namespace w1;
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= 32 * 41 * 11) return;
+  const int kw = idx % 11, kh = (idx / 11) % 41, co = idx / (11 * 41);
+  int grp = 0;
+  while (KW1_OF_GROUP[grp] != kw) ++grp;
+  float s = 0.f;
+  for (int cls = 0; cls < CLASSES; ++cls)
+    for (int i = 0; i < DI; ++i) {
+      const int j = kh - RJ * cls + 2 * i;
+      if (j < 0 || j >= RJ) continue;
+      const float* src = part + (size_t)cls * slices * 128 * NROWS + (size_t)(DI * co + i) * NROWS + grp * RJ + j;
+      for (int y = 0; y < slices; ++y) s += src[(size_t)y * 128 * NROWS];
+    }
+  dw1[idx] = s;
+}
+
+// floats of the partial tiles of either weight gradient (they run one after the other and share the buffer)
+size_t conv_wgrad_tc_partial_floats() {
+  const size_t c2 = (size_t)2 * wg::GROUPS * 12 * 64 * cv::NN, c1 = (size_t)w1::CLASSES * 24 * 128 * w1::NROWS;
+  return c2 > c1 ? c2 : c1;
 }
 
 // dz1: (B,32,81,T') gradient of the conv1 output (after the BN1 / Hardtanh backward); x: (B,1,161,T); dw1 (32,1,41,11)
-// must be zeroed.  xs: 8 * B * 161 * (T'+4) floats.  Returns 1 when the shape is not eligible (T' % 4 != 0).
-int conv1_wgrad_tc(const float* dz1, const float* x, float* xs, int B, int T, int Tp, float* dw1, cudaStream_t st) {
+// is overwritten.  xs: 8 * B * 161 * (T'+4) floats; part: conv_wgrad_tc_partial_floats() floats.  Returns 1 when the
+// shape is not eligible (T' % 4 != 0).
+int conv1_wgrad_tc(const float* dz1, const float* x, float* xs, float* part, int B, int T, int Tp, float* dw1,
+                   cudaStream_t st) {
   if (Tp % 4 != 0) return 1;
   Wgrad1Params p{};
   const unsigned long long U = (unsigned long long)Tp + 4, F = DS2_NUM_FREQ;
-  DS2_LAUNCH(conv1_shift_copies_kernel, 148 * 8, 256, 0, st, B, T, Tp, x, xs);
+  DS2_LAUNCH(conv1_shift_copies_kernel, device_sm_count() * 8, 256, 0, st, B, T, Tp, x, xs);
   {
     unsigned long long dims[5] = {U, F, (unsigned long long)B, 2ull, 4ull};
     unsigned long long str[4] = {U * 4, F * U * 4, (unsigned long long)B * F * U * 4, 2ull * B * F * U * 4};
@@ -629,13 +631,14 @@ int conv1_wgrad_tc(const float* dz1, const float* x, float* xs, int B, int T, in
     int rc = make_tmap_4d_f32(&p.tmDz, dz1, dims, str, box);
     if (rc) return rc;
   }
-  p.B = B; p.Tp = Tp; p.dw1 = dw1;
+  p.B = B; p.Tp = Tp; p.part = part;
   static DeviceOnce attr_once;
   if (attr_once.first()) {
     DS2_CHECK_CUDA(cudaFuncSetAttribute(conv1_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, w1::SMEM_BYTES));
     attr_once.done();
   }
   DS2_LAUNCH(conv1_wgrad_tc_kernel, dim3(w1::CLASSES, 24), w1::THREADS, w1::SMEM_BYTES, st, p);
+  DS2_LAUNCH(conv1_wgrad_reduce_kernel, cdiv(32 * 41 * 11, 256), 256, 0, st, 24, part, dw1);
   return DS2_OK;
 }
 

@@ -1,6 +1,6 @@
 // fp32 -> fp16 operand copies for the precision-16 GEMMs (SURVEY.md §8f row N4; the reference trains with
 // `precision: 16`, configs/librispeech.yaml:12, i.e. autocast casts the GEMM operands to half and accumulates in fp32).
-// The tcgen05 fp16 GEMM takes K-major operands only, so operands whose reduction index is the row index in memory
+// The fp16 wgmma GEMM takes K-major operands only, so operands whose reduction index is the row index in memory
 // (dG^T, x^T, h^T for the weight gradients; W_ih^T for the data gradient) are transposed while they are converted.
 // Gradients are multiplied by a power of two first (a device-resident scale, like AMP's loss scale but per tensor and
 // exact to undo): fp16 has 5 exponent bits, the gate gradients of a T' = 500 recurrence span more.
@@ -116,7 +116,7 @@ int f32_to_f16_rows(int rows, int cols, const float* in, size_t ld_in, void* out
   DS2_REQUIRE(cols % 4 == 0 && ld_in % 4 == 0 && ld_out % 4 == 0, "f32_to_f16_rows: cols / pitches must be multiples of 4");
   const size_t total = (size_t)rows * (cols / 4);
   int blocks = (int)((total + 255) / 256);
-  blocks = blocks < 1 ? 1 : (blocks > 148 * 8 ? 148 * 8 : blocks);
+  blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
   DS2_LAUNCH(f32_to_f16_rows_kernel, blocks, 256, 0, st, rows, cols, in, ld_in, static_cast<__half*>(out), ld_out, scale_dev);
   return DS2_OK;
 }
@@ -136,7 +136,7 @@ int pow2_scale_for(int rows, int cols, const float* x, size_t ld, unsigned int* 
                    cudaStream_t st) {
   DS2_REQUIRE(cols % 4 == 0 && ld % 4 == 0, "pow2_scale_for: cols / pitch must be multiples of 4");
   DS2_CHECK_CUDA(cudaMemsetAsync(absmax_ws, 0, sizeof(unsigned int), st));
-  DS2_LAUNCH(absmax_strided_kernel, 148 * 4, 256, 0, st, rows, cols, x, ld, absmax_ws);
+  DS2_LAUNCH(absmax_strided_kernel, 132 * 4, 256, 0, st, rows, cols, x, ld, absmax_ws);
   DS2_LAUNCH(pow2_scale_kernel, 1, 1, 0, st, absmax_ws, scale, top);
   return DS2_OK;
 }

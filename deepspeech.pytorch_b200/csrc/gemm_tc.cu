@@ -1,13 +1,11 @@
-// tcgen05 TF32 GEMM:  C[M,N] = alpha * A[M,K] . B[N,K]^T + beta * C   (both operands K-major).
+// wgmma TF32 GEMM:  C[M,N] = alpha * A[M,K] . B[N,K]^T + beta * C   (both operands K-major).
 //
-//   warp 0      TMA producer: cp.async.bulk.tensor 2-D tiles (128B swizzle) of A (128 x 32 fp32) and
-//               B (256 x 32 fp32) into a 4-stage shared-memory ring, mbarrier complete_tx signalling
-//   warp 1      allocates 256 TMEM columns, then one elected lane issues tcgen05.mma.kind::tf32
-//               (M=128, N=256, K=8) x4 per stage, accumulating in TMEM; tcgen05.commit frees the stage
-//   warps 2..5  epilogue: tcgen05.ld (32 lanes x 32 columns per instruction) -> alpha/beta -> global
+//   warp 0       TMA producer: cp.async.bulk.tensor 2-D tiles (128B swizzle) of A (128 x 32 fp32) and
+//                B (128 x 32 fp32) into a 6-stage shared-memory ring, mbarrier complete_tx signalling
+//   warps 4..11  two MMA warpgroups: wgmma.mma_async m64n128k8 (tf32) x4 per stage on their 64-row half of
+//                the A tile, fp32 accumulators in registers; the epilogue stores them (alpha / beta) to global
 //
-// Operands that are not K-major in memory (transA / !transB) are read in place as MN-major tiles
-// (SWIZZLE_128B_BASE32B, see smem_desc_mn); unaligned ones are first transposed into the workspace.
+// Operands that are not K-major in memory (transA / !transB) are first transposed into the workspace.
 // Shapes the kernel does not take (tiny or unaligned) return 1 and the caller uses the FFMA GEMM.
 #include <stdio.h>
 #include <stdlib.h>
@@ -147,70 +145,31 @@ int make_tmap_f16(CUtensorMap* out, const void* base, int rank, int d0, int d1, 
 }
 
 // ---- kernel ---------------------------------------------------------------------------------------
-// NMB = number of 128-row M blocks per CTA.  With one block (tile 128 x 256) a K chunk moves 48 KB from L2 for
-// 512 tensor-pipe cycles = 94 B/cycle/SM, more than twice the ~42 B/cycle/SM the L2 can deliver to all SMs at
-// once: the kernel is L2-bandwidth bound at ~50 % of the TF32 peak (ncu: tensor pipe 54 % active).  With two
-// blocks (tile 256 x 256, two accumulators in the 512 TMEM columns, B tile shared) it is 64 KB per 1024 cycles.
+// 128 x 128 output tile per CTA; a 128-byte swizzle row holds 32 fp32 (or 64 fp16) of K, one stage = one row of K
+// for both operand tiles (32 KB), six stages in flight.
 namespace gtc {
-constexpr int BN = 256, BK = 32, THREADS = 192;
-// STG = pipeline stages.  (NMB 1, STG 2) fits two CTAs per SM (2 x 97 KB shared memory, 2 x 256 TMEM columns):
-// one CTA's epilogue then overlaps the other's main loop, which matters for short K (32 chunks at K = 1024).
-template <int NMB, int STG>
-struct Cfg {
-  static constexpr int BM = 128 * NMB;
-  static constexpr int A_BYTES = BM * BK * 4, B_BYTES = BN * BK * 4, STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = STG;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int TMEM_COLS = 256 * NMB;
-  static constexpr int CTAS_PER_SM = (NMB == 1 && STG == 2) ? 2 : 1;
-};
+constexpr int BM = 128, BN = 128, BK = 32, THREADS = 384, STAGES = 6;
+constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 }  // namespace gtc
-
-// MN-major operand tile (the matrix is stored (K, MN) row-major, i.e. "transposed" for this GEMM).  32-bit
-// MN-major operands have exactly one legal shared-memory layout on tcgen05, SWIZZLE_128B_BASE32B (descriptor
-// layout type 1; with the plain 128B swizzle the MMA returns zeros): rows of 32 mn elements (128 B), the
-// 32-byte chunk index of a row XOR-ed with (k & 3), repeating every 4 k-rows (512 B) — what the TMA unit
-// produces with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  The tile is ROWS/32 blocks of (32 mn x 32 k), 4 KB each;
-// leading byte offset = distance between consecutive 32-wide MN blocks (4096), stride byte offset = distance
-// between 4-row k groups (512); one MMA (K = 8) consumes two groups, so the k-step advance is 1024 B.  All blocks
-// of a tile come from ONE 3-D box (mn in block, k, block) when the MN extent is a multiple of 32 (the single
-// producer thread needs ~110 cycles per TMA instruction: 12 boxes per stage made it the bottleneck); otherwise
-// one 2-D box per block.  No transpose pass is needed.
-__device__ __forceinline__ uint64_t smem_desc_mn(uint32_t smem_addr, uint32_t layout, uint32_t lbo_bytes,
-                                                 uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo_bytes >> 4) << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout << 61;
-  return d;
-}
 
 // gridDim.z > 1: split-K, every CTA adds its partial tile into C with vector atomics (C holds beta * C_old,
 // prepared by the host).
-// F16 (both operands K-major fp16 in memory, precision-16 mode): the 128-byte swizzle rows hold 64 halfs instead of
-// 32 floats, so a stage covers twice the K extent with the same bytes, the same four 32-byte k-steps per stage and
-// tcgen05.mma.kind::f16 (K = 16) at twice the tensor rate; accumulation and C stay fp32.  `alpha_dev` (optional)
-// multiplies alpha by a device-resident factor (the inverse of the power-of-two scale of a scaled fp16 operand).
-template <bool A_MN, bool B_MN, int NMB, int STG, bool F16 = false>
-__global__ void __launch_bounds__(gtc::THREADS, gtc::Cfg<NMB, STG>::CTAS_PER_SM)
+// F16 (precision-16 mode): fp16 operands, the same 128-byte rows hold 64 halfs, wgmma k16 instead of tf32 k8;
+// accumulation and C stay fp32.  `alpha_dev` (optional) multiplies alpha by a device-resident factor (the inverse of
+// the power-of-two scale of a scaled fp16 operand).
+template <bool F16>
+__global__ void __launch_bounds__(gtc::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
-               float alpha, float beta, float* __restrict__ C, int ldc, unsigned int mn_cfg, int mn3d,
-               const float* __restrict__ alpha_dev) {
+               float alpha, float beta, float* __restrict__ C, int ldc, const float* __restrict__ alpha_dev) {
   using namespace gtc;
   using namespace tc;
-  using G = Cfg<NMB, STG>;
-  static_assert(!F16 || (!A_MN && !B_MN), "fp16 operands are K-major only");
   constexpr int BK = F16 ? 2 * gtc::BK : gtc::BK;         // K elements per stage (shadows gtc::BK)
   if (alpha_dev) alpha *= __ldg(alpha_dev);
-  constexpr int BM = G::BM, STAGES = G::STAGES, STAGE_BYTES = G::STAGE_BYTES, A_BYTES = G::A_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
   const int nk_all = (K + BK - 1) / BK, per = (nk_all + (int)gridDim.z - 1) / (int)gridDim.z;
@@ -220,17 +179,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(accum_bar, 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // two MMA warpgroups
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<G::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
+    // TMA producer
     if (lane == 0) {
       for (int it = 0; it < nk; ++it) {
         const int kb = kb0 + it, s = it % STAGES;
@@ -238,288 +193,69 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         mbar_wait(&empty[s], ph ^ 1);
         mbar_arrive_expect_tx(&full[s], STAGE_BYTES);
         uint8_t* sa = smem + s * STAGE_BYTES;
-        if (A_MN) {
-          if (mn3d & 1) {
-            tma_load_3d(sa, &tmA, &full[s], 0, kb * BK, m0 / 32);
-          } else {
-#pragma unroll
-            for (int i = 0; i < BM / 32; ++i) tma_load_2d(sa + i * 4096, &tmA, &full[s], m0 + i * 32, kb * BK);
-          }
-        } else {
-          tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
-        }
-        if (B_MN) {
-          if (mn3d & 2) {
-            tma_load_3d(sa + A_BYTES, &tmB, &full[s], 0, kb * BK, n0 / 32);
-          } else {
-#pragma unroll
-            for (int i = 0; i < BN / 32; ++i) tma_load_2d(sa + A_BYTES + i * 4096, &tmB, &full[s], n0 + i * 32, kb * BK);
-          }
-        } else {
-          tma_load_2d(sa + A_BYTES, &tmB, &full[s], kb * BK, n0);
-        }
+        tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
+        tma_load_2d(sa + A_BYTES, &tmB, &full[s], kb * BK, n0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = instr_desc(F16 ? FMT_F16 : FMT_TF32, 128, BN) | (A_MN ? (1u << 15) : 0u) | (B_MN ? (1u << 16) : 0u);
-      const uint32_t mn_layout = mn_cfg & 7u, lbo = ((mn_cfg >> 4) & 0x3FFFu) << 4, sbo = (mn_cfg >> 18) << 4;
-      for (int it = 0; it < nk; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES), b_addr = smem_u32(smem + s * STAGE_BYTES + A_BYTES);
-        const uint64_t adesc = A_MN ? smem_desc_mn(a_addr, mn_layout, lbo, sbo) : smem_desc_sw128(a_addr);
-        const uint64_t bdesc = B_MN ? smem_desc_mn(b_addr, mn_layout, lbo, sbo) : smem_desc_sw128(b_addr);
-        // k-step: K-major +32 B inside the 128B swizzle row; MN-major +1024 B (the next group of 8 k-rows)
-        constexpr uint64_t a_adv = A_MN ? 64 : 2, b_adv = B_MN ? 64 : 2;
+  } else if (warp >= 4) {
+    // two MMA warpgroups, 64 rows of the tile each; the accumulators stay in registers for the epilogue
+    const int wg = warp / 4 - 1;
+    float acc[64];
 #pragma unroll
-        for (int mb = 0; mb < NMB; ++mb) {
-          // M block mb: rows 128*mb.. of the A tile are 16 KB further in either layout; its accumulator 256 columns
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int it = 0; it < nk; ++it) {
+      const int s = it % STAGES;
+      mbar_wait(&full[s], (it / STAGES) & 1);
+      const uint64_t adesc = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES)) + (uint64_t)(512 * wg);
+      const uint64_t bdesc = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES));
+      wg_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {                  // four 32-byte k-steps per 128-byte row (K = 8 tf32 / 16 fp16)
-            if (F16)
-              mma_f16(tmem_base + (uint32_t)(mb * 256), adesc + (uint64_t)(mb * 1024) + (uint64_t)k * a_adv,
-                      bdesc + (uint64_t)k * b_adv, idesc, (it | k) != 0);
-            else
-              mma_tf32(tmem_base + (uint32_t)(mb * 256), adesc + (uint64_t)(mb * 1024) + (uint64_t)k * a_adv,
-                       bdesc + (uint64_t)k * b_adv, idesc, (it | k) != 0);
-          }
-        }
-        mma_commit(&empty[s]);             // stage reusable when these MMAs have read it
-      }
-      mma_commit(accum_bar);               // accumulator complete
+      for (int k = 0; k < 4; ++k)          // four 32-byte k-steps per 128-byte row (K = 8 tf32 / 16 fp16)
+        Wgmma<BN, F16>::mma(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+      wg_release(&empty[s]);
     }
-  } else if (nk > 0) {
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int q = warp % 4;                // TMEM lane quarter this warp may read
-    const bool vec_ok = ((ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
-#pragma unroll 1
-    for (int mb = 0; mb < NMB; ++mb) {
-      const int row = m0 + mb * 128 + q * 32 + lane;
-      if (m0 + mb * 128 >= M) break;       // warp-uniform
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= N) break;              // warp-uniform
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mb * 256 + c * 32), v);
-        if (vec_ok && col0 + 32 <= N) {
-          // A lane holds one accumulator row: storing from the registers would touch 32 rows x 16 bytes per
-          // instruction (the 524 MB projection output then runs at 1.6 TB/s and the tensor pipe idles 60 % of the
-          // kernel).  Turn the 32 x 32 block through shared memory — the pipeline stages are free once the accumulator
-          // barrier has completed — so that an instruction writes 4 rows x 128 contiguous bytes.
-          float* stg = reinterpret_cast<float*>(smem) + q * (32 * 36);
+    if (nk > 0) {
+      // fragment: rows 16 w + l/4 (+8), column pairs 8 i + 2 (l%4)
+      const int w = warp % 4;
+      const bool vec_ok = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(C) & 7) == 0);
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<float4*>(stg + lane * 36 + 4 * j) =
-                make_float4(alpha * v[4 * j], alpha * v[4 * j + 1], alpha * v[4 * j + 2], alpha * v[4 * j + 3]);
-          __syncwarp();
-          const int c4 = lane & 7;
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = m0 + 64 * wg + 16 * w + (lane >> 2) + 8 * hh;
+        if (row >= M) continue;
+        float* crow = C + (size_t)row * ldc;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = 4 * i + (lane >> 3), grow = m0 + mb * 128 + q * 32 + rr;
-            if (grow < M) {
-              float4 o = *reinterpret_cast<const float4*>(stg + rr * 36 + 4 * c4);
-              float* cp4 = C + (size_t)grow * ldc + col0 + 4 * c4;
-              if (split) {
-                atomicAdd(reinterpret_cast<float4*>(cp4), o);
-              } else {
-                if (beta != 0.f) {
-                  const float4 old = *reinterpret_cast<const float4*>(cp4);
-                  o.x = fmaf(beta, old.x, o.x); o.y = fmaf(beta, old.y, o.y);
-                  o.z = fmaf(beta, old.z, o.z); o.w = fmaf(beta, old.w, o.w);
-                }
-                *reinterpret_cast<float4*>(cp4) = o;
-              }
-            }
-          }
-          __syncwarp();
-        } else if (row < M) {
-          float* cp = C + (size_t)row * ldc + col0;
-          {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (col0 + j < N) {
-                float o = alpha * v[j];
-                if (split) {
-                  atomicAdd(cp + j, o);
-                } else {
-                  if (beta != 0.f) o = fmaf(beta, cp[j], o);
-                  cp[j] = o;
-                }
-              }
-          }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<G::TMEM_COLS>(tmem_base);
-}
-
-// ---- Not selected automatically (DS2_GEMM_CFG=4): correct on hardware (bit-identical results,
-// profiles/r01_gemm_pair_kernel.txt) but no faster than the single-CTA 256 x 256 tile — the limit is the
-// shared-memory bandwidth of each SM (TMA fill + MMA operand reads), not the L2 reads this variant halves.
-// Kept as the cluster / multicast plumbing for a cta_group::2 version.
-// 256 x 256 tiles in 2-CTA clusters along M that SHARE the B tile: each CTA loads its own A tile (32 KB per K
-// chunk) and one half of the B tile (16 KB), multicast into both CTAs' shared memory.  Per CTA that is 48 KB of
-// L2 reads per 1024 tensor-pipe cycles = 47 B/cycle/SM, just above what the L2 delivers to all SMs at once
-// (the 256 x 256 single-CTA tile needs 64, the 128 x 256 tile 94).  A stage may be refilled only when BOTH CTAs'
-// MMAs have read it (the peer's multicast writes into it too): the `empty` barriers count two arrivals, and every
-// tcgen05.commit is multicast to the pair.
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster "
-      "[%0], [%1, {%3, %4}], [%2], %5;" ::"r"(tc::smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(tc::smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                               int c2, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster "
-      "[%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(tc::smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(tc::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   tc::smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_gemm() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-
-template <bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(gtc::THREADS, 1)
-gemm_tc_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
-                    float alpha, float beta, float* __restrict__ C, int ldc, unsigned int mn_cfg, int mn3d) {
-  using namespace gtc;
-  using namespace tc;
-  using G = Cfg<2, 3>;
-  constexpr int BM = G::BM, STAGES = G::STAGES, STAGE_BYTES = G::STAGE_BYTES, A_BYTES = G::A_BYTES;
-  constexpr int BH = G::B_BYTES / 2;                      // half of the B tile: 128 rows / 4 MN blocks
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const int rank = (int)cluster_rank();                   // cluster = two consecutive blockIdx.y
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int nk = (K + BK - 1) / BK;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
-    mbar_init(accum_bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc<G::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  cluster_sync_gemm();                                    // the peer's barriers exist before anything is multicast
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      for (int it = 0; it < nk; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&empty[s], ph ^ 1);                     // both CTAs have released slot s
-        mbar_arrive_expect_tx(&full[s], STAGE_BYTES);     // own A + both halves of B
-        uint8_t* sa = smem + s * STAGE_BYTES;
-        if (A_MN) tma_load_3d(sa, &tmA, &full[s], 0, it * BK, m0 / 32);
-        else tma_load_2d(sa, &tmA, &full[s], it * BK, m0);
-        uint8_t* sb = sa + A_BYTES + rank * BH;           // this CTA's half, same offset in both CTAs
-        if (B_MN) tma_load_3d_mc(sb, &tmB, &full[s], 0, it * BK, n0 / 32 + rank * 4, (uint16_t)3);
-        else tma_load_2d_mc(sb, &tmB, &full[s], it * BK, n0 + rank * 128, (uint16_t)3);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = instr_desc(FMT_TF32, 128, BN) | (A_MN ? (1u << 15) : 0u) | (B_MN ? (1u << 16) : 0u);
-      const uint32_t mn_layout = mn_cfg & 7u, lbo = ((mn_cfg >> 4) & 0x3FFFu) << 4, sbo = (mn_cfg >> 18) << 4;
-      for (int it = 0; it < nk; ++it) {
-        const int s = it % STAGES;
-        const uint32_t ph = (it / STAGES) & 1;
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES), b_addr = smem_u32(smem + s * STAGE_BYTES + A_BYTES);
-        const uint64_t adesc = A_MN ? smem_desc_mn(a_addr, mn_layout, lbo, sbo) : smem_desc_sw128(a_addr);
-        const uint64_t bdesc = B_MN ? smem_desc_mn(b_addr, mn_layout, lbo, sbo) : smem_desc_sw128(b_addr);
-        constexpr uint64_t a_adv = A_MN ? 64 : 2, b_adv = B_MN ? 64 : 2;
-#pragma unroll
-        for (int mb = 0; mb < 2; ++mb) {
-#pragma unroll
-          for (int k = 0; k < BK / 8; ++k)
-            mma_tf32(tmem_base + (uint32_t)(mb * 256), adesc + (uint64_t)(mb * 1024) + (uint64_t)k * a_adv,
-                     bdesc + (uint64_t)k * b_adv, idesc, (it | k) != 0);
-        }
-        mma_commit_mc(&empty[s], (uint16_t)3);            // slot s of THIS CTA is free: tell both producers
-      }
-      mma_commit(accum_bar);
-    }
-  } else if (nk > 0) {
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int q = warp % 4;
-    const bool vec_ok = ((ldc & 3) == 0) && ((reinterpret_cast<uintptr_t>(C) & 15) == 0);
-#pragma unroll 1
-    for (int mb = 0; mb < 2; ++mb) {
-      const int row = m0 + mb * 128 + q * 32 + lane;
-      if (m0 + mb * 128 >= M) break;
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int col0 = n0 + c * 32;
-        if (col0 >= N) break;
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(mb * 256 + c * 32), v);
-        if (row < M) {
-          float* cp = C + (size_t)row * ldc + col0;
-          if (vec_ok && col0 + 32 <= N) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 o = make_float4(alpha * v[4 * j], alpha * v[4 * j + 1], alpha * v[4 * j + 2], alpha * v[4 * j + 3]);
+        for (int i = 0; i < BN / 8; ++i) {
+          const int col = n0 + 8 * i + 2 * (lane & 3);
+          float2 o = make_float2(alpha * acc[4 * i + 2 * hh], alpha * acc[4 * i + 2 * hh + 1]);
+          if (vec_ok && col + 1 < N) {
+            float2* cp2 = reinterpret_cast<float2*>(crow + col);
+            if (split) {
+              atomicAdd(cp2, o);
+            } else {
               if (beta != 0.f) {
-                float4 old = *reinterpret_cast<const float4*>(cp + 4 * j);
-                o.x = fmaf(beta, old.x, o.x); o.y = fmaf(beta, old.y, o.y);
-                o.z = fmaf(beta, old.z, o.z); o.w = fmaf(beta, old.w, o.w);
+                const float2 old = *cp2;
+                o.x = fmaf(beta, old.x, o.x);
+                o.y = fmaf(beta, old.y, o.y);
               }
-              *reinterpret_cast<float4*>(cp + 4 * j) = o;
+              *cp2 = o;
             }
           } else {
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (col0 + j < N) {
-                float o = alpha * v[j];
-                if (beta != 0.f) o = fmaf(beta, cp[j], o);
-                cp[j] = o;
+            for (int j = 0; j < 2; ++j) {
+              if (col + j >= N) break;
+              float v = j ? o.y : o.x;
+              if (split) {
+                atomicAdd(crow + col + j, v);
+              } else {
+                if (beta != 0.f) v = fmaf(beta, crow[col + j], v);
+                crow[col + j] = v;
               }
+            }
           }
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_gemm();                                    // the peer may still multicast / arrive until it is done too
-  if (warp == 1) tmem_dealloc<G::TMEM_COLS>(tmem_base);
 }
 
 // out (C x R, pitch ldo) = in (R x C, pitch ldi)^T
@@ -545,19 +281,6 @@ int transpose(int R, int C, const float* in, float* out, cudaStream_t st) {
 
 static inline size_t k4(int K) { return (size_t)((K + 3) / 4 * 4); }
 
-// MN-major operands are read in place (no transpose pass); DS2_GEMM_MN_MAJOR=0 restores the transposes;
-// DS2_GEMM_MN_CFG="tma_swizzle,layout,lbo,sbo" overrides the tile layout parameters (bring-up only).
-struct MnCfg { int on, sw, layout, lbo, sbo; };
-static MnCfg mn_cfg_from_env() {
-  MnCfg c{1, (int)CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, 1, 4096, 512};
-  const char* e = getenv("DS2_GEMM_MN_MAJOR");
-  if (e) c.on = atoi(e);
-  const char* f = getenv("DS2_GEMM_MN_CFG");
-  if (f) sscanf(f, "%d,%d,%d,%d", &c.sw, &c.layout, &c.lbo, &c.sbo);
-  return c;
-}
-static bool use_mn_major() { return mn_cfg_from_env().on != 0; }
-
 size_t gemm_tc_workspace_bytes(int transA, int transB, int M, int N, int K) {
   size_t n = 0;
   if (transA) n += align_up((size_t)M * k4(K) * 4, 256);
@@ -567,139 +290,66 @@ size_t gemm_tc_workspace_bytes(int transA, int transB, int M, int N, int K) {
 
 static bool tc_eligible(int M, int N, int K) { return K >= 32 && M >= 32 && N >= 16 && (long long)M * N * K >= (1 << 18); }
 
-template <bool A_MN, bool B_MN, int NMB, int STG, bool F16 = false>
+// K-way split (DS2_GEMM_CFG / DS2_GEMM16_CFG = 2, 3: 2 or 4 parts, added into C with float atomics).  Never chosen
+// by itself: the order of the atomic adds varies from run to run, and the training step must be bit-repeatable.
+static int choose_splits(const char* env, float beta) {
+  const char* e = getenv(env);
+  const int forced = e ? atoi(e) : 0;
+  if (forced >= 2 && forced <= 3 && (beta == 0.f || beta == 1.f)) return 1 << (forced - 1);
+  return 1;
+}
+
+template <bool F16>
 static int launch_gemm_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, float alpha, float beta,
-                          float* C, int ldc, int mn3d, int splits, cudaStream_t st, const float* alpha_dev = nullptr) {
-  using G = gtc::Cfg<NMB, STG>;
-  auto kern = gemm_tc_kernel<A_MN, B_MN, NMB, STG, F16>;
+                          float* C, int ldc, int splits, cudaStream_t st, const float* alpha_dev = nullptr) {
+  auto kern = gemm_tc_kernel<F16>;
   static DeviceOnce attr_once;
   if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM_BYTES));
+    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, gtc::SMEM_BYTES));
     attr_once.done();
   }
-  const MnCfg mc = mn_cfg_from_env();
-  const unsigned int mn_cfg = (unsigned)(mc.layout & 7) | ((unsigned)(mc.lbo >> 4) << 4) | ((unsigned)(mc.sbo >> 4) << 18);
   if (splits > 1 && beta == 0.f)
     DS2_CHECK_CUDA(cudaMemset2DAsync(C, (size_t)ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, st));
-  dim3 grid(cdiv(N, gtc::BN), cdiv(M, G::BM), splits);
-  DS2_LAUNCH(kern, grid, gtc::THREADS, G::SMEM_BYTES, st, tmA, tmB, M, N, K, alpha, beta, C, ldc, mn_cfg, mn3d, alpha_dev);
+  dim3 grid(cdiv(N, gtc::BN), cdiv(M, gtc::BM), splits);
+  DS2_LAUNCH(kern, grid, gtc::THREADS, gtc::SMEM_BYTES, st, tmA, tmB, M, N, K, alpha, beta, C, ldc, alpha_dev);
   return DS2_OK;
 }
 
-template <bool A_MN, bool B_MN>
-static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, float alpha, float beta,
-                            float* C, int ldc, int mn3d, cudaStream_t st) {
-  using G = gtc::Cfg<2, 3>;
-  auto kern = gemm_tc_pair_kernel<A_MN, B_MN>;
-  static DeviceOnce attr_once;
-  if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM_BYTES));
-    attr_once.done();
-  }
-  const MnCfg mc = mn_cfg_from_env();
-  const unsigned int mn_cfg = (unsigned)(mc.layout & 7) | ((unsigned)(mc.lbo >> 4) << 4) | ((unsigned)(mc.sbo >> 4) << 18);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(cdiv(N, gtc::BN), (cdiv(M, G::BM) + 1) / 2 * 2);    // whole pairs; surplus rows are masked
-  cfg.blockDim = dim3(gtc::THREADS);
-  cfg.dynamicSmemBytes = G::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeClusterDimension;
-  attr.val.clusterDim.x = 1; attr.val.clusterDim.y = 2; attr.val.clusterDim.z = 1;
-  cfg.attrs = &attr;
-  cfg.numAttrs = 1;
-  DS2_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, M, N, K, alpha, beta, C, ldc, mn_cfg, mn3d));
-  g_launches.fetch_add(1, std::memory_order_relaxed);
-  return DS2_OK;
-}
-
+// TF32 wgmma reads both operands K-major: an operand stored the other way round (transA / !transB) is first
+// transposed into the workspace.
 int gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const float* A, int lda, const float* B,
             int ldb, float beta, float* C, int ldc, void* ws, size_t ws_bytes, cudaStream_t st) {
   if (!tc_eligible(M, N, K)) return 1;
   Arena ar(ws, ws_bytes);
   const float* Ak = A;
   int ldak = lda;
-  bool a_mn = false, b_mn = false;
   if (transA) {  // stored (K, M)
-    if (use_mn_major() && (lda & 3) == 0 && (reinterpret_cast<uintptr_t>(A) & 15) == 0) {
-      a_mn = true;
-    } else {
-      float* t = ar.take<float>((size_t)M * k4(K));
-      if (!t) return 1;
-      int rc = transpose_strided(K, M, A, (size_t)lda, t, k4(K), st);
-      if (rc) return rc;
-      Ak = t;
-      ldak = (int)k4(K);
-    }
+    float* t = ar.take<float>((size_t)M * k4(K));
+    if (!t) return 1;
+    int rc = transpose_strided(K, M, A, (size_t)lda, t, k4(K), st);
+    if (rc) return rc;
+    Ak = t;
+    ldak = (int)k4(K);
   }
   const float* Bk = B;
   int ldbk = ldb;
   if (!transB) {  // stored (K, N)
-    if (use_mn_major() && (ldb & 3) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0) {
-      b_mn = true;
-    } else {
-      float* t = ar.take<float>((size_t)N * k4(K));
-      if (!t) return 1;
-      int rc = transpose_strided(K, N, B, (size_t)ldb, t, k4(K), st);
-      if (rc) return rc;
-      Bk = t;
-      ldbk = (int)k4(K);
-    }
+    float* t = ar.take<float>((size_t)N * k4(K));
+    if (!t) return 1;
+    int rc = transpose_strided(K, N, B, (size_t)ldb, t, k4(K), st);
+    if (rc) return rc;
+    Bk = t;
+    ldbk = (int)k4(K);
   }
   if ((ldak & 3) || (ldbk & 3) || (reinterpret_cast<uintptr_t>(Ak) & 15) || (reinterpret_cast<uintptr_t>(Bk) & 15))
     return 1;
-  // tile configuration (DS2_GEMM_CFG: 0 auto, 1 = 128x256 / 4 stages, 2 = 256x256 / 3 stages, 3 = 128x256 / 2 stages
-  // with two CTAs per SM): 256 x 256 when that still fills the machine, if necessary with a 2-way split of K
-  int cfg = 1, splits = 1;
-  {
-    const char* e = getenv("DS2_GEMM_CFG");
-    const int forced = e ? atoi(e) : 0;
-    const long long tiles2 = (long long)cdiv(M, 256) * cdiv(N, gtc::BN);
-    if (forced >= 1 && forced <= 4) {
-      cfg = (forced == 2 && M < 256) ? 1 : forced;
-      // 4 (experimental CTA-pair kernel): MN-major operands only through 3-D boxes, no split-K
-      if (cfg == 4 && (M < 256 || (a_mn && M % 32 != 0) || (b_mn && N % 32 != 0))) cfg = 1;
-    } else if (M >= 256) {
-      if (tiles2 >= 90) cfg = 2;      // (96 tiles: the 4096 x 1312 first-layer weight gradient, one wave)
-      else if (tiles2 * 2 >= 100 && tiles2 * 2 <= 148 && K >= 2048 && (beta == 0.f || beta == 1.f)) { cfg = 2; splits = 2; }
-    }
-  }
-  const int bm = (cfg == 2 || cfg == 4) ? 256 : 128;
-  const int bn_box = cfg == 4 ? gtc::BN / 2 : gtc::BN;      // pair kernel: each CTA loads half of the B tile
+  const int splits = choose_splits("DS2_GEMM_CFG", beta);
   CUtensorMap tmA, tmB;
-  // K-major: matrix [rows, K] box (32 k, rows).  MN-major: matrix [K, rows]: one 3-D box (32 rows, 32 k, blocks)
-  // when rows % 32 == 0, else 2-D boxes (32 rows, 32 k)
-  const CUtensorMapSwizzle mn_sw = (CUtensorMapSwizzle)mn_cfg_from_env().sw;
-  int mn3d = 0, rc;
-  if (a_mn && M % 32 == 0) {
-    mn3d |= 1;
-    rc = make_tmap_3d_sw(&tmA, Ak, 32, K, M / 32, (size_t)ldak, 32, 32, 32, bm / 32, mn_sw);
-  } else {
-    rc = a_mn ? make_tmap_2d_sw(&tmA, Ak, K, M, ldak, 32, 32, mn_sw) : make_tmap_2d(&tmA, Ak, M, K, ldak, bm, gtc::BK);
-  }
+  int rc = make_tmap_2d(&tmA, Ak, M, K, ldak, gtc::BM, gtc::BK);
   if (rc) return rc;
-  if (b_mn && N % 32 == 0) {
-    mn3d |= 2;
-    rc = make_tmap_3d_sw(&tmB, Bk, 32, K, N / 32, (size_t)ldbk, 32, 32, 32, bn_box / 32, mn_sw);
-  } else {
-    rc = b_mn ? make_tmap_2d_sw(&tmB, Bk, K, N, ldbk, 32, 32, mn_sw) : make_tmap_2d(&tmB, Bk, N, K, ldbk, bn_box, gtc::BK);
-  }
+  rc = make_tmap_2d(&tmB, Bk, N, K, ldbk, gtc::BN, gtc::BK);
   if (rc) return rc;
-  if (cfg == 4) {
-    if (a_mn && b_mn) return launch_gemm_pair<true, true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, mn3d, st);
-    if (a_mn) return launch_gemm_pair<true, false>(tmA, tmB, M, N, K, alpha, beta, C, ldc, mn3d, st);
-    if (b_mn) return launch_gemm_pair<false, true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, mn3d, st);
-    return launch_gemm_pair<false, false>(tmA, tmB, M, N, K, alpha, beta, C, ldc, mn3d, st);
-  }
-#define DS2_GEMM_DISPATCH(AM, BMN)                                                                                   \
-  return cfg == 2   ? launch_gemm_tc<AM, BMN, 2, 3>(tmA, tmB, M, N, K, alpha, beta, C, ldc, mn3d, splits, st)        \
-         : cfg == 3 ? launch_gemm_tc<AM, BMN, 1, 2>(tmA, tmB, M, N, K, alpha, beta, C, ldc, mn3d, splits, st)        \
-                    : launch_gemm_tc<AM, BMN, 1, 4>(tmA, tmB, M, N, K, alpha, beta, C, ldc, mn3d, splits, st)
-  if (a_mn && b_mn) { DS2_GEMM_DISPATCH(true, true); }
-  if (a_mn) { DS2_GEMM_DISPATCH(true, false); }
-  if (b_mn) { DS2_GEMM_DISPATCH(false, true); }
-  DS2_GEMM_DISPATCH(false, false);
-#undef DS2_GEMM_DISPATCH
+  return launch_gemm_tc<false>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st);
 }
 
 // C[M,N] (fp32) = alpha * [*alpha_dev] * A[M,K] . B[N,K]^T + beta * C with fp16 K-major operands (precision-16 mode).
@@ -708,30 +358,13 @@ int gemm_tc_f16(int M, int N, int K, float alpha, const void* A16, int lda, cons
                 float* C, int ldc, const float* alpha_dev, cudaStream_t st) {
   if (!tc_eligible(M, N, K) || M < 128) return 1;
   if ((lda & 7) || (ldb & 7) || (reinterpret_cast<uintptr_t>(A16) & 15) || (reinterpret_cast<uintptr_t>(B16) & 15)) return 1;
-  int cfg = 1, splits = 1;
-  const long long tiles2 = (long long)cdiv(M, 256) * cdiv(N, gtc::BN);
-  if (M >= 256) {
-    if (tiles2 >= 90) cfg = 2;
-    else if (tiles2 * 2 >= 100 && tiles2 * 2 <= 148 && K >= 4096 && (beta == 0.f || beta == 1.f)) { cfg = 2; splits = 2; }
-  }
-  // short K, large output (the input projection: K = 1024, 524 MB of fp32 C): the main loop of a 256 x 256 tile is 16
-  // stages, shorter than its epilogue — 128 x 256 tiles with TWO CTAs per SM let one CTA's epilogue overlap the other's
-  // main loop (DS2_GEMM16_CFG forces 1 / 2 / 3)
-  if (cfg == 2 && splits == 1 && K <= 2048 && tiles2 >= 4 * 148) cfg = 3;
-  {
-    const char* e = getenv("DS2_GEMM16_CFG");
-    const int forced = e ? atoi(e) : 0;
-    if (forced >= 1 && forced <= 3 && !(forced == 2 && M < 256)) { cfg = forced; if (forced != 2) splits = 1; }
-  }
-  const int bm = cfg == 2 ? 256 : 128;
+  const int splits = choose_splits("DS2_GEMM16_CFG", beta);
   CUtensorMap tmA, tmB;
-  int rc = make_tmap_f16(&tmA, A16, 2, K, M, 1, (size_t)lda, 0, 64, bm, 1);
+  int rc = make_tmap_f16(&tmA, A16, 2, K, M, 1, (size_t)lda, 0, 64, gtc::BM, 1);
   if (rc) return rc;
   rc = make_tmap_f16(&tmB, B16, 2, K, N, 1, (size_t)ldb, 0, 64, gtc::BN, 1);
   if (rc) return rc;
-  if (cfg == 2) return launch_gemm_tc<false, false, 2, 3, true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, 0, splits, st, alpha_dev);
-  if (cfg == 3) return launch_gemm_tc<false, false, 1, 2, true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, 0, splits, st, alpha_dev);
-  return launch_gemm_tc<false, false, 1, 4, true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, 0, splits, st, alpha_dev);
+  return launch_gemm_tc<true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st, alpha_dev);
 }
 
 }  // namespace ds2

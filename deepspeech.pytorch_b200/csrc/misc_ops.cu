@@ -117,25 +117,50 @@ __global__ void greedy_decode_kernel(int B, int T, int C, const float* __restric
 }
 
 // ------------------------------------------------------------------ optimizer (model.py:273-297 + clip 400)
-__global__ void sumsq_kernel(int64_t n, const float* __restrict__ g, double* __restrict__ out) {
-  __shared__ double red[32];
+// Squared gradient norm, bit-repeatable: a fixed grid of NORM_PARTS blocks (every block's share of the vector and its
+// summation order depend on n only) writes one double partial each to ws[1 + block]; sumsq_final_kernel adds them in
+// order into ws[0].  (The 256-byte optimizer workspace holds the 31 partials.)
+constexpr int NORM_PARTS = 31, NORM_THREADS = 1024;
+__global__ void __launch_bounds__(NORM_THREADS) sumsq_kernel(int64_t n, const float* __restrict__ g,
+                                                             double* __restrict__ ws) {
+  __shared__ double red[NORM_THREADS / 32];
   double acc = 0.0;
-  float part = 0.f;
-  int cnt = 0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-    float v = g[i];
-    part = fmaf(v, v, part);
-    if (++cnt == 32) { acc += part; part = 0.f; cnt = 0; }
+  const int64_t stride = (int64_t)NORM_PARTS * NORM_THREADS, tid = (int64_t)blockIdx.x * NORM_THREADS + threadIdx.x;
+  const bool vec = (reinterpret_cast<uintptr_t>(g) & 15) == 0;
+  const int64_t n4 = vec ? n / 4 : 0;
+  const float4* g4 = reinterpret_cast<const float4*>(g);
+  int64_t i = tid;
+  for (; i + 3 * stride < n4; i += 4 * stride) {      // four independent 16-byte loads in flight per thread
+    const float4 a = g4[i], b = g4[i + stride], c = g4[i + 2 * stride], d = g4[i + 3 * stride];
+    float part = a.x * a.x;
+    part = fmaf(a.y, a.y, part); part = fmaf(a.z, a.z, part); part = fmaf(a.w, a.w, part);
+    part = fmaf(b.x, b.x, part); part = fmaf(b.y, b.y, part); part = fmaf(b.z, b.z, part); part = fmaf(b.w, b.w, part);
+    part = fmaf(c.x, c.x, part); part = fmaf(c.y, c.y, part); part = fmaf(c.z, c.z, part); part = fmaf(c.w, c.w, part);
+    part = fmaf(d.x, d.x, part); part = fmaf(d.y, d.y, part); part = fmaf(d.z, d.z, part); part = fmaf(d.w, d.w, part);
+    acc += part;
   }
-  acc += part;
+  for (; i < n4; i += stride) {
+    const float4 a = g4[i];
+    acc += (double)fmaf(a.w, a.w, fmaf(a.z, a.z, fmaf(a.y, a.y, a.x * a.x)));
+  }
+  for (int64_t j = 4 * n4 + tid; j < n; j += stride) acc += (double)g[j] * g[j];
   acc = warp_sum_d(acc);
   if (threadIdx.x % 32 == 0) red[threadIdx.x / 32] = acc;
   __syncthreads();
   if (threadIdx.x < 32) {
-    double v = threadIdx.x < blockDim.x / 32 ? red[threadIdx.x] : 0.0;
-    v = warp_sum_d(v);
-    if (threadIdx.x == 0) atomicAdd(out, v);
+    double v = warp_sum_d(red[threadIdx.x]);
+    if (threadIdx.x == 0) ws[1 + blockIdx.x] = v;
   }
+}
+__global__ void sumsq_final_kernel(double* __restrict__ ws) {
+  double s = 0.0;
+  for (int i = 0; i < NORM_PARTS; ++i) s += ws[1 + i];
+  ws[0] = s;
+}
+static int launch_sumsq(int64_t n, const float* g, double* ws, cudaStream_t st) {
+  DS2_LAUNCH(sumsq_kernel, NORM_PARTS, NORM_THREADS, 0, st, n, g, ws);
+  DS2_LAUNCH(sumsq_final_kernel, 1, 1, 0, st, ws);
+  return DS2_OK;
 }
 
 __device__ __forceinline__ float clip_coef(const double* sumsq, float grad_scale, float max_norm, float* norm_out) {
@@ -262,7 +287,7 @@ int ds2_fc_head_bwd(int rows, int H, int C, const float* g, const float* b, cons
   size_t gws_bytes = ar.cap - ar.off;
   size_t total = (size_t)rows * H;
   int blocks = (int)((total + 1023) / 1024);
-  blocks = blocks > 148 * 16 ? 148 * 16 : blocks;
+  blocks = blocks > 132 * 16 ? 132 * 16 : blocks;
   // dW = dlogits^T (C x rows) . xbn (rows x H)
   DS2_LAUNCH(affine_rows_kernel, blocks, 256, 0, st, total, H, xhat, g, b, tmp);
   int r = ds2_gemm(1, 0, C, H, rows, 1.f, dlogits, C, tmp, H, 0.f, dw, H, gws, gws_bytes, stream);
@@ -284,7 +309,7 @@ int ds2_greedy_decode(int B, int T, int C, const float* probs, const int32_t* ou
   return DS2_OK;
 }
 
-size_t ds2_optim_workspace_bytes(void) { return 256; }
+size_t ds2_optim_workspace_bytes(void) { return (1 + NORM_PARTS) * sizeof(double); }   // 256
 
 int ds2_adamw_step(int64_t n, float* p, const float* g, float* m, float* v, float lr, float beta1, float beta2,
                    float eps, float wd, int step, float grad_scale, float max_norm, float* grad_norm_out,
@@ -293,10 +318,10 @@ int ds2_adamw_step(int64_t n, float* p, const float* g, float* m, float* v, floa
   cudaStream_t st = as_stream(stream);
   double* sumsq = static_cast<double*>(norm_ws);
   DS2_PROF("optim", st);
-  DS2_CHECK_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(double), st));
   int blocks = (int)((n + 4095) / 4096);
-  blocks = blocks < 1 ? 1 : (blocks > 148 * 8 ? 148 * 8 : blocks);
-  DS2_LAUNCH(sumsq_kernel, blocks, 256, 0, st, n, g, sumsq);
+  blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
+  int rc = launch_sumsq(n, g, sumsq, st);
+  if (rc) return rc;
   float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
   const int vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                     reinterpret_cast<uintptr_t>(v)) & 15) == 0;
@@ -311,10 +336,10 @@ int ds2_sgd_nesterov_step(int64_t n, float* p, const float* g, float* buf, float
   DS2_REQUIRE(n >= 0 && norm_ws, "ds2_sgd_nesterov_step: bad arguments");
   cudaStream_t st = as_stream(stream);
   double* sumsq = static_cast<double*>(norm_ws);
-  DS2_CHECK_CUDA(cudaMemsetAsync(sumsq, 0, sizeof(double), st));
   int blocks = (int)((n + 4095) / 4096);
-  blocks = blocks < 1 ? 1 : (blocks > 148 * 8 ? 148 * 8 : blocks);
-  DS2_LAUNCH(sumsq_kernel, blocks, 256, 0, st, n, g, sumsq);
+  blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
+  int rc = launch_sumsq(n, g, sumsq, st);
+  if (rc) return rc;
   DS2_LAUNCH(sgd_nesterov_kernel, blocks, 256, 0, st, n, p, g, buf, lr, momentum, wd, first_step, grad_scale,
              max_norm, sumsq, grad_norm_out);
   return DS2_OK;

@@ -1,4 +1,4 @@
-// Gate math shared by every recurrent kernel (FFMA step kernels and the tcgen05 persistent kernel).
+// Gate math shared by every recurrent kernel (FFMA step kernels and the wgmma persistent kernels).
 // PyTorch conventions (SURVEY.md Appendix B): LSTM rows [i,f,g,o]; GRU rows [r,z,n] with
 // n = tanh(x_n + r * (W_hn h + b_hn)); tanh-RNN single gate.
 #pragma once

@@ -4,7 +4,7 @@
 // gate activations, then three dense GEMMs (dW_ih, dW_hh, dX) and the BatchNorm backward.
 //
 // This file holds the host orchestration and the generic FFMA step kernels (any H, any B): one
-// launch per time step covering both directions.  rnn_persistent_tc.cu provides the tcgen05
+// launch per time step covering both directions.  rnn_persistent_tc.cu provides the wgmma
 // persistent sweep that replaces the step launches when the shape is eligible.
 //
 // reserve layout (floats):  gates (T,B,D,G*H) | hseq (D,T,B,H) | aux (D,T,B,H: LSTM cell states /
@@ -280,7 +280,7 @@ static int fill_w_hh_cb(void* ctx, void* stream) {
   return DS2_OK;
 }
 
-// tcgen05 persistent sweeps (rnn_persistent_tc.cu).  Return 1 when the shape is not eligible.
+// wgmma persistent sweeps (rnn_persistent_tc.cu).  Return 1 when the shape is not eligible.
 int rnn_sweep_fwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st);
 int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D);
@@ -432,7 +432,7 @@ int ds2_rnn_layer_fwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
   }
   size_t n = (size_t)TB * H;
   int blocks = (int)((n + 1023) / 1024);
-  blocks = blocks > 148 * 16 ? 148 * 16 : blocks;
+  blocks = blocks > 132 * 16 ? 132 * 16 : blocks;
   DS2_LAUNCH(sum_dirs_kernel, blocks, 256, 0, st, n, D, R.hseq, y);
   if (hn) DS2_LAUNCH(final_state_kernel, cdiv((long long)D * B * H, 256), 256, 0, st, T, B, H, D, len, R.hseq, h0, hn);
   if (cn && d->rnn_type == DS2_RNN_LSTM)

@@ -1,14 +1,14 @@
-// Persistent, warp-specialised recurrent sweeps on tcgen05 (SURVEY.md §7 step 4b).
+// Persistent, warp-specialised recurrent sweeps on wgmma tensor cores.
 //
 // One launch per layer covers ALL time steps and both directions.  A CTA owns 16 hidden units of
 // one direction: the G*16 rows of W_hh for those units form the M=64 operand of
-//     acc[(g,u), b] = sum_k W_hh[g*H+u, k] * h_{t-1}[b, k]        (tcgen05.mma kind::tf32, N = batch)
-// with fp32 accumulators in TMEM.  Per step:
+//     acc[(g,u), b] = sum_k W_hh[g*H+u, k] * h_{t-1}[b, k]        (wgmma, tf32 or f16, N = batch)
+// with fp32 accumulators.  Per step:
 //   warp 0   TMA producer: weight chunks (3-D box over [gate][unit][k], prefetched ahead of the
 //            barrier because they do not depend on it) and h_{t-1} chunks (after the grid barrier)
 //            into an 8-stage 128B-swizzled shared-memory ring
-//   warp 1   single-thread MMA issue, tcgen05.commit -> mbarriers
-//   warps 2-5 epilogue: TMEM -> registers, + input projection + biases, gate non-linearities spread
+//   warps 8-11 MMA warpgroup: wgmma into registers, then the accumulator image in shared memory -> mbarrier
+//   warps 2-5 epilogue: accumulator image -> registers, + input projection + biases, gate non-linearities spread
 //            over 64 lanes, exchange through shared memory, cell update (c / h state stays in shared
 //            memory for the whole sweep), masked stores of h_t (and the saved tensors for backward)
 // Steps are separated by a per-direction grid barrier (monotonic counter in global memory, release /
@@ -36,7 +36,7 @@ constexpr int UT = 16;        // hidden units per CTA
 constexpr int MM = 64;        // MMA M (G*UT rows, padded for GRU / tanh)
 constexpr int BK = 32;        // fp32 elements per 128-byte swizzle row
 constexpr int STAGES = 8;
-constexpr int THREADS = 192;  // producer, mma, 4 epilogue warps
+constexpr int THREADS = 288;  // warps 0..3 epilogue, warps 4..7 MMA warpgroup, warp 8 producer
 constexpr int A_BYTES = MM * 128;
 constexpr long long SPIN_LIMIT = 4000000000LL;   // ~2 s of SM clocks
 }  // namespace rp
@@ -66,7 +66,7 @@ struct PersistParams {
   const float* b_ih[2];
   const float* b_hh[2];
   unsigned int* bar;    // [2][NT] per-CTA step flags (zeroed by the host): flag = number of finished steps
-  int nacc, acc_cols;   // independent TMEM accumulator chains (K is dealt round-robin over them)
+  int nacc, acc_cols;   // independent accumulator chains (K is dealt round-robin over them)
   int defer;            // 1: stores that only later kernels read are issued after the barrier arrival
   int d0;               // first direction handled by this launch (directions can be launched one at a time
                         // when both together would not be co-resident, e.g. H = 1536)
@@ -89,6 +89,8 @@ __device__ __forceinline__ void red_release(unsigned int* p, unsigned int v) {
 // gpu-scope ordering comes from the release / acquire pair on the barrier counter, which is needed anyway.
 __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
+// The waits below only set *err on a timeout (sweep_check_kernel reports it after the launch): a device printf is
+// a function call, and a call anywhere in a kernel makes ptxas serialise every wgmma of that kernel.
 // Grid barrier of one direction: every CTA publishes the number of steps it has finished in its own
 // 4-byte flag (plain release store, no atomic serialisation); a whole warp polls all NT flags
 // (coalesced acquire loads) until each is >= target.  Bounded spin: a fault cannot hang the GPU.
@@ -114,7 +116,6 @@ __device__ __forceinline__ void grid_wait_flags(const unsigned int* flags, int n
       if (*(volatile int*)err) return;
       if (clock64() - t0 > rp::SPIN_LIMIT) {
         *(volatile int*)err = 1;
-        if (lane == 0) printf("ds2: recurrent sweep barrier timeout (block %d, target %u)\n", blockIdx.x, target);
         return;
       }
     }
@@ -132,8 +133,6 @@ __device__ __forceinline__ void grid_wait_counter(const unsigned int* ctr, unsig
         if (*(volatile int*)err) break;
         if (clock64() - t0 > rp::SPIN_LIMIT) {
           *(volatile int*)err = 1;
-          printf("ds2: recurrent sweep barrier timeout (block %d, target %u, have %u)\n", blockIdx.x, target,
-                 ld_relaxed(ctr));
           break;
         }
       }
@@ -208,7 +207,6 @@ __device__ __forceinline__ void ll_wait(uint4& v, const void* src, int* err) {
       if (*(volatile int*)err) return;
       if (clock64() - t0 > rp::SPIN_LIMIT) {
         *(volatile int*)err = 1;
-        printf("ds2: recurrent sweep data-flag timeout (block %d)\n", blockIdx.x);
         return;
       }
     }
@@ -242,7 +240,7 @@ __device__ __forceinline__ unsigned int ll_wait_u32(const unsigned int* src, int
 // (G*16 rows x H, 128 KB at H=1024) stays in shared memory for the whole sweep; per step only the
 // fp16 copy of h_{t-1} (B x H, 64 KB) is streamed by TMA, and the MMAs are kind::f16 (K=16, half the
 // instruction count).  fp16 has the same 10-bit mantissa as TF32 and |h| < 1, |w| << 65504, so this
-// is the same arithmetic class as the TF32 path (fp32 accumulation in TMEM either way).
+// is the same arithmetic class as the TF32 path (fp32 accumulation either way).
 template <int RNN, bool RES>
 __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const __grid_constant__ PersistParams p) {
   using namespace rp;
@@ -263,7 +261,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
   uint64_t* full = reinterpret_cast<uint64_t*>(lens_s + ((NB + 1) & ~1));   // resident: one per h chunk (<= 32)
   uint64_t* empty = full + (RES ? 32 : STAGES);                             // resident: [0] = weights landed
   uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
+  float* acc_img = reinterpret_cast<float*>(accum_bar + 1);   // accumulator image (tc::wg_store_acc)
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int d = p.d0 + blockIdx.x / p.NT, tile = blockIdx.x % p.NT, u0 = tile * UT;
@@ -275,29 +273,16 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
     tma_prefetch_desc(&p.tmW[d]);
     tma_prefetch_desc(&p.tmV[d]);
     for (int i = 0; i < (RES ? 32 : STAGES); ++i) mbar_init(&full[i], 1);
-    for (int i = 0; i < STAGES; ++i) mbar_init(&empty[i], 1);
+    for (int i = 0; i < STAGES; ++i) mbar_init(&empty[i], RES ? 1 : 128);   // streaming: every MMA-warpgroup thread arrives
     mbar_init(accum_bar, 1);
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < UT * NBp; i += THREADS) cst[i] = 0.f;
   for (int i = threadIdx.x; i < NB; i += THREADS) lens_s[i] = i < B ? p.len[i] : 0;
-  if (warp == 1) {
-    tmem_alloc<512>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // The CTA owns all 512 TMEM columns, so the allocation starts at address 0.  Using the literal keeps the
-  // accumulator operand of tcgen05.mma in a uniform register without the ELECT / R2UR.BROADCAST waterfall
-  // loop nvcc otherwise emits per MMA for a value it cannot prove warp-uniform.
-  if (tmem_base != 0 && threadIdx.x == 0) {
-    *(volatile int*)p.err = 2;
-    printf("ds2: unexpected TMEM base %u (block %d)\n", tmem_base, blockIdx.x);
-  }
   const uint32_t tx_bytes = (uint32_t)(G * UT * 128 + B * 128);
 
-  if (warp == 0) {
+  if (warp == 8) {                                        // TMA producer
     if (RES) {
       if (lane == 0) {
         // weights once: NKR chunks of (G*16 rows x 64 fp16) into the resident region
@@ -349,69 +334,62 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
         }
       }
     }
-  } else if (warp == 1) {
-    if (RES) {
-      {   // the whole warp runs the issue loop converged (mma_f16_w: elect.sync inside), see tc_common.cuh
-        const uint32_t idesc = instr_desc(FMT_F16, MM, NB);
-        const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
-        const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * A_BYTES)));
-        const uint64_t a_step = (uint64_t)(A_BYTES >> 4), b_step = (uint64_t)(B_BYTES >> 4);
-        mbar_wait(&empty[0], 0);                 // weights resident
+  } else if (warp >= 4) {
+    // MMA warpgroup: accumulators in registers, handed to the epilogue warps as an image in shared memory; the
+    // accumulator width (batch padded to 32 * NCH) is chosen once, outside the step loop
+    with_nch<4>(NB, [&](auto nch) {
+      WgAcc<1, decltype(nch)::value> acc;
+      if (RES) {
+        {
+          const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
+          const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * A_BYTES)));
+          const uint64_t a_step = (uint64_t)(A_BYTES >> 4), b_step = (uint64_t)(B_BYTES >> 4);
+          mbar_wait(&empty[0], 0);                 // weights resident
+          uint32_t ph = 0;
+          for (int step = 1; step < T; ++step) {
+            for (int g = 0; g < NG; ++g) {
+              mbar_wait(full + g, ph);
+              if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+              const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
+              if (c1 == NKR && lane == 0) trace_stamp(p.trace, p.T, step, 3);
+              for (int c = c0; c < c1; ++c) {
+                const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
+                wg_mma4<true>(acc, ad, bd, c > 0);
+              }
+            }
+            wg_publish(acc, acc_img, accum_bar);
+            if (lane == 0) trace_stamp(p.trace, p.T, step, 4);
+            ph ^= 1;
+          }
+        }
+      } else
+      {
+        // The issue chain is the critical path of a step: the loop is free of div/mod and descriptor construction.
+        const uint64_t a_base = smem_desc_sw128(smem_u32(smem));
+        const uint64_t b_base = smem_desc_sw128(smem_u32(smem + A_BYTES));
+        const uint64_t stage_step = (uint64_t)(STAGE_BYTES >> 4);
+        int s = 0;
         uint32_t ph = 0;
         for (int step = 1; step < T; ++step) {
-          for (int g = 0; g < NG; ++g) {
-            mbar_wait(full + g, ph);
-            tc_fence_after();
-            if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-            const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
-            if (c1 == NKR && lane == 0) trace_stamp(p.trace, p.T, step, 3);
-            for (int c = c0; c < c1; ++c) {
-              const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
-              mma_f16_w(0u, ad, bd, idesc, c > 0);
-              mma_f16_w(0u, ad + 2, bd + 2, idesc, 1);
-              mma_f16_w(0u, ad + 4, bd + 4, idesc, 1);
-              mma_f16_w(0u, ad + 6, bd + 6, idesc, 1);
-            }
+          for (int c = 0; c < NK; ++c) {
+            mbar_wait(&full[s], ph);
+            if (c == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 1);
+            if (c == NK - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+            const uint64_t ad = a_base + (uint64_t)s * stage_step, bd = b_base + (uint64_t)s * stage_step;
+            wg_mma4<false>(acc, ad, bd, c > 0);
+            wg_release_all(&empty[s]);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
           }
-          mma_commit_w(accum_bar);
-          if (lane == 0) trace_stamp(p.trace, p.T, step, 4);
-          ph ^= 1;
+          wg_publish(acc, acc_img, accum_bar);
         }
       }
-    } else
-    {
-      // The issue chain is the critical path of a step: the whole warp runs it converged (mma_tf32_w: elect.sync
-      // inside; a single divergent lane costs ~70 cycles per tcgen05.mma, converged ~30-40) and the loop is free of
-      // div/mod and descriptor construction.
-      const uint32_t idesc = instr_desc(FMT_TF32, MM, NB);
-      const uint64_t a_base = smem_desc_sw128(smem_u32(smem));
-      const uint64_t b_base = smem_desc_sw128(smem_u32(smem + A_BYTES));
-      const uint64_t stage_step = (uint64_t)(STAGE_BYTES >> 4);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int step = 1; step < T; ++step) {
-        for (int c = 0; c < NK; ++c) {
-          mbar_wait(&full[s], ph);
-          if (c == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 1);
-          if (c == NK - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-          tc_fence_after();
-          const uint64_t ad = a_base + (uint64_t)s * stage_step, bd = b_base + (uint64_t)s * stage_step;
-          mma_tf32_w(0u, ad, bd, idesc, c > 0);
-          mma_tf32_w(0u, ad + 2, bd + 2, idesc, 1);
-          mma_tf32_w(0u, ad + 4, bd + 4, idesc, 1);
-          mma_tf32_w(0u, ad + 6, bd + 6, idesc, 1);
-          mma_commit_w(&empty[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        mma_commit_w(accum_bar);
-      }
-    }
-  } else {
-    // ---------------- epilogue warps: quarter q of TMEM == gate q (rows q*16 .. q*16+15 in lanes 0..15)
+    });
+  } else {                                                // warps 0..3: epilogue
+    // ---------------- epilogue warps: quarter q of accumulator-image == gate q (rows q*16 .. q*16+15 in lanes 0..15)
     // All 32 lanes work: lane L<16 owns row (q, L); its 32 batch columns are split with lane L+16
     // (columns 16..31 travel by shuffle), so every lane activates 16 values per 32-column chunk.
     const int q = warp % 4;
-    const int e = threadIdx.x - 64;          // 0..127
+    const int e = threadIdx.x;          // 0..127
     const int ul = lane & 15, half = lane >> 4;
     const int u = u0 + ul;
     const bool has_row = (q < G) || (RNN == DS2_RNN_GRU && q == 3);
@@ -432,9 +410,9 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
         }
         float a16[16];
         if (step > 0 && q < G) {
-          if (cb == 0) { mbar_wait(accum_bar, acc_phase); tc_fence_after(); if (e == 0) trace_stamp(p.trace, p.T, step, 5); }
+          if (cb == 0) { mbar_wait(accum_bar, acc_phase); if (e == 0) trace_stamp(p.trace, p.T, step, 5); }
           float acc[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
+          tmem_ld32(acc_img, acc_pitch(NB), ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
             const float hi = __shfl_sync(0xffffffffu, acc[16 + j], ul);   // row owner's upper columns
@@ -475,7 +453,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
         }
       }
       if (step > 0) acc_phase ^= 1;
-      tc_fence_before();
       if (e == 0) trace_stamp(p.trace, p.T, step, 6);
       named_bar_sync(1, 128);
       if (e == 0) trace_stamp(p.trace, p.T, step, 7);
@@ -584,14 +561,10 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
-// A sweep whose barrier wait timed out (or that found an unexpected TMEM base) leaves garbage behind: fail loudly.
+// A sweep whose barrier wait timed out leaves garbage behind: fail loudly.
 // Runs right after every sweep launch; the trap makes the next CUDA call of the process return an error.
 __global__ void sweep_check_kernel(const int* err) {
   if (*err != 0) {
@@ -601,9 +574,8 @@ __global__ void sweep_check_kernel(const int* err) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Every persistent CTA allocates all 512 TMEM columns, so two of them must never share an SM (the second
-// tcgen05.alloc would block while the first waits for it at the grid barrier): ask for more than half of
-// the 227 KB of shared memory even when the tiles are small.
+// One persistent CTA per SM (they spin at the grid barrier and would only take issue slots from each other): ask for
+// more than half of the 227 KB of shared memory even when the tiles are small.
 static size_t one_cta_per_sm(size_t smem) { return smem < 116 * 1024 ? 116 * 1024 : smem; }
 
 static long long* trace_ptr_from_env(const char* name) {
@@ -648,7 +620,7 @@ static size_t fwd_smem_bytes(int NB) {
   using namespace rp;
   size_t NBp = NB + 1;
   return 1024 + (size_t)STAGES * (A_BYTES + (size_t)NB * 128) + (5 * UT * NBp + NB + 4) * sizeof(float) +
-         (2 * STAGES + 2) * sizeof(uint64_t) + 64;
+         (2 * STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
 size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
@@ -662,7 +634,7 @@ size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
 }
 
 static void set_acc_layout(PersistParams& p) {
-  // accumulator width = power of two >= max(32, NB) columns; as many chains as fit in the 512 TMEM columns
+  // accumulator width = power of two >= max(32, NB) columns; as many chains as fit in the 512 accumulator columns
   int cols = 32;
   while (cols < p.NB) cols *= 2;
   p.acc_cols = cols;
@@ -684,7 +656,7 @@ static size_t res_smem_bytes(int NB, int H) {
   using namespace rp;
   size_t NBp = NB + 1;
   return 1024 + (size_t)(H / 64) * (A_BYTES + (size_t)NB * 128) + (5 * UT * NBp + NB + 4) * sizeof(float) +
-         (32 + STAGES + 2) * sizeof(uint64_t) + 64;
+         (32 + STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
 // workspace of the resident forward: [4 KB control][W16: D*G*H*H halfs][h16: D*T*B*H halfs]
@@ -700,7 +672,8 @@ static int launch_fwd_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cuda
   if (!vec_ok(a.gates, a.hseq, a.aux)) return 1;
   if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
   PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 7) / 8 * 8; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   p.training = a.training;
   p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux;
   p.trace = trace_ptr_from_env("DS2_TRACE_FWD");
@@ -732,7 +705,7 @@ static int launch_fwd_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cuda
   for (int d = 0; d < a.D; ++d) {
     p.b_ih[d] = a.b_ih[d];
     p.b_hh[d] = a.b_hh[d];
-    DS2_LAUNCH(f32_to_f16_kernel, 148 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
+    DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
     int rc = make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
     if (rc) return rc;
     rc = make_tmap_f16(&p.tmV[d], p.h16 + (size_t)d * a.T * a.B * a.H, 2, a.H, a.T * a.B, 1, (size_t)a.H, 0, 64, a.B, 1);
@@ -777,7 +750,8 @@ static int launch_fwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t 
     if (rc != 1) return rc;
   }
   PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 7) / 8 * 8; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   p.training = a.training;
   p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux;
   p.trace = trace_ptr_from_env("DS2_TRACE_FWD");
@@ -852,7 +826,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const _
   uint64_t* full = reinterpret_cast<uint64_t*>(cst + UT * NBp);
   uint64_t* empty = full + STAGES;
   uint64_t* accum_bar = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accum_bar + 1);
+  float* acc_img = reinterpret_cast<float*>(accum_bar + 1);   // accumulator image (tc::wg_store_acc)
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int d = p.d0 + blockIdx.x / p.NT, tile = blockIdx.x % p.NT, u0 = tile * UT;
@@ -863,28 +837,15 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const _
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmW[d]);
     tma_prefetch_desc(&p.tmV[d]);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 128); }   // every MMA-warpgroup thread arrives
     mbar_init(accum_bar, 1);
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < UT * NBp; i += THREADS) { cst[i] = 0.f; ex[i] = 0.f; }
-  if (warp == 1) {
-    tmem_alloc<512>(tmem_slot);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // The CTA owns all 512 TMEM columns, so the allocation starts at address 0.  Using the literal keeps the
-  // accumulator operand of tcgen05.mma in a uniform register without the ELECT / R2UR.BROADCAST waterfall
-  // loop nvcc otherwise emits per MMA for a value it cannot prove warp-uniform.
-  if (tmem_base != 0 && threadIdx.x == 0) {
-    *(volatile int*)p.err = 2;
-    printf("ds2: unexpected TMEM base %u (block %d)\n", tmem_base, blockIdx.x);
-  }
   const uint32_t tx_bytes = (uint32_t)(UT * 128 + B * 128);
 
-  if (warp == 0) {
+  if (warp == 8) {                                        // TMA producer
     if (lane == 0) {
       int s = 0;
       uint32_t ph = 0;
@@ -909,37 +870,35 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const _
         }
       }
     }
-  } else if (warp == 1) {
-    {
-      // The issue chain is the critical path of a step: the whole warp runs it converged (mma_tf32_w: elect.sync
-      // inside; a single divergent lane costs ~70 cycles per tcgen05.mma, converged ~30-40) and the loop is free of
-      // div/mod and descriptor construction.
-      const uint32_t idesc = instr_desc(FMT_TF32, MM, NB);
-      const uint64_t a_base = smem_desc_sw128(smem_u32(smem));
-      const uint64_t b_base = smem_desc_sw128(smem_u32(smem + A_BYTES));
-      const uint64_t stage_step = (uint64_t)(STAGE_BYTES >> 4);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int step = 1; step < T; ++step) {
-        for (int c = 0; c < NK; ++c) {
-          mbar_wait(&full[s], ph);
-          if (c == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 1);
-          if (c == NK - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-          tc_fence_after();
-          const uint64_t ad = a_base + (uint64_t)s * stage_step, bd = b_base + (uint64_t)s * stage_step;
-          mma_tf32_w(0u, ad, bd, idesc, c > 0);
-          mma_tf32_w(0u, ad + 2, bd + 2, idesc, 1);
-          mma_tf32_w(0u, ad + 4, bd + 4, idesc, 1);
-          mma_tf32_w(0u, ad + 6, bd + 6, idesc, 1);
-          mma_commit_w(&empty[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+  } else if (warp >= 4) {
+    // MMA warpgroup: accumulators in registers, handed to the epilogue warps as an image in shared memory; the
+    // accumulator width (batch padded to 32 * NCH) is chosen once, outside the step loop
+    with_nch<4>(NB, [&](auto nch) {
+      WgAcc<1, decltype(nch)::value> acc;
+      {
+        // The issue chain is the critical path of a step: the loop is free of div/mod and descriptor construction.
+        const uint64_t a_base = smem_desc_sw128(smem_u32(smem));
+        const uint64_t b_base = smem_desc_sw128(smem_u32(smem + A_BYTES));
+        const uint64_t stage_step = (uint64_t)(STAGE_BYTES >> 4);
+        int s = 0;
+        uint32_t ph = 0;
+        for (int step = 1; step < T; ++step) {
+          for (int c = 0; c < NK; ++c) {
+            mbar_wait(&full[s], ph);
+            if (c == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 1);
+            if (c == NK - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+            const uint64_t ad = a_base + (uint64_t)s * stage_step, bd = b_base + (uint64_t)s * stage_step;
+            wg_mma4<false>(acc, ad, bd, c > 0);
+            wg_release_all(&empty[s]);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
+          }
+          wg_publish(acc, acc_img, accum_bar);
         }
-        mma_commit_w(accum_bar);
       }
-    }
-  } else {
+    });
+  } else {                                                // warps 0..3: epilogue
     const int q = warp % 4;
-    const int e = threadIdx.x - 64;
+    const int e = threadIdx.x;
     uint32_t acc_phase = 0;
     for (int step = 0; step < T; ++step) {
       const int t = d == 0 ? T - 1 - step : step;
@@ -947,15 +906,14 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const _
       const bool tp_in = tp >= 0 && tp < T;
       if (q == 0 && step > 0) {          // rows 0..15 of the accumulator live in lanes 0..15 of quarter 0
         mbar_wait(accum_bar, acc_phase);
-        tc_fence_after();
         if (lane == 0) trace_stamp(p.trace, p.T, step, 3);
         for (int cb = 0; cb < NB; cb += 32) {
           float acc[32];
           const int nsum = min(p.nacc, NK * (BK / 8));
-          tmem_ld32(tmem_base + (uint32_t)cb, acc);
+          tmem_ld32(acc_img, acc_pitch(NB), (uint32_t)cb, acc);
           for (int a2 = 1; a2 < nsum; ++a2) {
             float part[32];
-            tmem_ld32(tmem_base + (uint32_t)(a2 * p.acc_cols + cb), part);
+            tmem_ld32(acc_img, acc_pitch(NB), (uint32_t)(a2 * p.acc_cols + cb), part);
 #pragma unroll
             for (int j = 0; j < 32; ++j) acc[j] += part[j];
           }
@@ -967,7 +925,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const _
         }
       }
       if (step > 0) acc_phase ^= 1;
-      tc_fence_before();
       named_bar_sync(1, 128);
       if (e == 0) trace_stamp(p.trace, p.T, step, 4);
       for (int pi = e; pi < UT * B; pi += 128) {
@@ -1009,18 +966,14 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const _
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
 // Backward sweep, split-K variant (the fast path): a 4-CTA cluster owns 64 hidden units; CTA `ks` of
 // the cluster reduces over a quarter of K = G*H, so every CTA issues the same number of MMAs per
 // step as the forward sweep with all 64 M rows useful.  The partial sums (64 units x B) are exchanged
-// through distributed shared memory in push form: TMEM quarter q of every CTA holds the rows that CTA q
+// through distributed shared memory in push form: accumulator-image quarter q of every CTA holds the rows that CTA q
 // of the cluster finishes, so epilogue warp q sends them straight into CTA q's shared memory with
 // st.async (16-byte stores that complete_tx on the destination's mbarrier); each CTA then reduces the four
 // slices it received from its own shared memory and finishes its 16 units (gate backward, carried dc / dh).
@@ -1125,7 +1078,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
   uint64_t* empty = full + (RES ? 32 : STAGES);                          // resident: [0] = weights landed
   uint64_t* accum_bar = empty + STAGES;
   uint64_t* part_bar = accum_bar + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(part_bar + 1);
+  float* acc_img = reinterpret_cast<float*>(part_bar + 1);   // accumulator image (tc::wg_store_acc)
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int ks = blockIdx.x % CL;                         // rank in the cluster == K split
@@ -1143,7 +1096,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
     tma_prefetch_desc(&p.tmW[d]);
     if (!LL) tma_prefetch_desc(&p.tmV[d]);
     for (int i = 0; i < (RES ? 32 : STAGES); ++i) mbar_init(&full[i], LL ? 4 : 1);   // LL: one arrival per loader warp
-    for (int i = 0; i < STAGES; ++i) mbar_init(&empty[i], 1);
+    for (int i = 0; i < STAGES; ++i) mbar_init(&empty[i], RES ? 1 : 128);   // streaming: every MMA-warpgroup thread arrives
     mbar_init(accum_bar, 1);
     mbar_init(part_bar, 1);
     fence_barrier_init();
@@ -1160,22 +1113,11 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
     }
     fence_proxy_async();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   cluster_sync_all();                                     // peers' mbarriers are initialised
-  const uint32_t tmem_base = *tmem_slot;
-  // The CTA owns all 512 TMEM columns, so the allocation starts at address 0.  Using the literal keeps the
-  // accumulator operand of tcgen05.mma in a uniform register without the ELECT / R2UR.BROADCAST waterfall
-  // loop nvcc otherwise emits per MMA for a value it cannot prove warp-uniform.
-  if (tmem_base != 0 && threadIdx.x == 0) {
-    *(volatile int*)p.err = 2;
-    printf("ds2: unexpected TMEM base %u (block %d)\n", tmem_base, blockIdx.x);
-  }
   const uint32_t tx_bytes = (uint32_t)(UM * 128 + B * 128);
 
-  if (warp == 0) {
+  if (warp == 8) {                                        // TMA producer
     if (RES) {
       if (lane == 0) {
         mbar_arrive_expect_tx(&empty[0], (uint32_t)(NKR * UM * 128));
@@ -1233,87 +1175,77 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         }
       }
     }
-  } else if (warp == 1) {
-    if (RES) {
-      {   // the whole warp runs the issue loop converged (mma_f16_w: elect.sync inside): 64 MMAs per step in ~1.9k
-          // cycles instead of ~4.9k from a single divergent lane
-        const uint32_t idesc = instr_desc(FMT_F16, UM, NB);
-        const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
-        const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * A_BYTES)));
-        const uint64_t a_step = (uint64_t)(A_BYTES >> 4), b_step = (uint64_t)(B_BYTES >> 4);
-        mbar_wait(&empty[0], 0);
+  } else if (warp >= 4) {
+    // MMA warpgroup: accumulators in registers, handed to the epilogue warps as an image in shared memory; the
+    // accumulator width (batch padded to 32 * NCH) is chosen once, outside the step loop
+    with_nch<UM == 64 ? 4 : 2>(NB, [&](auto nch) {
+      WgAcc<UM / 64, decltype(nch)::value> acc;
+      if (RES) {
+        {
+          const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
+          const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * A_BYTES)));
+          const uint64_t a_step = (uint64_t)(A_BYTES >> 4), b_step = (uint64_t)(B_BYTES >> 4);
+          mbar_wait(&empty[0], 0);
+          uint32_t ph = 0;
+          for (int step = 1; step < T; ++step) {
+            if constexpr (NKR_T > 0) {
+              constexpr int NGT = (NKR_T + 3) / 4;
+  #pragma unroll
+              for (int g = 0; g < NGT; ++g) {
+                mbar_wait(full + g, ph);
+                if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+                if (g == NGT - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 3);
+  #pragma unroll
+                for (int c = 4 * g; c < (4 * g + 4 < NKR_T ? 4 * g + 4 : NKR_T); ++c) {
+                  const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
+                  wg_mma4<true>(acc, ad, bd, c > 0);
+                }
+              }
+            } else {
+              for (int g = 0; g < NG; ++g) {
+                mbar_wait(full + g, ph);
+                if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+                const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
+                if (c1 == NKR && lane == 0) trace_stamp(p.trace, p.T, step, 3);
+                for (int c = c0; c < c1; ++c) {
+                  const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
+                  wg_mma4<true>(acc, ad, bd, c > 0);
+                }
+              }
+            }
+            wg_publish(acc, acc_img, accum_bar);
+            if (lane == 0) trace_stamp(p.trace, p.T, step, 4);
+            ph ^= 1;
+          }
+        }
+      } else
+      {
+        const uint64_t a_base = smem_desc_sw128(smem_u32(smem));
+        const uint64_t b_base = smem_desc_sw128(smem_u32(smem + A_BYTES));
+        const uint64_t stage_step = (uint64_t)(STAGE_BYTES >> 4);
+        int s = 0;
         uint32_t ph = 0;
         for (int step = 1; step < T; ++step) {
-          if constexpr (NKR_T > 0) {
-            constexpr int NGT = (NKR_T + 3) / 4;
-#pragma unroll
-            for (int g = 0; g < NGT; ++g) {
-              mbar_wait(full + g, ph);
-              tc_fence_after();
-              if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-              if (g == NGT - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 3);
-#pragma unroll
-              for (int c = 4 * g; c < (4 * g + 4 < NKR_T ? 4 * g + 4 : NKR_T); ++c) {
-                const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
-                mma_f16_w(0u, ad, bd, idesc, c > 0);
-                mma_f16_w(0u, ad + 2, bd + 2, idesc, 1);
-                mma_f16_w(0u, ad + 4, bd + 4, idesc, 1);
-                mma_f16_w(0u, ad + 6, bd + 6, idesc, 1);
-              }
-            }
-          } else {
-            for (int g = 0; g < NG; ++g) {
-              mbar_wait(full + g, ph);
-              tc_fence_after();
-              if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-              const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
-              if (c1 == NKR && lane == 0) trace_stamp(p.trace, p.T, step, 3);
-              for (int c = c0; c < c1; ++c) {
-                const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
-                mma_f16_w(0u, ad, bd, idesc, c > 0);
-                mma_f16_w(0u, ad + 2, bd + 2, idesc, 1);
-                mma_f16_w(0u, ad + 4, bd + 4, idesc, 1);
-                mma_f16_w(0u, ad + 6, bd + 6, idesc, 1);
-              }
-            }
+          for (int c = 0; c < NK; ++c) {
+            mbar_wait(&full[s], ph);
+            if (c == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 1);
+            if (c == NK - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+            const uint64_t ad = a_base + (uint64_t)s * stage_step, bd = b_base + (uint64_t)s * stage_step;
+            wg_mma4<false>(acc, ad, bd, c > 0);
+            wg_release_all(&empty[s]);
+            if (++s == STAGES) { s = 0; ph ^= 1; }
           }
-          mma_commit_w(accum_bar);
-          if (lane == 0) trace_stamp(p.trace, p.T, step, 4);
-          ph ^= 1;
+          wg_publish(acc, acc_img, accum_bar);
         }
       }
-    } else
-    {   // converged issue, see mma_tf32_w
-      const uint32_t idesc = instr_desc(FMT_TF32, UM, NB);
-      const uint64_t a_base = smem_desc_sw128(smem_u32(smem));
-      const uint64_t b_base = smem_desc_sw128(smem_u32(smem + A_BYTES));
-      const uint64_t stage_step = (uint64_t)(STAGE_BYTES >> 4);
-      int s = 0;
-      uint32_t ph = 0;
-      for (int step = 1; step < T; ++step) {
-        for (int c = 0; c < NK; ++c) {
-          mbar_wait(&full[s], ph);
-          if (c == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 1);
-          if (c == NK - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-          tc_fence_after();
-          const uint64_t ad = a_base + (uint64_t)s * stage_step, bd = b_base + (uint64_t)s * stage_step;
-          mma_tf32_w(0u, ad, bd, idesc, c > 0);
-          mma_tf32_w(0u, ad + 2, bd + 2, idesc, 1);
-          mma_tf32_w(0u, ad + 4, bd + 4, idesc, 1);
-          mma_tf32_w(0u, ad + 6, bd + 6, idesc, 1);
-          mma_commit_w(&empty[s]);
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-        mma_commit_w(accum_bar);
-      }
-    }
-  } else {
+    });
+  } else {                                                // warps 0..3: epilogue
     const int q = warp % 4;
-    const int e = threadIdx.x - 64;
+    const int e = threadIdx.x;
     const int ul = lane & 15, half = lane >> 4;
     uint32_t acc_phase = 0, part_phase = 0;
     // Destination of this lane's accumulator row: the CTA that finishes the row's unit, slice ks (= this CTA's rank)
-    // of its tile.  M = 64 (CL 4): TMEM quarter q holds rows 16q..16q+15 in lanes 0..15 -> CTA q, the 32 columns are
+    // of its tile.  M = 64 (CL 4): accumulator-image quarter q holds rows 16q..16q+15 in lanes 0..15 -> CTA q, the 32 columns are
     // split with lane+16 by shuffle.  M = 128 (CL 8): lane l of quarter q holds row 32q+l -> CTA 2q + l/16, all 32
     // columns of the row are sent by that lane.
     const int dst_cta = CL == 4 ? q : 2 * q + half;
@@ -1413,7 +1345,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         if (e == 0) mbar_arrive_expect_tx(part_bar, part_tx);   // arm this step's phase (peers may already have sent)
         // send this CTA's partial tile: row (16q + ul), 32 columns split over the two half-warps
         mbar_wait(accum_bar, acc_phase);
-        tc_fence_after();
         if (RES) {
           // non-LL: this step's MMAs ran, so the grid barrier was passed: the maximum of step-1 the producer forwarded
           // is final.  LL: the four loader warps left the maximum over all (CTA, warp) words of step-1 in wmax[parity]
@@ -1433,7 +1364,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         if (e == 0) trace_stamp(p.trace, p.T, step, 5);
         for (int cb = 0; cb < NB; cb += 32) {
           float acc[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
+          tmem_ld32(acc_img, acc_pitch(NB), ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
           if (CL == 4) {
             float v[16];
 #pragma unroll
@@ -1457,7 +1388,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
           }
         }
         acc_phase ^= 1;
-        tc_fence_before();
         if (e == 0) trace_stamp(p.trace, p.T, step, 6);
         mbar_wait_cluster(part_bar, part_phase, p.err);   // all CL slices of this CTA's units have landed
         part_phase ^= 1;
@@ -1699,17 +1629,15 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
   cluster_sync_all();                                     // nobody exits while a peer may still read its tile
-  if (warp == 1) tmem_dealloc<512>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Forward sweep, split-K variant (LSTM / GRU, resident fp16 weights).  A 2-CTA cluster owns 32 hidden units of
 // one direction; CTA `rank` multiplies the G*32 gate rows (MMA M = 128, rows ordered [owner CTA][gate][unit])
 // with its half of K = H, so a step issues H/32 MMAs instead of H/16 — the single-thread MMA issue chain is the
-// longest part of a step.  TMEM lanes 0..63 hold the rows CTA 0 finishes, lanes 64..127 those of CTA 1: every
+// longest part of a step.  accumulator-image lanes 0..63 hold the rows CTA 0 finishes, lanes 64..127 those of CTA 1: every
 // epilogue warp pushes its 32 accumulator rows into the owner's shared memory with st.async (complete_tx on
 // the owner's mbarrier); the owner adds the two partial tiles, the input projection and the biases, and runs
 // gates + cell update for its 16 units in one pass (thread = 4 consecutive units x one batch column).
@@ -1735,7 +1663,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
   uint64_t* wbar = full + 8;
   uint64_t* accum_bar = wbar + 1;
   uint64_t* part_bar = accum_bar + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(part_bar + 1);
+  float* acc_img = reinterpret_cast<float*>(part_bar + 1);   // accumulator image (tc::wg_store_acc)
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int rank = blockIdx.x & 1, cl = blockIdx.x >> 1;
@@ -1765,19 +1693,11 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
     }
     fence_proxy_async();
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   cluster_sync_all();                                     // the peer's mbarriers are initialised
-  const uint32_t tmem_base = *tmem_slot;
-  if (tmem_base != 0 && threadIdx.x == 0) {               // literal TMEM address 0 in the MMAs, see the other kernels
-    *(volatile int*)p.err = 2;
-    printf("ds2: unexpected TMEM base %u (block %d)\n", tmem_base, blockIdx.x);
-  }
   const int kc0 = rank * NKR;                             // first K chunk (of H/64) of this CTA
 
-  if (warp == 0) {
+  if (warp == 8) {                                        // TMA producer
     if (lane == 0) {
       // weights once: per chunk the rows of the two owners, [gate][16 units] each (rows >= 16 G of a half unused)
       mbar_arrive_expect_tx(wbar, (uint32_t)(NKR * 2 * G * UT * 128));
@@ -1806,58 +1726,53 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
         trace_stamp(p.trace, p.T, step, 1);
       }
     }
-  } else if (warp == 1) {
-    {   // the whole warp runs the issue loop converged (mma_f16_w: elect.sync inside): 32 MMAs per step in ~1.2k
-        // cycles instead of ~2.4k from a single divergent lane
-      const uint32_t idesc = instr_desc(FMT_F16, 128, NB);
-      const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
-      const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * AW)));
-      const uint64_t a_step = (uint64_t)(AW >> 4), b_step = (uint64_t)(B_BYTES >> 4);
-      mbar_wait(wbar, 0);
-      uint32_t ph = 0;
-      for (int step = 1; step < T; ++step) {
-        if constexpr (NKR_T > 0) {
-          constexpr int NGT = (NKR_T + 3) / 4;
-#pragma unroll
-          for (int g = 0; g < NGT; ++g) {
-            mbar_wait(full + g, ph);
-            tc_fence_after();
-            if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-            if (g == NGT - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 3);
-#pragma unroll
-            for (int c = 4 * g; c < (4 * g + 4 < NKR_T ? 4 * g + 4 : NKR_T); ++c) {
-              const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
-              mma_f16_w(0u, ad, bd, idesc, c > 0);
-              mma_f16_w(0u, ad + 2, bd + 2, idesc, 1);
-              mma_f16_w(0u, ad + 4, bd + 4, idesc, 1);
-              mma_f16_w(0u, ad + 6, bd + 6, idesc, 1);
+  } else if (warp >= 4) {
+    // MMA warpgroup: accumulators in registers, handed to the epilogue warps as an image in shared memory; the
+    // accumulator width (batch padded to 32 * NCH) is chosen once, outside the step loop
+    with_nch<2>(NB, [&](auto nch) {
+      WgAcc<2, decltype(nch)::value> acc;
+      {
+        const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
+        const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * AW)));
+        const uint64_t a_step = (uint64_t)(AW >> 4), b_step = (uint64_t)(B_BYTES >> 4);
+        mbar_wait(wbar, 0);
+        uint32_t ph = 0;
+        for (int step = 1; step < T; ++step) {
+          if constexpr (NKR_T > 0) {
+            constexpr int NGT = (NKR_T + 3) / 4;
+  #pragma unroll
+            for (int g = 0; g < NGT; ++g) {
+              mbar_wait(full + g, ph);
+              if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+              if (g == NGT - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 3);
+  #pragma unroll
+              for (int c = 4 * g; c < (4 * g + 4 < NKR_T ? 4 * g + 4 : NKR_T); ++c) {
+                const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
+                wg_mma4<true>(acc, ad, bd, c > 0);
+              }
+            }
+          } else {
+            for (int g = 0; g < NG; ++g) {
+              mbar_wait(full + g, ph);
+              if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
+              const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
+              if (c1 == NKR && lane == 0) trace_stamp(p.trace, p.T, step, 3);
+              for (int c = c0; c < c1; ++c) {
+                const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
+                wg_mma4<true>(acc, ad, bd, c > 0);
+              }
             }
           }
-        } else {
-          for (int g = 0; g < NG; ++g) {
-            mbar_wait(full + g, ph);
-            tc_fence_after();
-            if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-            const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
-            if (c1 == NKR && lane == 0) trace_stamp(p.trace, p.T, step, 3);
-            for (int c = c0; c < c1; ++c) {
-              const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
-              mma_f16_w(0u, ad, bd, idesc, c > 0);
-              mma_f16_w(0u, ad + 2, bd + 2, idesc, 1);
-              mma_f16_w(0u, ad + 4, bd + 4, idesc, 1);
-              mma_f16_w(0u, ad + 6, bd + 6, idesc, 1);
-            }
-          }
+          wg_publish(acc, acc_img, accum_bar);
+          if (lane == 0) trace_stamp(p.trace, p.T, step, 4);
+          ph ^= 1;
         }
-        mma_commit_w(accum_bar);
-        if (lane == 0) trace_stamp(p.trace, p.T, step, 4);
-        ph ^= 1;
       }
-    }
-  } else {
+    });
+  } else {                                                // warps 0..3: epilogue
     const int q = warp % 4;
-    const int e = threadIdx.x - 64;          // 0..127
-    // TMEM lane (= row) 32q + lane belongs to CTA q/2; inside that CTA's 64-row slice it is row 32 (q&1) + lane
+    const int e = threadIdx.x;          // 0..127
+    // accumulator-image lane (= row) 32q + lane belongs to CTA q/2; inside that CTA's 64-row slice it is row 32 (q&1) + lane
     const int dst_cta = q >> 1;
     const int my_row = 32 * (q & 1) + lane;
     const uint32_t dst_row = mapa_u32(smem_u32(part), (uint32_t)dst_cta) + (uint32_t)(rank * xt_slice(64, NB) * 4);
@@ -1895,11 +1810,10 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
       if (step > 0) {
         if (e == 0) mbar_arrive_expect_tx(part_bar, part_tx);   // arm this step's phase (the peer may already have sent)
         mbar_wait(accum_bar, acc_phase);
-        tc_fence_after();
         if (e == 0) trace_stamp(p.trace, p.T, step, 5);
         for (int cb = 0; cb < NB; cb += 32) {
           float acc[32];
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
+          tmem_ld32(acc_img, acc_pitch(NB), ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const int c0 = cb + 4 * i;                    // NB is a multiple of 8: a group of 4 columns is in or out
@@ -1908,7 +1822,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
           }
         }
         acc_phase ^= 1;
-        tc_fence_before();
         if (e == 0) trace_stamp(p.trace, p.T, step, 6);
         mbar_wait_cluster(part_bar, part_phase, p.err);   // both partial tiles of this CTA's rows have landed
         part_phase ^= 1;
@@ -2007,7 +1920,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
       // step completed, i.e. when the MMAs that read the tile are done.  One 16-byte packet = 8 consecutive k of
       // one batch row; consecutive threads take consecutive packets of a row (512 contiguous bytes per warp
       // instruction); up to 8 polls in flight per thread; a group of 4 K chunks is handed to the MMA thread as soon
-      // as it is complete (fence.proxy.async: generic-proxy stores -> async-proxy reads of tcgen05.mma).
+      // as it is complete (fence.proxy.async: generic-proxy stores -> async-proxy reads of wgmma).
       auto fetch_h = [&](int t_src) {
         const __half* src = p.h16 + ((size_t)d * T + t_src) * B * H + (size_t)kc0 * 64;
         const uint32_t hb = smem_u32(smem + NKR * AW);
@@ -2078,17 +1991,15 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
       }
     }
   }
-  tc_fence_before();
   __syncthreads();
   cluster_sync_all();                                     // nobody exits while the peer may still write into its tile
-  if (warp == 1) tmem_dealloc<512>(tmem_base);
 }
 
 static size_t fwd_splitk_smem_bytes(int NB, int H) {
   using namespace rp;
   size_t NBp = NB + 1;
   return 1024 + (size_t)(H / 128) * (128 * 128 + (size_t)NB * 128) + (2 * xt_slice(64, NB) + UT * NBp + NB + 4) * sizeof(float) +
-         12 * sizeof(uint64_t) + 64;
+         12 * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
 // returns 1 when the shape / device does not take this variant (the caller then uses the 16-unit resident kernel)
@@ -2100,7 +2011,8 @@ static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   if (!vec_ok(a.gates, a.hseq, a.aux) || !a.aux) return 1;
   if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
   PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 15) / 16 * 16;   // MMA M = 128 needs N % 16 == 0
+  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32;
+  if (p.NB > 64) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   p.H = a.H; p.D = a.D; p.NT = a.H / 32; p.G = G;
   p.training = a.training;
   p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux;
@@ -2146,7 +2058,7 @@ static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   for (int d = 0; d < a.D; ++d) {
     p.b_ih[d] = a.b_ih[d];
     p.b_hh[d] = a.b_hh[d];
-    DS2_LAUNCH(f32_to_f16_kernel, 148 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
+    DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
     int rc = make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
     if (rc) return rc;
     rc = make_tmap_f16(&p.tmV[d], p.h16 + (size_t)d * a.T * a.B * a.H, 2, a.H, a.T * a.B, 1, (size_t)a.H, 0, 64, a.B, 1);
@@ -2184,7 +2096,7 @@ static size_t splitk_smem_bytes(int NB, int CL) {
   using namespace rp;
   size_t NBp = NB + 1;
   return 1024 + (size_t)STAGES * ((size_t)UT * CL * 128 + (size_t)NB * 128) +
-         ((size_t)CL * xt_slice(UT, NB) + UT * NBp + NB + 16) * sizeof(float) + (2 * STAGES + 3) * sizeof(uint64_t) + 64;
+         ((size_t)CL * xt_slice(UT, NB) + UT * NBp + NB + 16) * sizeof(float) + (2 * STAGES + 3) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
 // max |x| over n floats -> atomicMax on float bits (x >= 0 after fabs)
@@ -2221,7 +2133,7 @@ static size_t splitk_res_smem_bytes(int NB, int Kc, int CL) {
   using namespace rp;
   size_t NBp = NB + 1;
   return 1024 + (size_t)(Kc / 64) * ((size_t)UT * CL * 128 + (size_t)NB * 128) +
-         ((size_t)CL * xt_slice(UT, NB) + UT * NBp + NB + 16) * sizeof(float) + (32 + STAGES + 3) * sizeof(uint64_t) + 64;
+         ((size_t)CL * xt_slice(UT, NB) + UT * NBp + NB + 16) * sizeof(float) + (32 + STAGES + 3) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 // workspace of the resident backward: [4 KB control][gmax D*(T+1) uints][W^T fp16: D*H*GH][dg16: T*B*D*GH]
 // (+ [dymax: T uints][gmeta: D*T*(H/16)*4 uints] after gmax: H/16 CTAs per direction, 4 epilogue warps each)
@@ -2243,7 +2155,8 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
   if (!vec_ok(a.gates, a.hseq, a.aux, a.dy)) return 1;
   if (ws_bytes < splitk_res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
   PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 7) / 8 * 8; p.H = a.H; p.D = a.D; p.NT = a.H / UM; p.G = G;
+  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UM; p.G = G;
+  if (p.NB > (CL == 8 ? 64 : 128)) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   p.training = 1;
   p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
   p.trace = trace_ptr_from_env("DS2_TRACE_BWD");
@@ -2297,8 +2210,8 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
   cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg);
   if (oe != cudaSuccess) { (void)cudaGetLastError(); return 1; }
   if (max_clusters * CL < grid) {
-    // 8-CTA clusters are only worth it when both directions run concurrently (B200: 16 clusters of 8 do not fit the
-    // GPCs, measured: 10.4k cycles per step instead of 11.7k, but the two directions then run back to back)
+    // 8-CTA clusters are only worth it when both directions run concurrently (otherwise the two directions run
+    // back to back)
     if (CL == 8 || max_clusters * CL < p.NT * CL) return 1;
     grid = p.NT * CL;
     launches = a.D;
@@ -2314,7 +2227,7 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
   for (int d = 0; d < a.D; ++d) {
     const __half* wsrc = static_cast<const __half*>(a.w_hhT16[d]);
     if (!cached) {
-      DS2_LAUNCH(f32_to_f16_kernel, 148 * 4, 256, 0, st, wn, a.w_hh[d], wT16 + (size_t)d * wn);
+      DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], wT16 + (size_t)d * wn);
       wsrc = wT16 + (size_t)d * wn;
     }
     int rc = make_tmap_f16(&p.tmW[d], wsrc, 2, GH, a.H, 1, (size_t)GH, 0, 64, UM, 1);
@@ -2373,7 +2286,8 @@ static int launch_bwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   if (CL == 8 && ((a.B + 7) / 8 * 8) % 16 != 0) return 1;
   if (!vec_ok(a.gates, a.hseq, a.aux, a.dy)) return 1;
   PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 7) / 8 * 8; p.H = a.H; p.D = a.D; p.NT = a.H / UM; p.G = G;
+  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UM; p.G = G;
+  if (p.NB > (CL == 8 ? 64 : 128)) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   p.training = 1;
   p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
   p.trace = trace_ptr_from_env("DS2_TRACE_BWD");
@@ -2446,7 +2360,8 @@ static int launch_bwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t 
   const int GH = G * a.H;
   { int mrc = materialize_w_hh(a, st); if (mrc) return mrc; }   // fp32 W_hh^T through TMA
   PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 7) / 8 * 8; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   p.training = 1;
   p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
   p.trace = trace_ptr_from_env("DS2_TRACE_BWD");

@@ -136,7 +136,7 @@ int ds2_spectrogram_batch(int n_utts, const float* wave, const int64_t* offsets,
              reinterpret_cast<const long long*>(offsets), dst_row, n_fft, hop, window, pad_reflect, out, Tmax, sums);
   const int F = n_fft / 2 + 1;
   int bx = cdiv((long long)F * Tmax, 256 * 4);
-  bx = bx < 1 ? 1 : (bx > 148 ? 148 : bx);
+  bx = bx < 1 ? 1 : (bx > 132 ? 132 : bx);
   DS2_LAUNCH(spect_normalize_pad_kernel, dim3(bx, n_utts), 256, 0, st, n_utts, F, Tmax,
              reinterpret_cast<const long long*>(offsets), dst_row, hop, normalize, sums, out);
   return DS2_OK;

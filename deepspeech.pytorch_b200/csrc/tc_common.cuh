@@ -1,10 +1,14 @@
-// sm_100a building blocks shared by the tcgen05 kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// TMEM allocation, UMMA shared-memory / instruction descriptors, tcgen05.mma / commit / ld.
-// Bit layouts follow cute/arch/mma_sm100_desc.hpp (UMMA::SmemDescriptor / InstrDescriptor).
+// sm_90a building blocks shared by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA
+// (wgmma) shared-memory descriptors, issue / commit / wait, and the shared-memory accumulator image the recurrent
+// sweeps hand from the MMA warpgroup to their epilogue warps.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <type_traits>
+
+#include "wgmma.cuh"
 
 namespace ds2 {
 namespace tc {
@@ -71,9 +75,8 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-// Warp-converged issue: every lane executes the instruction stream, one elected lane issues.  A lone divergent
-// lane (`if (lane == 0)`) pays a uniform-register round trip per descriptor / address operand: ~110 cycles per TMA
-// instruction, ~76 per tcgen05.mma (see mma_*_w below).
+// Warp-converged issue: every lane executes the instruction stream, one elected lane issues (a lone divergent
+// lane pays a uniform-register round trip per descriptor / address operand).
 __device__ __forceinline__ void mbar_arrive_expect_tx_w(uint64_t* bar, uint32_t bytes) {
   asm volatile(
       "{\n\t.reg .pred pe;\n\telect.sync _|pe, 0xffffffff;\n\t"
@@ -96,118 +99,125 @@ __device__ __forceinline__ void tma_load_3d_w(void* smem_dst, const CUtensorMap*
       : "memory");
 }
 
-// ---- TMEM -------------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {  // one full warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(NCOLS));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS));
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---- descriptors ------------------------------------------------------------------------------
-// K-major operand tile stored as rows of 128 bytes (32 fp32 / 64 fp16) with the 128-byte swizzle
-// (what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 bytes apart (SBO).
+// ---- warpgroup MMA (wgmma) --------------------------------------------------------------------
+// K-major operand tile stored as rows of 128 bytes (32 fp32 / 64 fp16) with the 128-byte swizzle (what TMA writes
+// with CU_TENSOR_MAP_SWIZZLE_128B): 8-row groups are 1024 bytes apart (stride byte offset), the leading byte offset
+// is unused for swizzled K-major tiles.  A k-step (32 bytes) advances the start address field by 2, 64 rows by 512.
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);   // start address, bits [0,14)
-  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major) = 1
+  d |= (uint64_t)1 << 16;                        // leading byte offset (unused)
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                        // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                        // layout type SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                        // layout type SWIZZLE_128B
   return d;
 }
-enum { FMT_F16 = 0, FMT_BF16 = 1, FMT_TF32 = 2 };
-// fp32 accumulate, both operands K-major
-__host__ __device__ constexpr uint32_t instr_desc(int fmt, int M, int N) {
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; issued by ONE thread
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Warp-converged issue: EVERY lane of the MMA warp executes the call, elect.sync picks the lane that issues.  With
-// warp-uniform operands the descriptors stay in uniform registers; issuing from one divergent lane instead costs an
-// R2UR / ELECT / branch waterfall per instruction (measured, tools/mma_ts_microbench.cu: 64-76 cycles per tcgen05.mma
-// against 29-38 converged — the single-thread issue chain, not the tensor pipe, bounded the recurrent steps' MMA phase).
-// tell the compiler a value is warp-uniform (lane 0's copy): arithmetic on it then runs in the uniform datapath and the
-// MMA operands need no R2UR per instruction
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// tell the compiler a value is warp-uniform (lane 0's copy): arithmetic on it then runs in the uniform datapath
 __device__ __forceinline__ uint64_t warp_uniform(uint64_t v) {
   const uint32_t lo = __shfl_sync(0xffffffffu, (uint32_t)v, 0), hi = __shfl_sync(0xffffffffu, (uint32_t)(v >> 32), 0);
   return ((uint64_t)hi << 32) | lo;
 }
-__device__ __forceinline__ void mma_f16_w(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, pe;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_tf32_w(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p, pe;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "@pe tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_commit_w(uint64_t* bar) {
-  asm volatile(
-      "{\n\t.reg .pred pe;\n\t"
-      "elect.sync _|pe, 0xffffffff;\n\t"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}" ::"r"(smem_u32(bar))
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// Release a pipeline stage once the MMAs issued so far have read it: every thread of the warpgroup waits for its
+// wgmma groups, one thread arrives on the stage's (count 1) mbarrier.
+__device__ __forceinline__ void wg_release(uint64_t* bar) {
+  wg_commit();
+  wg_wait<0>();
+  if ((threadIdx.x & 127) == 0) mbar_arrive(bar);
 }
 
-// TMEM -> registers: this thread's lane (row), 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// floats of the accumulator image for a batch width NB (a multiple of 32: the epilogues read 32 columns at a time; odd
+// pitch: the 32 lanes of a warp read 32 different rows without bank conflicts)
+__host__ __device__ constexpr int acc_pitch(int NB) { return (NB + 31) / 32 * 32 + 1; }
+__host__ __device__ constexpr int acc_image_bytes(int NB) { return 128 * acc_pitch(NB) * 4; }
+
+// The same for a stage barrier initialised with count 128: every thread arrives, so no wgmma of the loop sits behind a
+// divergent branch (which makes ptxas serialise them).
+__device__ __forceinline__ void wg_release_all(uint64_t* bar) {
+  wg_commit();
+  wg_wait<0>();
+  mbar_arrive(bar);
+}
+
+// Accumulator of the recurrent sweeps: MH blocks of 64 rows x 32*NCH columns (the batch, padded to a multiple of 32),
+// issued as wgmma m64n32 per (row block, column chunk).  Shapes are compile-time, so no wgmma sits on a divergent path.
+template <int MH, int NCH>
+struct WgAcc {
+  float r[MH][NCH][16];
+};
+// D (+)= A . B^T for a K step: A = MH x 64 rows at adesc (+512 per 64 rows), B = 32*NCH rows at bdesc (+256 per 32 rows)
+template <bool F16, int MH, int NCH>
+__device__ __forceinline__ void wg_mma_nb(WgAcc<MH, NCH>& acc, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+  for (int h = 0; h < MH; ++h) {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+      Wgmma<32, F16>::mma(acc.r[h][c], adesc + (uint64_t)(512 * h), bdesc + (uint64_t)(256 * c), accumulate);
+  }
 }
-
+// the four k-steps of one 128-byte K chunk (K = 32 tf32 / 64 fp16); `accumulate` = 0 starts a new sum
+template <bool F16, int MH, int NCH>
+__device__ __forceinline__ void wg_mma4(WgAcc<MH, NCH>& acc, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  wg_fence();
+  wg_mma_nb<F16>(acc, adesc, bdesc, accumulate);
+#pragma unroll
+  for (int k = 1; k < 4; ++k) wg_mma_nb<F16>(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
+}
+// Call f(std::integral_constant<int, NB / 32>) for a batch width NB = 32, 64, .. 32 * MAXCH: the MMA loop of a sweep is
+// instantiated once per accumulator width and chosen once per launch, outside the step loop.
+template <int MAXCH, class F>
+__device__ __forceinline__ void with_nch(int NB, F&& f) {
+  if (NB == 32) f(std::integral_constant<int, 1>{});
+  else if constexpr (MAXCH >= 2) {
+    if (NB == 64) f(std::integral_constant<int, 2>{});
+    else if constexpr (MAXCH >= 4) {
+      if (NB == 96) f(std::integral_constant<int, 3>{});
+      else if (NB == 128) f(std::integral_constant<int, 4>{});
+    }
+  }
+}
+// Shared-memory image of the accumulator, addressed like the accumulator rows the epilogues read: row `lane` of
+// `pitch` floats.  M = 128 (MH = 2): lane = row; M = 64: row r sits in lane 32 (r / 16) + r % 16 (rows 16 q .. 16 q + 15
+// in lanes 0..15 of quarter q).  Called by the whole warpgroup after wg_wait<0>().
+template <int MH, int NCH>
+__device__ __forceinline__ void wg_store_acc(const WgAcc<MH, NCH>& acc, float* tm, int pitch) {
+  const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < MH; ++h) {
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int col = 32 * c + 8 * i + 2 * (l & 3);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int r = 16 * w + (l >> 2) + 8 * hh;
+          const int lane = MH == 2 ? 64 * h + r : 32 * (r >> 4) + (r & 15);
+          tm[lane * pitch + col] = acc.r[h][c][4 * i + 2 * hh];
+          tm[lane * pitch + col + 1] = acc.r[h][c][4 * i + 2 * hh + 1];
+        }
+      }
+    }
+  }
+}
+// All MMAs of the step done: write the accumulator image, then one arrival on `bar` (count 1) once the whole
+// warpgroup has written (named barrier 2 orders the other threads' stores before the arrival's release).
+template <int MH, int NCH>
+__device__ __forceinline__ void wg_publish(const WgAcc<MH, NCH>& acc, float* tm, uint64_t* bar) {
+  wg_commit();
+  wg_wait<0>();
+  wg_store_acc(acc, tm, acc_pitch(32 * NCH));
+  asm volatile("bar.sync 2, 128;" ::: "memory");
+  if ((threadIdx.x & 127) == 0) mbar_arrive(bar);
+}
+// accumulator image -> registers: this thread's lane (taddr >> 16 plus the lane id), 32 consecutive columns
+__device__ __forceinline__ void tmem_ld32(const float* tm, int pitch, uint32_t taddr, float* v) {
+  const float* src = tm + (size_t)((taddr >> 16) + (threadIdx.x & 31)) * pitch + (taddr & 0xFFFFu);
+#pragma unroll
+  for (int i = 0; i < 32; ++i) v[i] = src[i];
+}
 }  // namespace tc
 
 // ---- host: tensor-map encoding through the driver entry point (no -lcuda link dependency) ------

@@ -17,7 +17,7 @@ class GreedyDecoder:
     def decode_indices(self, probs, sizes=None):
         """probs (B,T,C) CUDA -> (labels (B,T) int32, offsets (B,T) int32, counts (B) int32) on the CPU"""
         if not probs.is_cuda:
-            raise _lib.Ds2Error("GreedyDecoder (B200): probs must be a CUDA tensor")
+            raise _lib.Ds2Error("GreedyDecoder: probs must be a CUDA tensor")
         import ctypes as C
         probs = probs.float().contiguous()
         B, T, Cn = probs.shape

@@ -49,7 +49,7 @@ class SpectrogramBatcher:
     def __init__(self, spect_cfg, normalize: bool = True, pad_mode: str = "constant", device="cuda"):
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise _lib.Ds2Error("SpectrogramBatcher (B200): needs a CUDA device; there is no CPU path")
+            raise _lib.Ds2Error("SpectrogramBatcher: needs a CUDA device; there is no CPU path")
         self.n_fft = int(spect_cfg.sample_rate * spect_cfg.window_size)
         self.hop = int(spect_cfg.sample_rate * spect_cfg.window_stride)
         wname = spect_cfg.window.value if hasattr(spect_cfg.window, "value") else str(spect_cfg.window)

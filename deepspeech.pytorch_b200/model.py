@@ -1,5 +1,5 @@
 """DeepSpeech shell: the reference's drop-in seam (deepspeech_pytorch/model.py:138-310) over the
-B200 C-ABI.
+CUDA C-ABI.
 
 Same constructor, attributes, `forward(x, lengths, hs) -> (out, output_lengths, new_hs)` contract,
 Lightning hooks (`training_step`, `validation_step`, `configure_optimizers`) and — because the
@@ -38,7 +38,7 @@ class _Holder(nn.Module):
     """parameter container; `.module` / `.seq_module` attribute names give the reference's keys"""
 
     def forward(self, *a, **k):  # pragma: no cover
-        raise RuntimeError("parameter container of the B200 shell: not callable")
+        raise RuntimeError("parameter container of the CUDA shell: not callable")
 
 
 class _MaskConvParams(_Holder):      # keys conv.seq_module.{0,1,3,4}.*  (model.py:157-164)
@@ -97,7 +97,7 @@ class DeepSpeech(_Base):
         self.conv = _MaskConvParams()
         freq = int(math.floor((spect_cfg.sample_rate * spect_cfg.window_size) / 2) + 1)
         if freq != 161:
-            raise _lib.Ds2Error(f"the B200 front-end kernels are built for 161 frequency bins, got {freq}")
+            raise _lib.Ds2Error(f"the front-end kernels are built for 161 frequency bins, got {freq}")
         rnn_input_size = 32 * 41
         H = model_cfg.hidden_size
         self.rnns = nn.Sequential(
@@ -128,7 +128,7 @@ class DeepSpeech(_Base):
         of the call; the autograd nodes remember it for their backward.  Any other value leaves the process-wide
         switch (`set_precision`) alone."""
         if not x.is_cuda:
-            raise _lib.Ds2Error("DeepSpeech (B200 shell): input must be a CUDA tensor; there is no CPU path")
+            raise _lib.Ds2Error("DeepSpeech (CUDA shell): input must be a CUDA tensor; there is no CPU path")
         if self.precision == 16:
             lib = _lib.get_lib()
             saved = lib.ds2_get_precision()

@@ -70,7 +70,7 @@ def _on_device(fn):
     def wrapped(ctx, *args):
         dev = next((a.device for a in args if isinstance(a, torch.Tensor) and a.is_cuda), None)
         if dev is None:
-            raise _lib.Ds2Error(f"{fn.__qualname__}: no CUDA tensor among the arguments (the B200 path has no CPU "
+            raise _lib.Ds2Error(f"{fn.__qualname__}: no CUDA tensor among the arguments (the CUDA path has no CPU "
                                 "fallback)")
         with torch.cuda.device(dev):
             lib = get_lib()
@@ -111,7 +111,7 @@ _side = {"stream": None, "slot": 0}
 
 def enable_deferred_weight_grads(device=None, enable=True):
     """Let RnnLayer.backward queue dW_ih / dW_hh on a side stream so that they run in the shadow of the next layer's
-    latency-bound sweep (20 of the 148 SMs are idle there).  Effective only for parameters with registered gradient
+    latency-bound sweep (whose pipes are mostly idle; DESIGN.md §5.6).  Effective only for parameters with registered gradient
     sinks (FlatParams(direct_grads=True)): their memory is persistent, and whoever reads the gradients
     (FusedOptimizer.step, OverlappedGradAllReduce) calls `join_deferred()` first.  Run the training loop on a stream
     of higher priority than the side stream (`torch.cuda.Stream(priority=-1)`), otherwise a queued GEMM grid keeps the
@@ -143,7 +143,7 @@ def _req(t, name):
         return None
     if not (t.is_cuda and t.dtype == torch.float32):
         raise _lib.Ds2Error(f"{name}: expected a float32 CUDA tensor, got {t.dtype} on {t.device} "
-                            "(the B200 path has no CPU fallback)")
+                            "(the CUDA path has no CPU fallback)")
     return t if t.is_contiguous() else t.contiguous()
 
 

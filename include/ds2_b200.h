@@ -1,5 +1,5 @@
 /*
- * ds2_b200.h — C-ABI of the B200-native DeepSpeech2 train-step path (libds2_b200.so).
+ * ds2_b200.h — C-ABI of the H100-native DeepSpeech2 train-step path (libds2_b200.so).
  *
  * The reference (SeanNaren/deepspeech.pytorch) has no FFI layer of its own: its hot path is the
  * Python class deepspeech_pytorch/model.py::DeepSpeech calling third-party torch ops.  This header
@@ -20,7 +20,7 @@
  *
  * Precision: DS2_PREC_FP32 = fp32 FFMA everywhere (bit-for-bit independent of tensor cores);
  *            DS2_PREC_TF32 = dense GEMMs (input projections, recurrent products, weight gradients)
- *            on tcgen05 tensor cores with TF32 operands / fp32 accumulation — the same arithmetic
+ *            on wgmma tensor cores with TF32 operands / fp32 accumulation — the same arithmetic
  *            class the reference's stock CUDA path uses (cuDNN allow_tf32=True).
  *            DS2_PREC_F16 = the reference's `precision: 16` (configs/librispeech.yaml:12, torch autocast): the
  *            dense GEMMs of the recurrent stack (input projections, weight gradients, data gradients) take fp16
@@ -56,14 +56,14 @@ enum { DS2_PREC_FP32 = 0, DS2_PREC_TF32 = 1, DS2_PREC_F16 = 2 };
 
 const char* ds2_version(void);
 const char* ds2_last_error(void);
-/* Fails (DS2_ERR_CUDA) when no sm_100 device is usable: there is no CPU fallback. */
+/* Fails (DS2_ERR_CUDA) when no sm_90 (H100) device is usable: there is no CPU fallback. */
 int ds2_device_check(int* sm_count, int* cc_major, int* cc_minor);
 int ds2_set_precision(int prec);
 int ds2_get_precision(void);
 /* Kernel-launch counter (all kernels launched by this library since the last reset). */
 int64_t ds2_launch_count(int reset);
 /* Number of tensor-core-mode recurrent sweeps that had to take the one-launch-per-time-step FFMA kernels
- * because their shape is not eligible for the persistent tcgen05 kernels (also reported once per shape on
+ * because their shape is not eligible for the persistent tensor-core kernels (also reported once per shape on
  * stderr): a benchmark line with a non-zero count did not run the path it claims.                      */
 int64_t ds2_fallback_count(int reset);
 
@@ -221,7 +221,7 @@ int ds2_spectrogram_batch(int n_utts, const float* wave, const int64_t* offsets,
 
 /* ---- dense GEMM used by the blocks above, exported for tests / the roofline bench ------------
  *   C[M,N] = alpha * op(A) op(B) + beta * C ; row-major ; transX: 0 = as stored, 1 = transposed.
- *   Dispatches on ds2_get_precision(): fp32 FFMA kernel or the tcgen05 TF32 kernel.            */
+ *   Dispatches on ds2_get_precision(): fp32 FFMA kernel or the wgmma TF32 kernel.            */
 size_t ds2_gemm_workspace_bytes(int transA, int transB, int M, int N, int K);
 int ds2_gemm(int transA, int transB, int M, int N, int K, float alpha, const float* A, int lda,
              const float* B, int ldb, float beta, float* C, int ldc,

@@ -32,7 +32,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_version_and_error_string():
     lib = ds.get_lib()
-    assert b"sm_100a" in lib.ds2_version()
+    assert b"sm_90a" in lib.ds2_version()
     assert lib.ds2_set_precision(7) != 0
     assert b"precision" in lib.ds2_last_error()
 

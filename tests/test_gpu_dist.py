@@ -2,7 +2,7 @@
 
 Reference semantics (configs/librispeech.yaml:14 `strategy: ddp`, training.py:42-47): every rank computes the
 SUM-reduced CTC loss of its own minibatch, DDP averages the gradients over ranks, BatchNorm running statistics are
-not synchronised and rank 0's are what gets checkpointed.  Two real ranks run the B200 path on their own shard —
+not synchronised and rank 0's are what gets checkpointed.  Two real ranks run the CUDA path on their own shard —
 both processes on cuda:0 over gloo (which moves CUDA tensors) when the box has one GPU, over NCCL on cuda:0 / cuda:1
 when it has two — through `OverlappedGradAllReduce` and the fused optimizer's 1/world scale; the flat gradient must
 equal the oracle's mean of per-shard gradients and the parameters after one fused AdamW step must equal torch AdamW

@@ -1,4 +1,4 @@
-"""-m gpu: the BENCHMARKED kernels (tensor-core mode: tcgen05 GEMMs, fp16-resident split-K sweeps) at the sizes
+"""-m gpu: the BENCHMARKED kernels (tensor-core mode: wgmma GEMMs, fp16-resident split-K sweeps) at the sizes
 BASELINE.json quotes, against the reference's own arithmetic in fp32.
 
 The reference implementation of a BatchRNN layer is `pack_padded_sequence -> nn.LSTM/GRU (cuDNN) ->
@@ -204,7 +204,7 @@ def test_full_model_tf32_logits_within_north_star_bound():
         torch.backends.cudnn.allow_tf32 = saved
     m, l2 = rel(out, ref), rel_l2(out, ref)
     ms, l2s = rel(stock, ref), rel_l2(stock, ref)
-    print(f"\n[fullsize] 5x bi-LSTM-1024 logits vs fp32 reference: B200 path rel {m:.2e} rel-L2 {l2:.2e}; "
+    print(f"\n[fullsize] 5x bi-LSTM-1024 logits vs fp32 reference: CUDA path rel {m:.2e} rel-L2 {l2:.2e}; "
           f"reference's default cuDNN-TF32 path rel {ms:.2e} rel-L2 {l2s:.2e}", flush=True)
     assert m < 1.5e-3 and m < max(1e-3, 2.0 * ms), (m, l2, ms, l2s)
 

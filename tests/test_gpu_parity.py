@@ -220,7 +220,7 @@ def test_adamw_and_sgd_step_match_torch_optim():
         assert rel(p, ref.data) < 1e-5
 
 
-# ---- tensor-core (TF32) mode: tcgen05 GEMMs + persistent recurrent sweeps --------------------------
+# ---- tensor-core (TF32) mode: wgmma GEMMs + persistent recurrent sweeps --------------------------
 # Same arithmetic class as the reference's stock CUDA path (cuDNN allow_tf32): 10-bit operand
 # mantissas, fp32 accumulation.  Tolerances against the fp32 oracle: logits 3e-3 rel (measured ~5e-4);
 # gradients 3e-2 in relative L2 norm and 1e-1 in max-norm (measured ~3e-3 typical; the worst max-norm case,
@@ -277,7 +277,7 @@ def test_tf32_full_size_properties_librispeech_layer():
 
 
 def test_tf32_stress_shape_h1536_one_launch_per_direction():
-    """BASELINE configs[4] layer shape (H=1536, B=8): 2 x 96 CTAs do not fit on 148 SMs, so the persistent sweeps are
+    """BASELINE configs[4] layer shape (H=1536, B=8): 2 x 96 CTAs do not fit on 132 SMs, so the persistent sweeps are
     launched one direction at a time; result must agree with the FFMA step kernels, masked frames stay exactly 0."""
     from deepspeech_pytorch_b200 import _lib
     T, B, In, H = 40, 8, 1536, 1536
@@ -364,8 +364,8 @@ def test_tf32_sweep_variants_agree_with_the_fp32_path(rnn, B, monkeypatch):
 
 @pytest.mark.parametrize("cfg", ["1", "2", "3"])
 def test_gemm_tile_configurations_vs_fp64(cfg, monkeypatch):
-    """128x256x4 stages, 256x256x3 stages (two TMEM accumulators), 128x256x2 stages with two CTAs per SM; K-major and
-    MN-major operands (3-D boxes when the extent is a multiple of 32, 2-D boxes otherwise); TF32 error level."""
+    """128x128 tiles with K in one pass, in 2 and in 4 split-K parts; operands stored K-major and transposed (the
+    latter go through a transpose into the workspace); TF32 error level."""
     monkeypatch.setenv("DS2_GEMM_CFG", cfg)
     ds.set_precision("tf32")
     g = torch.Generator(device="cuda").manual_seed(3)
@@ -378,8 +378,10 @@ def test_gemm_tile_configurations_vs_fp64(cfg, monkeypatch):
         assert rel_l2(c, ref) < 1e-3, (cfg, tA, tB, M, N, K)
 
 
-def test_gemm_split_k_accumulates_into_c():
-    """weight-gradient shape class (64 tiles of 256x256): 2-way split-K with vector atomics, beta = 0 and beta = 1"""
+def test_gemm_split_k_accumulates_into_c(monkeypatch):
+    """weight-gradient shape class: 2-way split-K with vector atomics (opt-in: never chosen by the library itself, whose
+    training step is bit-repeatable), beta = 0 and beta = 1"""
+    monkeypatch.setenv("DS2_GEMM_CFG", "2")
     ds.set_precision("tf32")
     g = torch.Generator(device="cuda").manual_seed(5)
     M, N, K = 4096, 1024, 2304
@@ -470,8 +472,8 @@ def test_deferred_weight_gradient_gemms_give_the_same_gradients():
 
 @pytest.mark.parametrize("cfg", ["1", "2", "3"])
 def test_gemm_f16_tile_configurations_vs_fp64(cfg, monkeypatch):
-    """the precision-16 mode's GEMM (fp16 K-major operands, fp32 accumulation) in every tile configuration, incl. the
-    2-CTAs-per-SM one the short-K projection shape selects, a K tail (K % 64 != 0), split-K and alpha / beta"""
+    """the precision-16 mode's GEMM (fp16 K-major operands, fp32 accumulation) with K in one pass, in 2 and in 4
+    split-K parts, a K tail (K % 64 != 0) and alpha / beta"""
     import ctypes as C
     monkeypatch.setenv("DS2_GEMM16_CFG", cfg)
     lib = ds.get_lib()
@@ -490,10 +492,10 @@ def test_gemm_f16_tile_configurations_vs_fp64(cfg, monkeypatch):
 
 @pytest.mark.parametrize("T,B", [(301, 5), (1000, 3), (301, 4), (640, 6)])
 def test_conv_frontend_tensor_core_paths_vs_fp32(T, B):
-    """tensor-core front-end (conv2 forward / data gradient / weight gradient on tcgen05, TF32) against the FFMA
-    front-end on a ragged batch: several 128-position tiles per row, a partially filled last tile, fully masked tiles,
-    BatchNorm batch statistics (running stats) from the fused partial sums; masked frames exactly zero.  Odd batches
-    run one CTA per tile, even ones the 2-CTA clusters that share the tap matrices by multicast."""
+    """tensor-core front-end (conv2 forward / data gradient / weight gradient on wgmma, TF32) against the FFMA
+    front-end on a ragged batch: several 64-position tiles per row, a partially filled last tile, fully masked tiles,
+    BatchNorm batch statistics (running stats) from the fused partial sums; masked frames exactly zero; odd and even
+    batch sizes."""
     g = torch.Generator().manual_seed(T)
     x = torch.randn(B, 1, 161, T, generator=g)
     lens = sorted([max(40, T - (T // 4) * i) for i in range(B)], reverse=True)
