@@ -138,16 +138,23 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
     // accumulator (position pl, column (kw, co)) feeds output pl - kw.  One kw at a time (the two warpgroups hold
     // different column blocks; inside a block every output has one contributor): the sum over kw always runs in the
     // same order, so the result is bit-repeatable.
+    // The 8-column block i of warpgroup wg holds tap column kw = (22 wg + i) / 4 (a block never straddles two taps), so
+    // with kw and i unrolled each pass touches only the (at most 4) blocks of its own tap instead of testing all 88
+    // accumulators: the epilogue runs while the tensor cores of the SM idle, so its instruction count is paid per CTA.
     const int w = warp % 4;
+#pragma unroll
     for (int kw = 0; kw < KW; ++kw) {
 #pragma unroll
       for (int i = 0; i < NN / 16; ++i) {
+        const bool in0 = (i >> 2) == kw, in1 = ((NN / 16 + i) >> 2) == kw;   // block i of warpgroup 0 / 1 is tap kw
+        if (!in0 && !in1) continue;
+        if (wg == 0 ? !in0 : !in1) continue;
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int pl = 16 * w + (lane >> 2) + 8 * (e >> 1);
           const int n = NN / 2 * wg + 8 * i + 2 * (lane & 3) + (e & 1);
           const int to = pl - kw;
-          if (n / CH == kw && to >= 0 && to < TO) out_s[to * OUT_LD + n % CH] += acc[4 * i + e];
+          if (to >= 0 && to < TO) out_s[to * OUT_LD + n % CH] += acc[4 * i + e];
         }
       }
       asm volatile("bar.sync 1, 256;" ::: "memory");
