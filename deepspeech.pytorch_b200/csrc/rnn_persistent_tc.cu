@@ -72,6 +72,8 @@ struct PersistParams {
                         // when both together would not be co-resident, e.g. H = 1536)
   float* dbias[2];      // split-K bwd: bias-gradient accumulators (G*H per direction, zeroed by the host) or null
   float* dbias_hn[2];   // split-K bwd, GRU: sum of dGh_n (H per direction)
+  float* xbuf;          // split-K bwd, exchange through L2: [CTA][source rank][step parity] partial dh_rec tiles
+  unsigned int* xcnt;   //   ... [CTA] number of partial tiles received (monotonic, zeroed by the host)
   int* err;             // set to 1 if a barrier wait timed out
 };
 
@@ -623,13 +625,12 @@ static size_t fwd_smem_bytes(int NB) {
          (2 * STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
+static size_t splitk_res_ws_bytes(int G, int T, int B, int H, int D);
+
 size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
   const int G = rnn == DS2_RNN_LSTM ? 4 : (rnn == DS2_RNN_GRU ? 3 : 1);
   const size_t fwd = 4096 + align_up((size_t)D * G * H * H * 2, 256) + align_up((size_t)D * T * B * H * 2, 256);
-  const size_t GH = (size_t)G * H;
-  const size_t bwd = 4096 + align_up((size_t)D * (T + 1) * 4, 256) + align_up((size_t)T * 4, 256) +
-                     align_up((size_t)D * T * (H / 16 + 1) * 4 * 4, 256) + align_up((size_t)D * H * GH * 2, 256) +
-                     align_up((size_t)T * B * D * GH * 2, 256);   // >= splitk_res_ws_bytes()
+  const size_t bwd = splitk_res_ws_bytes(G, T, B, H, D);
   return (fwd > bwd ? fwd : bwd) + 256;
 }
 
@@ -1028,6 +1029,13 @@ __device__ __forceinline__ void st_async_v4(uint32_t cluster_addr, float a, floa
                "f"(a), "f"(b), "f"(c), "f"(d), "r"(cluster_bar)
                : "memory");
 }
+// 1-D bulk copy global -> this CTA's shared memory that counts its bytes on an mbarrier (16-byte aligned, size % 16 == 0)
+__device__ __forceinline__ void bulk_load(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
+                   tc::smem_u32(smem_dst)),
+               "l"(src), "r"(bytes), "r"(tc::smem_u32(bar))
+               : "memory");
+}
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
@@ -1053,11 +1061,17 @@ __device__ __forceinline__ float pow2f(int ex) { return __int_as_float((ex + 127
 // number of CTAs, but each reduces only K/8, i.e. half as many MMA instructions on the per-step critical path).
 // LL (RES only): no grid barrier; the scaled fp16 gate gradients are their own ready flags (see the LL helpers) and
 // the per-step maxima travel as one word per (CTA, epilogue warp) in `gmeta`.
-template <int RNN, bool RES, int CL, bool LL = false, int NKR_T = 0>   // NKR_T: see rnn_fwd_splitk_kernel
+// XG (RES, CL = 4 only): launched without clusters, as plain cooperative CTAs; a group of CL consecutive CTAs keeps
+// the roles of a cluster, but the partial dh_rec tiles travel through L2 (`xbuf`, counted in `xcnt`) instead of
+// distributed shared memory.  For GPUs whose GPCs cannot hold every cluster of the grid at once (a 132-SM H100 with
+// both directions of H = 1024: 32 clusters of 4), so that both directions still run in one launch.  The MMAs, sums
+// and scales are the cluster path's: the results are bit-identical.
+template <int RNN, bool RES, int CL, bool LL = false, int NKR_T = 0, bool XG = false>   // NKR_T: see rnn_fwd_splitk_kernel
 __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __grid_constant__ PersistParams p) {
   using namespace rp;
   using namespace tc;
   static_assert(!LL || RES, "the flag-in-data exchange streams the fp16 copy of the resident variant");
+  static_assert(!XG || (RES && !LL && CL == 4), "the L2 exchange is built for the resident 4-CTA variant");
   constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
   constexpr int UM = UT * CL;                  // units per cluster (all M rows valid): 64 or 128 = MMA M
   constexpr int A_BYTES = UM * 128;            // one K chunk of the weight tile (shadows rp::A_BYTES)
@@ -1091,6 +1105,11 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
   const int u0 = ut * UM + ks * UT;                       // the 16 units this CTA finishes
   unsigned int* ctr = p.bar + 32 * d;
   const unsigned int n_arrive = (unsigned int)(NTc * CL);
+  const int ss = xt_slice(UT, NB);                        // floats of one partial tile
+  // XG: CTA index over both directions (the directions may be launched one at a time); tile (cta, source, parity)
+  // of xbuf holds what `source` computed for `cta`'s units in a step of that parity
+  const int grp0 = (d * NTc + ut) * CL;
+  auto xslot = [&](int cta, int src, int step) { return p.xbuf + ((size_t)(cta * CL + src) * 2 + (step & 1)) * ss; };
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmW[d]);
@@ -1098,7 +1117,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
     for (int i = 0; i < (RES ? 32 : STAGES); ++i) mbar_init(&full[i], LL ? 4 : 1);   // LL: one arrival per loader warp
     for (int i = 0; i < STAGES; ++i) mbar_init(&empty[i], RES ? 1 : 128);   // streaming: every MMA-warpgroup thread arrives
     mbar_init(accum_bar, 1);
-    mbar_init(part_bar, 1);
+    mbar_init(part_bar, XG ? 2 : 1);                     // XG: the producer's bulk copies + the warp that kept its rows
     fence_barrier_init();
     cta_max[0] = 0u;
     for (int i = 0; i < 8; ++i) wmax[i] = 0u;
@@ -1114,7 +1133,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
     fence_proxy_async();
   }
   __syncthreads();
-  cluster_sync_all();                                     // peers' mbarriers are initialised
+  if constexpr (!XG) cluster_sync_all();                 // peers' mbarriers are initialised
   const uint32_t tx_bytes = (uint32_t)(UM * 128 + B * 128);
 
   if (warp == 8) {                                        // TMA producer
@@ -1148,6 +1167,19 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
             }
           }
           trace_stamp(p.trace, p.T, step, 1);
+          if constexpr (XG) {
+            // The CL - 1 partial tiles the other CTAs of the group send for this step: wait for them (relaxed polling,
+            // then an acquire fence, as at the step barrier) and copy them into `part` with bulk copies that complete
+            // on part_bar.  The epilogue read `part` of the previous step before its arrival at the barrier passed
+            // above.  Two parities of xbuf are enough: a source writes the tile of step s + 2 only after its MMAs of
+            // step s + 2, i.e. after every CTA of the direction arrived at the barrier that ends step s + 1, and this
+            // CTA's arrival there follows the copies of step s (its epilogue waited for them on part_bar).
+            grid_wait_counter(p.xcnt + grp0 + ks, (unsigned int)((CL - 1) * step), p.err);
+            fence_proxy_async_global();
+            mbar_arrive_expect_tx(part_bar, (uint32_t)((CL - 1) * ss * 4));
+            for (int src = 0; src < CL; ++src)
+              if (src != ks) bulk_load(part + src * ss, xslot(grp0 + ks, src, step), (uint32_t)(ss * 4), part_bar);
+          }
         }
       }
     } else
@@ -1249,8 +1281,8 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
     // split with lane+16 by shuffle.  M = 128 (CL 8): lane l of quarter q holds row 32q+l -> CTA 2q + l/16, all 32
     // columns of the row are sent by that lane.
     const int dst_cta = CL == 4 ? q : 2 * q + half;
-    const uint32_t dst_row = mapa_u32(smem_u32(part), (uint32_t)dst_cta) + (uint32_t)(ks * xt_slice(UT, NB) * 4);
-    const uint32_t dst_bar = mapa_u32(smem_u32(part_bar), (uint32_t)dst_cta);
+    const uint32_t dst_row = XG ? 0u : mapa_u32(smem_u32(part), (uint32_t)dst_cta) + (uint32_t)(ks * ss * 4);
+    const uint32_t dst_bar = XG ? 0u : mapa_u32(smem_u32(part_bar), (uint32_t)dst_cta);
     const uint32_t part_tx = (uint32_t)(CL * UT * NB * 4);               // bytes this CTA receives per step
     // resident: s_cur scales what this step writes, s_prev un-scales what this step's MMAs consumed
     const unsigned int* gmax_d = RES ? p.gmax + (size_t)d * (T + 1) : nullptr;
@@ -1342,7 +1374,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
       bool pvalid = false;
       if (single) load_coefs(b_own, kc, pdy, pvalid);
       if (step > 0) {
-        if (e == 0) mbar_arrive_expect_tx(part_bar, part_tx);   // arm this step's phase (peers may already have sent)
+        if (!XG && e == 0) mbar_arrive_expect_tx(part_bar, part_tx);   // arm this step's phase (peers may already have sent)
         // send this CTA's partial tile: row (16q + ul), 32 columns split over the two half-warps
         mbar_wait(accum_bar, acc_phase);
         if (RES) {
@@ -1362,6 +1394,8 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
           inv_prev = pow2f(-sx_prev);
         }
         if (e == 0) trace_stamp(p.trace, p.T, step, 5);
+        // XG: own rows straight into the own tile, the other CTAs' rows into xbuf
+        float* const xdst = XG ? (q == ks ? part + ks * ss : xslot(grp0 + q, ks, step)) : nullptr;
         for (int cb = 0; cb < NB; cb += 32) {
           float acc[32];
           tmem_ld32(acc_img, acc_pitch(NB), ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
@@ -1375,8 +1409,12 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
               const int c0 = cb + half * 16 + 4 * i;      // NB is a multiple of 8: a group of 4 columns is in or out
-              if (c0 < NB)
+              if (c0 >= NB) continue;
+              if constexpr (XG) {
+                *reinterpret_cast<float4*>(xdst + xt_off(UT, ul, c0)) = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+              } else {
                 st_async_v4(dst_row + (uint32_t)(xt_off(UT, ul, c0) * 4), v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3], dst_bar);
+              }
             }
           } else {
 #pragma unroll
@@ -1389,6 +1427,20 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         }
         acc_phase ^= 1;
         if (e == 0) trace_stamp(p.trace, p.T, step, 6);
+        if constexpr (XG) {
+          // Publish: the warp's stores happen-before lane 0's release (bar.warp.sync orders memory among the lanes);
+          // a destination counts one arrival per source CTA and step.  The warp that kept its rows arrives on
+          // part_bar instead.
+          __syncwarp();
+          if (lane == 0) {
+            if (q == ks) {
+              mbar_arrive(part_bar);
+            } else {
+              fence_proxy_async_global();
+              red_release(p.xcnt + grp0 + q, 1u);
+            }
+          }
+        }
         mbar_wait_cluster(part_bar, part_phase, p.err);   // all CL slices of this CTA's units have landed
         part_phase ^= 1;
       }
@@ -1428,7 +1480,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
           float rec = 0.f;
           if (step > 0) {
             const float* pr = part + xt_off(UT, uq + j, b);
-            const int ss = xt_slice(UT, NB);
             rec = (pr[0] + pr[ss]) + (pr[2 * ss] + pr[3 * ss]);
             if (CL == 8) rec += (pr[4 * ss] + pr[5 * ss]) + (pr[6 * ss] + pr[7 * ss]);
           }
@@ -1630,7 +1681,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
     }
   }
   __syncthreads();
-  cluster_sync_all();                                     // nobody exits while a peer may still read its tile
+  if constexpr (!XG) cluster_sync_all();                 // nobody exits while a peer may still read its tile
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2137,11 +2188,18 @@ static size_t splitk_res_smem_bytes(int NB, int Kc, int CL) {
 }
 // workspace of the resident backward: [4 KB control][gmax D*(T+1) uints][W^T fp16: D*H*GH][dg16: T*B*D*GH]
 // (+ [dymax: T uints][gmeta: D*T*(H/16)*4 uints] after gmax: H/16 CTAs per direction, 4 epilogue warps each)
+// (+ [xbuf: D*H/16 CTAs x 4 sources x 2 parities partial tiles] after dg16: the 4-CTA L2 exchange)
+// The control block holds err (offset 0), the step counters (128) and the L2 exchange's xcnt (1024: <= 768 CTAs).
+constexpr size_t XCNT_OFFSET = 1024;
+constexpr int XCNT_MAX = (4096 - (int)XCNT_OFFSET) / 4;
+static size_t splitk_xbuf_bytes(int B, int H, int D) {
+  return (size_t)D * (H / 16) * 4 * 2 * xt_slice(rp::UT, (B + 31) / 32 * 32) * sizeof(float);
+}
 static size_t splitk_res_ws_bytes(int G, int T, int B, int H, int D) {
   const size_t GH = (size_t)G * H;
   return 4096 + align_up((size_t)D * (T + 1) * 4, 256) + align_up((size_t)T * 4, 256) +
          align_up((size_t)D * T * (H / 16) * 4 * 4, 256) + align_up((size_t)D * H * GH * 2, 256) +
-         align_up((size_t)T * B * D * GH * 2, 256);
+         align_up((size_t)T * B * D * GH * 2, 256) + align_up(splitk_xbuf_bytes(B, H, D), 256);
 }
 
 template <int RNN, int CL, bool LL>
@@ -2179,16 +2237,30 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
   const size_t gmeta_bytes = (size_t)a.D * a.T * (a.H / 16) * 4 * 4;
   off += align_up(gmeta_bytes, 256);
   __half* wT16 = reinterpret_cast<__half*>(base + off); off += align_up((size_t)a.D * a.H * GH * 2, 256);
-  p.dg16 = reinterpret_cast<__half*>(base + off);
+  p.dg16 = reinterpret_cast<__half*>(base + off); off += align_up((size_t)a.T * a.B * a.D * GH * 2, 256);
+  p.xbuf = reinterpret_cast<float*>(base + off);
+  p.xcnt = reinterpret_cast<unsigned int*>(base + XCNT_OFFSET);
   const size_t smem = one_cta_per_sm(splitk_res_smem_bytes(p.NB, GH / CL, CL));
   if (smem > 227 * 1024) return 1;
+  // DS2_SPLITK_XCHG=cluster|global: force the partial-tile exchange through distributed shared memory or through L2
+  const char* xe = getenv("DS2_SPLITK_XCHG");
+  const bool force_cluster = xe && !strcmp(xe, "cluster"), force_global = xe && !strcmp(xe, "global");
+  if (force_global && (CL != 4 || LL)) return 1;   // only the 4-CTA non-LL variant has the L2 exchange
   // H = 1024 (the BASELINE shapes): compile-time chunk count -> unrolled issue loop
   constexpr int NKU = (G * 1024 / CL) / 64;   // chunks per CTA at H = 1024: 16 / 12 / 4 (CL 4), 8 / 6 / 2 (CL 8)
+  constexpr bool HAS_XG = CL == 4 && !LL;
   auto kern = (!LL && a.H == 1024) ? rnn_bwd_splitk_kernel<RNN, true, CL, LL, NKU> : rnn_bwd_splitk_kernel<RNN, true, CL, LL, 0>;
+  auto kern_xg = kern;
+  if constexpr (HAS_XG)
+    kern_xg = a.H == 1024 ? rnn_bwd_splitk_kernel<RNN, true, CL, false, NKU, true> : rnn_bwd_splitk_kernel<RNN, true, CL, false, 0, true>;
   static DeviceOnce attr_once;
-  if (attr_once.first()) {   // BOTH instantiations (see the forward launcher)
+  if (attr_once.first()) {   // ALL instantiations (see the forward launcher)
     DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, LL, NKU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, LL, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    if constexpr (HAS_XG) {
+      DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, false, NKU, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+      DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, false, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    }
     attr_once.done();
   }
   int grid = a.D * p.NT * CL, launches = 1;
@@ -2209,10 +2281,31 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
   int max_clusters = 0;
   cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg);
   if (oe != cudaSuccess) { (void)cudaGetLastError(); return 1; }
-  if (max_clusters * CL < grid) {
+  // Path, from what the device reports: (1) every cluster of the grid co-resident: cluster exchange, one launch.
+  // (2) Otherwise the plain cooperative grid co-resident (a cluster cannot span two GPCs, so clusters of 4 can fail
+  // where single CTAs fit: 32 clusters of 4 on a 132-SM H100): L2 exchange, one launch.  (3) Otherwise one launch
+  // per direction with the cluster exchange.
+  bool xg = false;
+  int fit = max_clusters * CL;                           // CTAs of the chosen path that can be co-resident
+  if (force_global || (fit < grid && !force_cluster)) {
+    if constexpr (HAS_XG) {
+      int per_sm = 0;
+      DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern_xg, THREADS, smem));
+      const int resident = per_sm * device_sm_count();
+      if (grid <= XCNT_MAX && (resident >= grid || force_global)) {
+        xg = true;
+        fit = resident;
+        kern = kern_xg;
+        cfg.attrs = attrs + 1;                           // cooperative, no cluster dimension
+        cfg.numAttrs = 1;
+      }
+    }
+    if (force_global && !xg) return 1;
+  }
+  if (fit < grid) {
     // 8-CTA clusters are only worth it when both directions run concurrently (otherwise the two directions run
     // back to back)
-    if (CL == 8 || max_clusters * CL < p.NT * CL) return 1;
+    if (CL == 8 || fit < p.NT * CL) return 1;
     grid = p.NT * CL;
     launches = a.D;
     cfg.gridDim = dim3(grid);

@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""Per-kernel device time of the conv front-end in the benchmarked train step.
+"""Per-kernel device time of one block of the benchmarked train step: the conv front-end or the recurrent layers.
 
-    python tools/profile_frontend.py [--workload librispeech] [--steps 3] [--warmup 3] [--precision fp16]
-                                     [--json OUT.json]
+    python tools/profile_frontend.py [--block conv|rnn] [--workload librispeech] [--steps 3] [--warmup 3]
+                                     [--precision fp16] [--json OUT.json]
 
 Builds the model, batch, precision mode and side stream exactly as `bench.py` does, warms up, then runs a few steps
-under `torch.profiler` (CUDA activities).  Every kernel / memset launched from inside `ds2_conv_frontend_fwd` or
-`ds2_conv_frontend_bwd` is attributed to that call through the launch's correlation id, and its device time is
-summed per step and per stream (the main stream and the side stream the conv2 weight gradient runs on are shown
-separately).  The card name and power limit are read in the same run.  Times under the profiler include its own
+under `torch.profiler` (CUDA activities).  Every kernel / memset launched from inside the block's library calls
+(`ds2_conv_frontend_fwd` / `_bwd`, or `ds2_rnn_layer_fwd` / `_bwd` for all layers) is attributed to that call
+through the launch's correlation id, and its device time and launch count are summed per step and per stream (the
+main stream and the side stream the weight gradients run on are shown separately).  The card name and power limit are read in the same run.  Times under the profiler include its own
 overhead per launch; step times come from `bench.py`, not from here.
 """
 import argparse
@@ -24,7 +24,8 @@ sys.path.insert(0, ROOT)
 
 from bench import WORKLOADS, synth_batch  # noqa: E402
 
-TAGS = {"ds2_conv_frontend_fwd": "conv_fwd", "ds2_conv_frontend_bwd": "conv_bwd"}
+BLOCKS = {"conv": {"ds2_conv_frontend_fwd": "conv_fwd", "ds2_conv_frontend_bwd": "conv_bwd"},
+          "rnn": {"ds2_rnn_layer_fwd": "rnn_fwd", "ds2_rnn_layer_bwd": "rnn_bwd"}}
 
 
 def card_info():
@@ -39,6 +40,7 @@ def card_info():
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--block", default="conv", choices=sorted(BLOCKS))
     ap.add_argument("--workload", default="librispeech", choices=sorted(WORKLOADS))
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
@@ -53,6 +55,8 @@ def main():
     from deepspeech_pytorch_b200.optim import FlatParams, FusedOptimizer
 
     assert torch.cuda.is_available(), "profile_frontend.py needs a GPU"
+    tags = BLOCKS[args.block]
+    fwd_tag = next(iter(tags.values()))
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     lib = ds.get_lib()
@@ -73,8 +77,8 @@ def main():
     x_dev = x.to(dev)
     targets_pinned = targets.pin_memory()
 
-    # mark the two front-end calls with profiler ranges (the ctypes attributes are looked up at call time)
-    for sym, tag in TAGS.items():
+    # mark the block's library calls with profiler ranges (the ctypes attributes are looked up at call time)
+    for sym, tag in tags.items():
         fn = getattr(lib, sym)
 
         def wrapped(*a, _fn=fn, _tag=tag):
@@ -107,7 +111,7 @@ def main():
 
     ev = trace["traceEvents"] if isinstance(trace, dict) else trace
     ranges = [(e["ts"], e["ts"] + e["dur"], e["tid"], e["name"]) for e in ev
-              if e.get("ph") == "X" and e.get("cat") == "user_annotation" and e.get("name") in TAGS.values()]
+              if e.get("ph") == "X" and e.get("cat") == "user_annotation" and e.get("name") in tags.values()]
     corr_tag = {}
     for e in ev:
         if e.get("ph") != "X" or e.get("cat") not in ("cuda_runtime", "cuda_driver"):
@@ -130,17 +134,17 @@ def main():
         table[key][1] += 1
     fwd_streams = defaultdict(float)
     for (tag, stream, _), (us, _) in table.items():
-        if tag == "conv_fwd":
+        if tag == fwd_tag:
             fwd_streams[stream] += us
     main_id = max(fwd_streams, key=fwd_streams.get) if fwd_streams else None
 
     rows = []
-    for (tag, stream, name), (us, cnt) in sorted(table.items(), key=lambda kv: (kv[0][0] != "conv_fwd",
+    for (tag, stream, name), (us, cnt) in sorted(table.items(), key=lambda kv: (kv[0][0] != fwd_tag,
                                                                                  kv[0][1] != main_id, -kv[1][0])):
         rows.append({"block": tag, "stream": "main" if stream == main_id else f"side({stream})", "kernel": name,
                      "ms_per_step": us / 1e3 / args.steps, "launches_per_step": cnt / args.steps})
     print(f"card: {card}")
-    print(f"workload {args.workload}, precision {args.precision}, {args.steps} profiled steps (device time per step, "
+    print(f"block {args.block}, workload {args.workload}, precision {args.precision}, {args.steps} profiled steps (device time per step, "
           f"under the profiler)")
     print(f"{'block':9s} {'stream':10s} {'ms/step':>8s} {'launches':>8s}  kernel")
     totals = defaultdict(float)
@@ -151,7 +155,7 @@ def main():
         print(f"total {blk} on {stream}: {ms:.3f} ms/step")
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
-        json.dump({"card": card, "workload": args.workload, "precision": args.precision, "steps": args.steps,
+        json.dump({"card": card, "block": args.block, "workload": args.workload, "precision": args.precision, "steps": args.steps,
                    "rows": rows}, open(args.json, "w"), indent=1)
 
 
