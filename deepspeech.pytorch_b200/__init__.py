@@ -3,8 +3,8 @@
 registers the package under that importable name)."""
 from . import _lib
 from ._lib import Ds2Error, get_lib
-from .configs import (AdamConfig, BiDirectionalConfig, DataConfig, OptimConfig, SGDConfig, SpectConfig,
-                      UniDirectionalConfig)
+from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, OptimConfig, SGDConfig,
+                      SpectConfig, UniDirectionalConfig)
 from .enums import DecoderType, RNNType, SpectrogramWindow
 from .labels import LABELS
 

@@ -50,6 +50,8 @@ PROTOTYPES = {
     "ds2_greedy_decode": (i32, [i32, i32, i32, vp, vp, i32, vp, vp, vp, vp]),
     "ds2_spectrogram_workspace_bytes": (sz, [i32]),
     "ds2_spectrogram_batch": (i32, [i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, vp, i32, vp, sz, vp]),
+    "ds2_spec_augment_workspace_bytes": (sz, [i32]),
+    "ds2_spec_augment": (i32, [i32, i32, i32] + [vp] * 5 + [sz, vp]),
     "ds2_optim_workspace_bytes": (sz, []),
     "ds2_adamw_step": (i32, [i64] + [vp] * 4 + [f32] * 5 + [i32, f32, f32, vp, vp, vp]),
     "ds2_sgd_nesterov_step": (i32, [i64] + [vp] * 3 + [f32] * 3 + [i32, f32, f32, vp, vp, vp]),

@@ -219,6 +219,36 @@ int ds2_spectrogram_batch(int n_utts, const float* wave, const int64_t* offsets,
                           int max_samples, int n_fft, int hop, const float* window, int pad_reflect, int normalize,
                           float* out, int Tmax, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- input pipeline: SpecAugment on a padded spectrogram batch ----------------------------------
+ * Replaces, per utterance, spec_augment (loader/spec_augment.py:68-115 with sparse_image_warp.py:88-410, the
+ * reference's defaults), which SpectrogramParser.parse_audio (data_loader.py:161-163) applies to each normalised
+ * (F, T) spectrogram before collation:
+ *   time warp   control point c = (F/2, fp32(p + d)) with p = in[u, F/2, idx] (the VALUE is used as the time
+ *               coordinate), x-flow fx = fp32(c1 - p); order-2 polyharmonic fit [[0, b^T], [b, Z]] [w; v] =
+ *               [fx; 0], b = (c0, c1, 1); dense x-flow phi(r) w + v0 j + v1 i + v2 with phi(r) = r log(r) / 2 and
+ *               r = sum over the whole (F, T) grid of (j^2 + i^2) - 2 (j c0 + i c1) + |c|^2; the y-flow is 0.
+ *               Output (j, i) is the bilinear sample at (j, i - flow), floor clamped to [0, size - 2] and alpha
+ *               to [0, 1] on the utterance's own width T; the last row takes alpha_y = 1.
+ *   masks       rows [f0, f0 + f) and frames [t0, t0 + t) become 0 (width 0: no mask).
+ * The random numbers are the caller's (deepspeech_pytorch_b200.input_pipeline.spec_augment_draws draws them from
+ * python's `random`, numpy and torch in the reference's order).
+ *   in, out   (n_utts, 1, F, Tmax) fp32, must not overlap; frames t >= frames[u] of `out` are written as 0
+ *   frames    int32 frame count T of each utterance (device), 11 <= T <= Tmax
+ *   draws     one Ds2SpecAugDraws per utterance (device)
+ * Deterministic: no atomics, the same inputs give bit-identical outputs.                                   */
+typedef struct {
+  int32_t idx;  /* random.randrange(5, T - 5): the frame whose row-F/2 value is the control point's time   */
+  int32_t d;    /* random.randrange(-5, 5): the warp distance                                              */
+  int32_t f0, f; /* frequency mask: rows [f0, f0 + f)                                                      */
+  int32_t t0, t; /* time mask: frames [t0, t0 + t); t = 0 when the reference skipped it                    */
+  float Z[9];   /* torch.randn((1, 3, 3)) / 1e10, row-major                                               */
+  int32_t reserved;
+} Ds2SpecAugDraws;
+
+size_t ds2_spec_augment_workspace_bytes(int n_utts);
+int ds2_spec_augment(int n_utts, int F, int Tmax, const float* in, const int32_t* frames,
+                     const Ds2SpecAugDraws* draws, float* out, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- dense GEMM used by the blocks above, exported for tests / the roofline bench ------------
  *   C[M,N] = alpha * op(A) op(B) + beta * C ; row-major ; transX: 0 = as stored, 1 = transposed.
  *   Dispatches on ds2_get_precision(): fp32 FFMA kernel or the wgmma TF32 kernel.            */
