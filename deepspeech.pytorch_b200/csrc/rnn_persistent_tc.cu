@@ -1,22 +1,22 @@
 // Persistent, warp-specialised recurrent sweeps on wgmma tensor cores.
 //
-// One launch per layer covers ALL time steps and both directions.  A CTA owns 16 hidden units of
-// one direction: the G*16 rows of W_hh for those units form the M=64 operand of
+// One launch per layer covers ALL time steps and, when the GPU holds both, both directions.  Per step a CTA computes
 //     acc[(g,u), b] = sum_k W_hh[g*H+u, k] * h_{t-1}[b, k]        (wgmma, tf32 or f16, N = batch)
-// with fp32 accumulators.  Per step:
-//   warp 0   TMA producer: weight chunks (3-D box over [gate][unit][k], prefetched ahead of the
-//            barrier because they do not depend on it) and h_{t-1} chunks (after the grid barrier)
-//            into an 8-stage 128B-swizzled shared-memory ring
-//   warps 8-11 MMA warpgroup: wgmma into registers, then the accumulator image in shared memory -> mbarrier
-//   warps 2-5 epilogue: accumulator image -> registers, + input projection + biases, gate non-linearities spread
-//            over 64 lanes, exchange through shared memory, cell update (c / h state stays in shared
-//            memory for the whole sweep), masked stores of h_t (and the saved tensors for backward)
-// Steps are separated by a per-direction grid barrier (monotonic counter in global memory, release /
-// acquire, bounded spin so that a fault cannot hang the GPU).  All CTAs must be co-resident: the host
-// checks occupancy and launches cooperatively; shapes that do not fit return 1 (FFMA step kernels).
+// for its hidden units with fp32 accumulators.  288 threads per CTA (rp::THREADS):
+//   warp 8     TMA producer: weight chunks and h_{t-1} chunks (after the grid barrier) into 128B-swizzled shared
+//              memory, either a ring of STAGES chunks (streaming variants) or, in the resident variants, the whole
+//              fp16 weight slice once and the fp16 h_{t-1} per step
+//   warps 4-7  MMA warpgroup: wgmma into registers, then the accumulator image in shared memory -> mbarrier
+//   warps 0-3  epilogue: accumulator image -> registers, + input projection + biases, gate non-linearities,
+//              cell update (c / h state stays in shared memory for the whole sweep), masked stores of h_t (and
+//              the saved tensors for backward)
+// Steps are separated by a per-direction grid barrier (monotonic counter in global memory, release / acquire,
+// bounded spin so that a fault cannot hang the GPU).  All CTAs of a launch must be co-resident: launch_sweep checks
+// occupancy and launches cooperatively; shapes that do not fit return 1 (FFMA step kernels).
 //
-// Backward sweep: the same skeleton on W_hh^T with split-K over the gates inside a 4-CTA cluster
-// (partial sums reduced through distributed shared memory) — see rnn_bwd_persist_kernel.
+// Kernels: rnn_fwd_persist_kernel (16 units per CTA), rnn_fwd_splitk_kernel (2-CTA clusters split K = H),
+// rnn_bwd_persist_kernel (16 units per CTA on W_hh^T) and rnn_bwd_splitk_kernel (4- or 8-CTA groups split
+// K = G*H; the partial sums travel through distributed shared memory or, with XG, through L2).
 #include <cooperative_groups.h>
 #include <cuda_fp16.h>
 #include <dlfcn.h>
@@ -57,7 +57,6 @@ struct PersistParams {
   __half* dgn16T;       //   ... transposed (D*G*H, T*B)
   __half* auxn16T;      //   ... GRU h-side n-gate gradient, transposed (D*H, T*B)
   const float* nscale;  //   device: power-of-two scale of those copies
-  unsigned int* gmeta;  // LL bwd: [D][T][NT*CL*4] float bits of max|dGh| per (step, epilogue warp), 0xFFFFFFFF = not yet
   long long* trace;     // optional: clock64 stamps of CTA 0, 4 per step
   const int32_t* len;
   float* gates;
@@ -66,7 +65,6 @@ struct PersistParams {
   const float* b_ih[2];
   const float* b_hh[2];
   unsigned int* bar;    // [2][NT] per-CTA step flags (zeroed by the host): flag = number of finished steps
-  int nacc, acc_cols;   // independent accumulator chains (K is dealt round-robin over them)
   int defer;            // 1: stores that only later kernels read are issued after the barrier arrival
   int d0;               // first direction handled by this launch (directions can be launched one at a time
                         // when both together would not be co-resident, e.g. H = 1536)
@@ -77,11 +75,6 @@ struct PersistParams {
   int* err;             // set to 1 if a barrier wait timed out
 };
 
-__device__ __forceinline__ unsigned int ld_acquire(const unsigned int* p) {
-  unsigned int v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
 __device__ __forceinline__ void red_release(unsigned int* p, unsigned int v) {
   asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
@@ -93,39 +86,14 @@ __device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence
 
 // The waits below only set *err on a timeout (sweep_check_kernel reports it after the launch): a device printf is
 // a function call, and a call anywhere in a kernel makes ptxas serialise every wgmma of that kernel.
-// Grid barrier of one direction: every CTA publishes the number of steps it has finished in its own
-// 4-byte flag (plain release store, no atomic serialisation); a whole warp polls all NT flags
-// (coalesced acquire loads) until each is >= target.  Bounded spin: a fault cannot hang the GPU.
 __device__ __forceinline__ unsigned int ld_relaxed(const unsigned int* p) {
   unsigned int v;
   asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ void grid_wait_flags(const unsigned int* flags, int nt, unsigned int target, int* err) {
-  const int lane = threadIdx.x % 32;
-  const long long t0 = clock64();
-  unsigned int it = 0;
-  for (;;) {
-    // up to 4 independent loads in flight per lane (nt <= 128 flags per direction), relaxed polling
-    unsigned int v0 = lane < nt ? ld_relaxed(flags + lane) : target;
-    unsigned int v1 = lane + 32 < nt ? ld_relaxed(flags + lane + 32) : target;
-    unsigned int v2 = lane + 64 < nt ? ld_relaxed(flags + lane + 64) : target;
-    unsigned int v3 = lane + 96 < nt ? ld_relaxed(flags + lane + 96) : target;
-    bool ok = v0 >= target && v1 >= target && v2 >= target && v3 >= target;
-    for (int i = lane + 128; i < nt; i += 32) ok = ok && (ld_relaxed(flags + i) >= target);
-    if (__all_sync(0xffffffffu, ok)) break;
-    if ((++it & 63u) == 0) {
-      if (*(volatile int*)err) return;
-      if (clock64() - t0 > rp::SPIN_LIMIT) {
-        *(volatile int*)err = 1;
-        return;
-      }
-    }
-  }
-  asm volatile("fence.acq_rel.gpu;" ::: "memory");   // acquire side of the flag protocol
-}
-// single-thread variant on a monotonically increasing arrival counter
-// (relaxed polling loads, then one acquire fence: an acquire load would invalidate L1 on every poll)
+// Grid barrier of one direction: every CTA adds 1 per finished step to a monotonic arrival counter (red.release);
+// one thread waits until it reaches target (relaxed polling loads, then one acquire fence: an acquire load would
+// invalidate L1 on every poll).  Bounded spin: a fault cannot hang the GPU.
 __device__ __forceinline__ void grid_wait_counter(const unsigned int* ctr, unsigned int target, int* err) {
   if (ld_relaxed(ctr) < target) {
     const long long t0 = clock64();
@@ -141,9 +109,6 @@ __device__ __forceinline__ void grid_wait_counter(const unsigned int* ctr, unsig
     }
   }
   asm volatile("fence.acquire.gpu;" ::: "memory");
-}
-__device__ __forceinline__ void st_release(unsigned int* p, unsigned int v) {
-  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 // MUFU.EX2 / MUFU.RCP without the denormal-range fix-up code of the CUDA fast-math intrinsics (that code
 // serialises independent chains through one predicate register); inputs are gate pre-activations.
@@ -175,66 +140,6 @@ __device__ __forceinline__ int grp_count(int nkr) { return (nkr + 3) / 4; }
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// ---- flag-in-data exchange ("LL": the data is its own ready flag) ---------------------------------------------
-// The per-step grid barrier costs store -> MEMBAR.ALL.GPU -> RED -> poll -> acquire fence -> TMA round trip, ~3.6k of
-// the 8.8k cycles of a forward step.  In the LL variants the streamed fp16 operand buffer is pre-filled with the
-// bit pattern 0xFFFF (an fp16 NaN that neither h in (-1,1) nor a saturated gate gradient can produce); producers
-// store their values with relaxed gpu-scope stores and NOTHING else, consumers poll the 16-byte packets they need
-// with relaxed gpu-scope loads until no 2-byte element equals the sentinel (every element is its own flag, so
-// torn 16-byte packets are harmless) and copy them into the 128B-swizzled K-major tile the MMA reads.  No fence, no
-// atomic, no barrier counter on the critical path; one L2 round trip from "stored" to "in shared memory".
-constexpr unsigned int LL_SENTINEL = 0xFFFFFFFFu;
-__device__ __forceinline__ uint4 ld_relaxed_v4(const void* p) {
-  uint4 v;
-  asm volatile("ld.relaxed.gpu.global.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_relaxed_v2(void* p, unsigned int a, unsigned int b) {
-  asm volatile("st.relaxed.gpu.global.v2.b32 [%0], {%1, %2};" ::"l"(p), "r"(a), "r"(b) : "memory");
-}
-__device__ __forceinline__ bool ll_ready(const uint4& v) {
-  return (__vcmpeq2(v.x, LL_SENTINEL) | __vcmpeq2(v.y, LL_SENTINEL) | __vcmpeq2(v.z, LL_SENTINEL) |
-          __vcmpeq2(v.w, LL_SENTINEL)) == 0u;
-}
-// poll one packet until it is complete; bounded (a protocol fault sets *err and lets the kernel run to its end)
-__device__ __forceinline__ void ll_wait(uint4& v, const void* src, int* err) {
-  if (ll_ready(v)) return;
-  const long long t0 = clock64();
-  unsigned int it = 0;
-  do {
-    v = ld_relaxed_v4(src);
-    if ((++it & 63u) == 0) {
-      if (*(volatile int*)err) return;
-      if (clock64() - t0 > rp::SPIN_LIMIT) {
-        *(volatile int*)err = 1;
-        return;
-      }
-    }
-  } while (!ll_ready(v));
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-__device__ __forceinline__ void st_relaxed_u32(void* p, unsigned int v) {
-  asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-// poll one 32-bit word until it differs from the sentinel (bounded like ll_wait)
-__device__ __forceinline__ unsigned int ll_wait_u32(const unsigned int* src, int* err) {
-  unsigned int v = ld_relaxed(src);
-  if (v != LL_SENTINEL) return v;
-  const long long t0 = clock64();
-  unsigned int it = 0;
-  do {
-    v = ld_relaxed(src);
-    if ((++it & 63u) == 0) {
-      if (*(volatile int*)err) return 0u;
-      if (clock64() - t0 > rp::SPIN_LIMIT) { *(volatile int*)err = 1; return 0u; }
-    }
-  } while (v == LL_SENTINEL);
-  return v;
 }
 
 
@@ -590,11 +495,10 @@ static bool vec_ok(const void* a, const void* b = nullptr, const void* c = nullp
   return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
            reinterpret_cast<uintptr_t>(d)) & 15) == 0;
 }
-// Nsight Compute cannot replay a cooperative launch of a kernel with a cluster dimension (it aborts the target:
-// `ncu_rc=9` in the round-1 driver record).  Under the profiler's injection — or with DS2_SPLITK_NONCOOP=1 — the
-// cluster sweeps are launched without the cooperative attribute; co-residency is still verified with
-// cudaOccupancyMaxActiveClusters, and a lone kernel of <= 148 one-per-SM CTAs on an otherwise idle stream becomes
-// resident as a whole either way.
+// Nsight Compute cannot replay a cooperative launch of a kernel with a cluster dimension (it aborts the target).
+// Under the profiler's injection — or with DS2_SPLITK_NONCOOP=1 — the cluster sweeps are launched without the
+// cooperative attribute; co-residency is still verified with cudaOccupancyMaxActiveClusters, and a lone kernel of
+// <= 148 one-per-SM CTAs on an otherwise idle stream becomes resident as a whole either way.
 static bool noncoop_cluster_launch() {
   const char* e = getenv("DS2_SPLITK_NONCOOP");
   if (e) return atoi(e) != 0;
@@ -618,6 +522,121 @@ static int env_flag(const char* name, int dflt) {
 // DS2_SWEEP_DEFER=0: store everything before the barrier arrival (see PersistParams::defer)
 static int sweep_defer_default() { return env_flag("DS2_SWEEP_DEFER", 1); }
 
+// The fields every sweep fills the same way.  `units`: hidden units per CTA, or per cluster (group of CTAs) of the
+// split-K variants.  The 4 KB control block at the start of the workspace holds err (offset 0) and the per-direction
+// step counters (offset 128).
+static PersistParams sweep_params(const SeqArgs& a, int units, const char* trace_env, void* ws) {
+  PersistParams p{};
+  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / units; p.G = a.G;
+  p.training = a.training;
+  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
+  for (int d = 0; d < a.D; ++d) { p.b_ih[d] = a.b_ih[d]; p.b_hh[d] = a.b_hh[d]; }
+  p.trace = trace_ptr_from_env(trace_env);
+  p.defer = sweep_defer_default();
+  p.err = static_cast<int*>(ws);
+  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + 128);
+  return p;
+}
+
+using SweepKernel = void (*)(const PersistParams);
+
+// Opt in to 227 KB of dynamic shared memory, once per device.  A launcher opts in every instantiation it can pick, so
+// that whichever shape comes first leaves none of them without it.  The occupancy queries below depend on the
+// opt-in: call this before them.
+static int opt_in_smem(DeviceOnce& once, std::initializer_list<SweepKernel> kerns) {
+  if (once.first()) {
+    for (SweepKernel k : kerns)
+      DS2_CHECK_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    once.done();
+  }
+  return DS2_OK;
+}
+
+// Launch configuration of a sweep for cudaLaunchKernelEx: cooperative (the grid barrier needs every CTA resident),
+// in clusters of `cluster` CTAs when cluster > 1.  Cluster launches drop the cooperative attribute under
+// noncoop_cluster_launch().
+struct SweepConfig {
+  cudaLaunchAttribute attrs[2];
+  cudaLaunchConfig_t cfg{};
+  SweepConfig(int cluster, int grid, size_t smem, cudaStream_t st) {
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(rp::THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    attrs[0].id = cudaLaunchAttributeClusterDimension;
+    attrs[0].val.clusterDim.x = cluster; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
+    attrs[1].id = cudaLaunchAttributeCooperative;
+    attrs[1].val.cooperative = 1;
+    cfg.attrs = cluster > 1 ? attrs : attrs + 1;
+    cfg.numAttrs = cluster > 1 && !noncoop_cluster_launch() ? 2 : 1;
+  }
+  SweepConfig(const SweepConfig&) = delete;   // cfg.attrs points into the object
+};
+
+// CTAs of `kern` that can be co-resident as plain CTAs (one per SM at most, see one_cta_per_sm)
+static int coop_fit(SweepKernel kern, size_t smem, int* fit) {
+  int per_sm = 0;
+  DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, rp::THREADS, smem));
+  *fit = per_sm * device_sm_count();
+  return DS2_OK;
+}
+
+// CTAs of `kern` that can be co-resident in whole clusters of `cluster` CTAs (a cluster cannot span two GPCs), or -1
+// when the device rejects the configuration
+static int cluster_fit(SweepKernel kern, int cluster, int grid, size_t smem, cudaStream_t st) {
+  SweepConfig c(cluster, grid, smem, st);
+  int max_clusters = 0;
+  if (cudaOccupancyMaxActiveClusters(&max_clusters, kern, &c.cfg) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return -1;
+  }
+  return max_clusters * cluster;
+}
+
+// The launch policy of every sweep.  `fit` CTAs can be co-resident, and the grid barrier needs every CTA of a launch
+// resident: both directions (p.D * per_dir CTAs) go in one launch when they fit; otherwise, if `per_dir_ok`, one
+// launch per direction; otherwise the shape is declined (return 1).  Then `prepare()` (operand copies, tensor maps),
+// the zeroed control block (its first `ctl_bytes` bytes of workspace), the launches and sweep_check_kernel.
+// cluster == 0: cudaLaunchCooperativeKernel, and a refused launch is an error.  cluster >= 1: cudaLaunchKernelEx in
+// clusters of that size (1: no cluster dimension); a refused first launch declines, with a warning on stderr
+// unless `fallback` is null, and a refused second launch is an error.
+template <typename Prepare>
+static int launch_sweep(SweepKernel kern, int cluster, int per_dir, size_t smem, int fit, bool per_dir_ok,
+                        size_t ctl_bytes, const char* what, const char* fallback, PersistParams& p, cudaStream_t st,
+                        Prepare&& prepare) {
+  int grid = p.D * per_dir, launches = 1;
+  if (fit < grid) {
+    if (!per_dir_ok || fit < per_dir) return 1;
+    grid = per_dir;
+    launches = p.D;
+  }
+  if (int rc = prepare()) return rc;
+  DS2_CHECK_CUDA(cudaMemsetAsync(p.err, 0, ctl_bytes, st));
+  SweepConfig c(cluster, grid, smem, st);
+  for (int li = 0; li < launches; ++li) {
+    p.d0 = li;
+    if (cluster == 0) {
+      void* args[] = {&p};
+      DS2_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3(grid), dim3(rp::THREADS), args, smem, st));
+    } else {
+      const cudaError_t le = cudaLaunchKernelEx(&c.cfg, kern, p);
+      if (le != cudaSuccess) {
+        (void)cudaGetLastError();
+        if (li == 0) {
+          if (fallback)
+            fprintf(stderr, "ds2_b200: WARNING %s launch failed (%s); using %s\n", what, cudaGetErrorString(le), fallback);
+          return 1;
+        }
+        set_error("%s: second launch failed: %s", what, cudaGetErrorString(le));
+        return DS2_ERR_CUDA;
+      }
+    }
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+  }
+  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
+  return DS2_OK;
+}
+
 static size_t fwd_smem_bytes(int NB) {
   using namespace rp;
   size_t NBp = NB + 1;
@@ -632,14 +651,6 @@ size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
   const size_t fwd = 4096 + align_up((size_t)D * G * H * H * 2, 256) + align_up((size_t)D * T * B * H * 2, 256);
   const size_t bwd = splitk_res_ws_bytes(G, T, B, H, D);
   return (fwd > bwd ? fwd : bwd) + 256;
-}
-
-static void set_acc_layout(PersistParams& p) {
-  // accumulator width = power of two >= max(32, NB) columns; as many chains as fit in the 512 accumulator columns
-  int cols = 32;
-  while (cols < p.NB) cols *= 2;
-  p.acc_cols = cols;
-  p.nacc = 1;   // one chain: switching accumulators between MMAs was measured slower, not faster
 }
 
 static bool fwd_eligible(const SeqArgs& a) {
@@ -665,71 +676,50 @@ static size_t res_ws_bytes(int G, int T, int B, int H, int D) {
   return 4096 + align_up((size_t)D * G * H * H * 2, 256) + align_up((size_t)D * T * B * H * 2, 256);
 }
 
-template <int RNN>
-static int launch_fwd_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+// Resident forward variants: the fp16 copy of W_hh (in the workspace) and the tensor maps of it and of the fp16 h
+// sequence.  `chunks`: 64-wide K chunks a CTA streams per step; a multiple of 4 takes one 3-D box per group of 4.
+static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chunks, cudaStream_t st) {
   using namespace rp;
-  const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
-  if (a.H % 64 != 0 || a.H / 64 > 32) return 1;
-  if (!vec_ok(a.gates, a.hseq, a.aux)) return 1;
-  if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
-  PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
-  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  p.training = a.training;
-  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux;
-  p.trace = trace_ptr_from_env("DS2_TRACE_FWD");
-  p.defer = sweep_defer_default();
-  set_acc_layout(p);
-  p.err = static_cast<int*>(ws);
-  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + 128);
+  const int G = a.G;
   __half* w16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096);
   p.h16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096 + align_up((size_t)a.D * G * a.H * a.H * 2, 256));
-  const size_t smem = one_cta_per_sm(res_smem_bytes(p.NB, a.H));
-  if (smem > 227 * 1024) return 1;
-  auto kern = rnn_fwd_persist_kernel<RNN, true>;
-  static DeviceOnce attr_once;
-  const int num_sms = device_sm_count();
-  if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_once.done();
-  }
-  int max_blocks_per_sm = 0;
-  DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_blocks_per_sm, kern, THREADS, smem));
-  int grid = a.D * p.NT, launches = 1;
-  if (max_blocks_per_sm < 1) return 1;
-  if (grid > max_blocks_per_sm * num_sms) {           // both directions do not fit: one launch per direction
-    if (p.NT > max_blocks_per_sm * num_sms) return 1;
-    grid = p.NT;
-    launches = a.D;
-  }
   const size_t wn = (size_t)G * a.H * a.H;
+  p.box3 = chunks % 4 == 0;
   for (int d = 0; d < a.D; ++d) {
-    p.b_ih[d] = a.b_ih[d];
-    p.b_hh[d] = a.b_hh[d];
     DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
     int rc = make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
     if (rc) return rc;
     rc = make_tmap_f16(&p.tmV[d], p.h16 + (size_t)d * a.T * a.B * a.H, 2, a.H, a.T * a.B, 1, (size_t)a.H, 0, 64, a.B, 1);
     if (rc) return rc;
-    p.box3 = (a.H / 64) % 4 == 0;
     if (p.box3) {   // rows b >= B of a box belong to the next time step (or are zero-filled): those N columns are discarded
       rc = make_tmap_f16(&p.tmV3[d], p.h16 + (size_t)d * a.T * a.B * a.H, 3, 64, a.T * a.B, a.H / 64, (size_t)a.H, 64, 64,
                          p.NB, 4);
       if (rc) return rc;
     }
   }
-  DS2_CHECK_CUDA(cudaMemsetAsync(ws, 0, 4096, st));
-  for (int li = 0; li < launches; ++li) {
-    p.d0 = li;
-    void* args[] = {&p};
-    DS2_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3(grid), dim3(THREADS), args, smem, st));
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
   return DS2_OK;
 }
 
-template <int RNN, bool LL>
+template <int RNN>
+static int launch_fwd_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+  const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  if (a.H % 64 != 0 || a.H / 64 > 32) return 1;
+  if (!vec_ok(a.gates, a.hseq, a.aux)) return 1;
+  if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
+  PersistParams p = sweep_params(a, rp::UT, "DS2_TRACE_FWD", ws);
+  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
+  const size_t smem = one_cta_per_sm(res_smem_bytes(p.NB, a.H));
+  if (smem > 227 * 1024) return 1;
+  const SweepKernel kern = rnn_fwd_persist_kernel<RNN, true>;
+  static DeviceOnce attr_once;
+  int fit = 0;
+  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
+  if (int rc = coop_fit(kern, smem, &fit)) return rc;
+  return launch_sweep(kern, 0, p.NT, smem, fit, true, 4096, nullptr, nullptr, p, st,
+                      [&] { return f16_weight_maps(a, p, ws, a.H / 64, st); });
+}
+
+template <int RNN>
 static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st);
 
 template <int RNN>
@@ -739,62 +729,31 @@ static int launch_fwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t 
   if (!getenv("DS2_NO_RESIDENT")) {
     if (RNN != DS2_RNN_TANH && env_flag("DS2_FWD_SPLITK", 1)) {   // 2-CTA clusters, half the MMA chain per step
       constexpr int R = RNN == DS2_RNN_TANH ? DS2_RNN_LSTM : RNN;
-      // DS2_FWD_LL=1: flag-in-data exchange instead of grid barrier + TMA of h_{t-1}.  Measured SLOWER (13.9k vs 8.7k
-      // cycles per step, profiles/r02_ll_exchange.md): strong per-thread loads do not pipeline (~600 cycles each),
-      // and even with the TMA engine as transport the exchange costs what the barrier costs — the floor is the
-      // store -> L2 -> load visibility latency, not the barrier.  Kept as a tested, selectable variant.
-      int rc = env_flag("DS2_FWD_LL", 0) ? launch_fwd_splitk<R, true>(a, ws, ws_bytes, st)
-                                         : launch_fwd_splitk<R, false>(a, ws, ws_bytes, st);
+      int rc = launch_fwd_splitk<R>(a, ws, ws_bytes, st);
       if (rc != 1) return rc;
     }
     int rc = launch_fwd_resident<RNN>(a, ws, ws_bytes, st);
     if (rc != 1) return rc;
   }
-  PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  PersistParams p = sweep_params(a, UT, "DS2_TRACE_FWD", ws);
   if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  p.training = a.training;
-  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux;
-  p.trace = trace_ptr_from_env("DS2_TRACE_FWD");
   if (ws_bytes < 4096) return 1;
-  set_acc_layout(p);
-  p.err = static_cast<int*>(ws);
-  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + 128);
   const size_t smem = one_cta_per_sm(fwd_smem_bytes(p.NB));
-  auto kern = rnn_fwd_persist_kernel<RNN, false>;
-  static DeviceOnce attr_once;
-  int max_blocks_per_sm = 0;
-  const int num_sms = device_sm_count();
-  if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_once.done();
-  }
   if (smem > 227 * 1024) return 1;
-  DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_blocks_per_sm, kern, THREADS, smem));
-  int grid = a.D * p.NT, launches = 1;
-  if (max_blocks_per_sm < 1) return 1;
-  if (grid > max_blocks_per_sm * num_sms) {           // both directions do not fit: one launch per direction
-    if (p.NT > max_blocks_per_sm * num_sms) return 1;
-    grid = p.NT;
-    launches = a.D;
-  }   // cannot be co-resident
-  for (int d = 0; d < a.D; ++d) {
-    p.b_ih[d] = a.b_ih[d];
-    p.b_hh[d] = a.b_hh[d];
-    int rc = make_tmap_3d(&p.tmW[d], a.w_hh[d], a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, BK, UT, G);
-    if (rc) return rc;
-    rc = make_tmap_2d(&p.tmV[d], a.hseq + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
-    if (rc) return rc;
-  }
-  DS2_CHECK_CUDA(cudaMemsetAsync(ws, 0, 4096, st));
-  for (int li = 0; li < launches; ++li) {
-    p.d0 = li;
-    void* args[] = {&p};
-    DS2_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3(grid), dim3(THREADS), args, smem, st));
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
-  return DS2_OK;
+  const SweepKernel kern = rnn_fwd_persist_kernel<RNN, false>;
+  static DeviceOnce attr_once;
+  int fit = 0;
+  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
+  if (int rc = coop_fit(kern, smem, &fit)) return rc;
+  return launch_sweep(kern, 0, p.NT, smem, fit, true, 4096, nullptr, nullptr, p, st, [&] {
+    for (int d = 0; d < a.D; ++d) {
+      int rc = make_tmap_3d(&p.tmW[d], a.w_hh[d], a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, BK, UT, G);
+      if (rc) return rc;
+      rc = make_tmap_2d(&p.tmV[d], a.hseq + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
+      if (rc) return rc;
+    }
+    return 0;
+  });
 }
 
 int rnn_sweep_fwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
@@ -910,14 +869,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const _
         if (lane == 0) trace_stamp(p.trace, p.T, step, 3);
         for (int cb = 0; cb < NB; cb += 32) {
           float acc[32];
-          const int nsum = min(p.nacc, NK * (BK / 8));
           tmem_ld32(acc_img, acc_pitch(NB), (uint32_t)cb, acc);
-          for (int a2 = 1; a2 < nsum; ++a2) {
-            float part[32];
-            tmem_ld32(acc_img, acc_pitch(NB), (uint32_t)(a2 * p.acc_cols + cb), part);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) acc[j] += part[j];
-          }
           if (lane < UT) {
 #pragma unroll
             for (int j = 0; j < 32; ++j)
@@ -1059,19 +1011,16 @@ __device__ __forceinline__ float pow2f(int ex) { return __int_as_float((ex + 127
 
 // CL = CTAs per cluster = K split: 4 (64 units per cluster, MMA M = 64) or 8 (128 units, M = 128: the same
 // number of CTAs, but each reduces only K/8, i.e. half as many MMA instructions on the per-step critical path).
-// LL (RES only): no grid barrier; the scaled fp16 gate gradients are their own ready flags (see the LL helpers) and
-// the per-step maxima travel as one word per (CTA, epilogue warp) in `gmeta`.
 // XG (RES, CL = 4 only): launched without clusters, as plain cooperative CTAs; a group of CL consecutive CTAs keeps
 // the roles of a cluster, but the partial dh_rec tiles travel through L2 (`xbuf`, counted in `xcnt`) instead of
 // distributed shared memory.  For GPUs whose GPCs cannot hold every cluster of the grid at once (a 132-SM H100 with
 // both directions of H = 1024: 32 clusters of 4), so that both directions still run in one launch.  The MMAs, sums
 // and scales are the cluster path's: the results are bit-identical.
-template <int RNN, bool RES, int CL, bool LL = false, int NKR_T = 0, bool XG = false>   // NKR_T: see rnn_fwd_splitk_kernel
+template <int RNN, bool RES, int CL, int NKR_T = 0, bool XG = false>   // NKR_T: see rnn_fwd_splitk_kernel
 __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __grid_constant__ PersistParams p) {
   using namespace rp;
   using namespace tc;
-  static_assert(!LL || RES, "the flag-in-data exchange streams the fp16 copy of the resident variant");
-  static_assert(!XG || (RES && !LL && CL == 4), "the L2 exchange is built for the resident 4-CTA variant");
+  static_assert(!XG || (RES && CL == 4), "the L2 exchange is built for the resident 4-CTA variant");
   constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
   constexpr int UM = UT * CL;                  // units per cluster (all M rows valid): 64 or 128 = MMA M
   constexpr int A_BYTES = UM * 128;            // one K chunk of the weight tile (shadows rp::A_BYTES)
@@ -1087,8 +1036,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
   float* cst = part + CL * xt_slice(UT, NB);                             // [16][NBp] carried dc / dh
   int* lens_s = reinterpret_cast<int*>(cst + UT * NBp);
   unsigned int* cta_max = reinterpret_cast<unsigned int*>(lens_s + ((NB + 1) & ~1));   // [2] (8 bytes)
-  unsigned int* wmax = cta_max + 2;                                      // LL: [2 step parities][4 epilogue warps]
-  uint64_t* full = reinterpret_cast<uint64_t*>(cta_max + 10);            // resident: one per group of 4 chunks
+  uint64_t* full = reinterpret_cast<uint64_t*>(cta_max + 2);            // resident: one per group of 4 chunks
   uint64_t* empty = full + (RES ? 32 : STAGES);                          // resident: [0] = weights landed
   uint64_t* accum_bar = empty + STAGES;
   uint64_t* part_bar = accum_bar + 1;
@@ -1113,25 +1061,16 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmW[d]);
-    if (!LL) tma_prefetch_desc(&p.tmV[d]);
-    for (int i = 0; i < (RES ? 32 : STAGES); ++i) mbar_init(&full[i], LL ? 4 : 1);   // LL: one arrival per loader warp
+    tma_prefetch_desc(&p.tmV[d]);
+    for (int i = 0; i < (RES ? 32 : STAGES); ++i) mbar_init(&full[i], 1);
     for (int i = 0; i < STAGES; ++i) mbar_init(&empty[i], RES ? 1 : 128);   // streaming: every MMA-warpgroup thread arrives
     mbar_init(accum_bar, 1);
     mbar_init(part_bar, XG ? 2 : 1);                     // XG: the producer's bulk copies + the warp that kept its rows
     fence_barrier_init();
     cta_max[0] = 0u;
-    for (int i = 0; i < 8; ++i) wmax[i] = 0u;
   }
   for (int i = threadIdx.x; i < UT * NBp; i += THREADS) cst[i] = 0.f;
   for (int i = threadIdx.x; i < NB; i += THREADS) lens_s[i] = i < B ? p.len[i] : 0;
-  if (LL) {   // batch-padding rows of the streamed tile are never loaded: keep them finite (their columns are unused)
-    uint8_t* vb = smem + NKR * A_BYTES;
-    for (int i = threadIdx.x; i < NKR * (NB - B) * 8; i += THREADS) {
-      const int c = i / ((NB - B) * 8), r = B + (i / 8) % (NB - B), j = i % 8;
-      *reinterpret_cast<uint4*>(vb + c * B_BYTES + r * 128 + j * 16) = make_uint4(0u, 0u, 0u, 0u);
-    }
-    fence_proxy_async();
-  }
   __syncthreads();
   if constexpr (!XG) cluster_sync_all();                 // peers' mbarriers are initialised
   const uint32_t tx_bytes = (uint32_t)(UM * 128 + B * 128);
@@ -1142,7 +1081,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         mbar_arrive_expect_tx(&empty[0], (uint32_t)(NKR * UM * 128));
         for (int c = 0; c < NKR; ++c) tma_load_2d(smem + c * A_BYTES, &p.tmW[d], &empty[0], kbase + c * 64, ut * UM);
         uint8_t* vbuf = smem + NKR * A_BYTES;
-        for (int step = 1; !LL && step < T; ++step) {     // LL: the epilogue warps fetch dGh[t_next] themselves
+        for (int step = 1; step < T; ++step) {
           const int t = d == 0 ? T - 1 - step : step;
           const int tn = d == 0 ? t + 1 : t - 1;
           grid_wait_counter(ctr, n_arrive * (unsigned int)step, p.err);
@@ -1284,20 +1223,17 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
     const uint32_t dst_row = XG ? 0u : mapa_u32(smem_u32(part), (uint32_t)dst_cta) + (uint32_t)(ks * ss * 4);
     const uint32_t dst_bar = XG ? 0u : mapa_u32(smem_u32(part_bar), (uint32_t)dst_cta);
     const uint32_t part_tx = (uint32_t)(CL * UT * NB * 4);               // bytes this CTA receives per step
-    // resident: s_cur scales what this step writes, s_prev un-scales what this step's MMAs consumed
-    const unsigned int* gmax_d = RES ? p.gmax + (size_t)d * (T + 1) : nullptr;
     // bias gradients: this thread's 4 units x (gate) sums over all steps of its batch column(s)
     float bsum[5][4];
 #pragma unroll
     for (int i = 0; i < 5; ++i)
 #pragma unroll
       for (int j = 0; j < 4; ++j) bsum[i][j] = 0.f;
+    // resident: s_cur scales what this step writes, s_prev un-scales what this step's MMAs consumed
     int sx_prev = 0, sx_cur = 0;
     // step-0 scale: |dGh| <= |dh| = |dY[t_first]| for every cell type
     if (RES) sx_cur = pow2_exp_for(__ldg(p.dymax + (d == 0 ? T - 1 : 0)), 0);
     float s_cur = pow2f(sx_cur), inv_prev = 1.f;
-    const int cta_in_dir = ut * CL + ks, nmeta = NTc * CL * 4;
-    (void)gmax_d;
     const float nscale = (RES && p.dgn16) ? __ldg(p.nscale) : 1.f;
     for (int step = 0; step < T; ++step) {
       const int t = d == 0 ? T - 1 - step : step;
@@ -1378,16 +1314,8 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         // send this CTA's partial tile: row (16q + ul), 32 columns split over the two half-warps
         mbar_wait(accum_bar, acc_phase);
         if (RES) {
-          // non-LL: this step's MMAs ran, so the grid barrier was passed: the maximum of step-1 the producer forwarded
-          // is final.  LL: the four loader warps left the maximum over all (CTA, warp) words of step-1 in wmax[parity]
-          // before their last full-barrier arrival (ordered by the full -> MMA -> accumulator barrier chain).
-          unsigned int gm;
-          if (LL) {
-            const volatile unsigned int* wm = wmax + (step & 1) * 4;
-            gm = max(max(wm[0], wm[1]), max(wm[2], wm[3]));
-          } else {
-            gm = *(volatile unsigned int*)(cta_max + 1);
-          }
+          // this step's MMAs ran, so the grid barrier was passed: the maximum of step-1 the producer forwarded is final
+          const unsigned int gm = *(volatile unsigned int*)(cta_max + 1);
           sx_prev = sx_cur;
           sx_cur = pow2_exp_for(max(gm, dym), sx_prev);      // non-negative floats order like their bit patterns
           s_cur = pow2f(sx_cur);
@@ -1454,8 +1382,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         uint2 pk;
         pk.x = *reinterpret_cast<const unsigned int*>(&lo);
         pk.y = *reinterpret_cast<const unsigned int*>(&hi);
-        if (LL) st_relaxed_v2(dst, pk.x, pk.y);            // saturated at +-65000: never the 0xFFFF sentinel
-        else *reinterpret_cast<uint2*>(dst) = pk;
+        *reinterpret_cast<uint2*>(dst) = pk;
       };
       auto finish4 = [&](int b, const float (&k)[6][NPF], const float (&dyv)[NPF], bool valid, float (&o)[5][NPF]) {
 #pragma unroll
@@ -1467,10 +1394,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
         if (!valid) {
           if (RES) {
 #pragma unroll
-            for (int g = 0; g < G; ++g) {
-              if (LL) st_relaxed_v2(hp16 + g * H, 0u, 0u);
-              else *reinterpret_cast<uint2*>(hp16 + g * H) = make_uint2(0u, 0u);
-            }
+            for (int g = 0; g < G; ++g) *reinterpret_cast<uint2*>(hp16 + g * H) = make_uint2(0u, 0u);
           }
           return;
         }
@@ -1560,49 +1484,8 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
           }
         }
       };
-      // LL: fetch the scaled fp16 gate gradients dGh[t] of ALL units of this CTA's K range (written by every CTA of
-      // the direction) into the swizzled K-major tile of the next step's MMAs; same packet / group scheme as the
-      // forward sweep (fetch_h).  Before the last group is handed over, the per-(CTA, warp) maxima of the step are
-      // polled too and their maximum is left in wmax[next parity][warp] for the scale of the next step.
-      auto fetch_dg = [&](int t_src) {
-        const size_t ld = (size_t)D * GH;
-        const __half* src = p.dg16 + (size_t)t_src * B * ld + (size_t)d * GH + kbase;
-        const uint32_t vb = smem_u32(smem + NKR * A_BYTES);
-        for (int g = 0; g < NG; ++g) {
-          const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
-          const int npk = (c1 - c0) * 8, total = B * npk;
-          for (int base = 0; base < total; base += 128 * 8) {
-            uint4 v[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const int idx = base + k * 128 + e;
-              if (idx < total) v[k] = ld_relaxed_v4(src + (size_t)(idx / npk) * ld + (size_t)(c0 * 8 + idx % npk) * 8);
-            }
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const int idx = base + k * 128 + e;
-              if (idx < total) {
-                const int row = idx / npk, pc = c0 * 8 + idx % npk;
-                ll_wait(v[k], src + (size_t)row * ld + (size_t)pc * 8, p.err);
-                st_shared_v4(vb + (uint32_t)((pc >> 3) * B_BYTES + row * 128 + (((pc & 7) ^ (row & 7)) << 4)), v[k]);
-              }
-            }
-          }
-          if (g == NG - 1) {
-            const unsigned int* mp = p.gmeta + ((size_t)d * T + step) * nmeta;
-            unsigned int m = 0u;
-            for (int i = e; i < nmeta; i += 128) m = max(m, ll_wait_u32(mp + i, p.err));
-            m = __reduce_max_sync(0xffffffffu, m);
-            if (lane == 0) wmax[((step + 1) & 1) * 4 + q] = m;
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(full + g);
-          if (e == 0 && g == 0) trace_stamp(p.trace, p.T, step + 1, 1);
-        }
-      };
       // the non-resident variants stream the fp32 gate gradients themselves: nothing can be deferred there
-      const bool defer = RES && (LL || p.defer) && single;
+      const bool defer = RES && p.defer && single;
       float sv[5][NPF];
       if (single) {
         finish4(b_own, kc, pdy, pvalid, sv);
@@ -1617,40 +1500,25 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
       if (RES) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
-        if (LL) {           // one word per (CTA, epilogue warp): no intra-CTA reduction on the critical path
-          unsigned int lb = __float_as_uint(lmax);
-          if (lb >= 0x7f800000u) lb = 0x7f7fffffu;                    // inf / nan: finite, and never the sentinel
-          if (lane == 0) st_relaxed_u32(p.gmeta + ((size_t)d * T + step) * nmeta + cta_in_dir * 4 + q, lb);
-        } else if (lane == 0) {
-          atomicMax(cta_max, __float_as_uint(lmax));                  // non-negative floats order like uints
-        }
+        if (lane == 0) atomicMax(cta_max, __float_as_uint(lmax));   // non-negative floats order like uints
       }
       if (e == 0) trace_stamp(p.trace, p.T, step, 8);
-      if (!LL) {
-        named_bar_sync(1, 128);
-        if (e == 0) {
-          trace_stamp(p.trace, p.T, step, 9);
-          if (RES) {
-            atomicMax(p.gmax + (size_t)d * (T + 1) + step + 1, cta_max[0]);
-            cta_max[0] = 0u;
-          }
-          fence_proxy_async_global();
-          trace_stamp(p.trace, p.T, step, 10);
-          red_release(ctr, 1u);
-          trace_stamp(p.trace, p.T, step, 11);
-          trace_stamp_ns(p.trace, p.T, step, 12);
+      named_bar_sync(1, 128);
+      if (e == 0) {
+        trace_stamp(p.trace, p.T, step, 9);
+        if (RES) {
+          atomicMax(p.gmax + (size_t)d * (T + 1) + step + 1, cta_max[0]);
+          cta_max[0] = 0u;
         }
-      } else if (e == 0) {
+        fence_proxy_async_global();
+        trace_stamp(p.trace, p.T, step, 10);
+        red_release(ctr, 1u);
         trace_stamp(p.trace, p.T, step, 11);
         trace_stamp_ns(p.trace, p.T, step, 12);
       }
       if (defer) {
         if (b_own < B) store_dg(b_own, sv);
         if (e == 0) trace_stamp(p.trace, p.T, step, 13);
-      }
-      if (LL && step + 1 < T) {        // the other CTAs' gate gradients land while the fp32 stores above drain
-        if (e == 0) trace_stamp(p.trace, p.T, step + 1, 0);
-        fetch_dg(t);
       }
     }
     if (p.dbias[d]) {
@@ -1694,7 +1562,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
 // gates + cell update for its 16 units in one pass (thread = 4 consecutive units x one batch column).
 // NKR_T: compile-time number of K chunks per CTA (0 = runtime): with constant chunk offsets the MMA descriptors are
 // "uniform base + immediate" and the issue loop needs no vector arithmetic / R2UR per instruction.
-template <int RNN, bool LL, int NKR_T = 0>
+template <int RNN, int NKR_T = 0>
 __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __grid_constant__ PersistParams p) {
   using namespace rp;
   using namespace tc;
@@ -1727,8 +1595,8 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmW[d]);
-    if (!LL) tma_prefetch_desc(&p.tmV[d]);
-    for (int i = 0; i < 8; ++i) mbar_init(&full[i], LL ? 4 : 1);   // LL: one arrival per loader (= epilogue) warp
+    tma_prefetch_desc(&p.tmV[d]);
+    for (int i = 0; i < 8; ++i) mbar_init(&full[i], 1);
     mbar_init(wbar, 1);
     mbar_init(accum_bar, 1);
     mbar_init(part_bar, 1);
@@ -1736,14 +1604,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
   }
   for (int i = threadIdx.x; i < UT * NBp; i += THREADS) cst[i] = 0.f;
   for (int i = threadIdx.x; i < NB; i += THREADS) lens_s[i] = i < B ? p.len[i] : 0;
-  if (LL) {   // batch-padding rows of the streamed tile are never loaded: keep them finite (their columns are unused)
-    uint8_t* hb = smem + NKR * AW;
-    for (int i = threadIdx.x; i < NKR * (NB - B) * 8; i += THREADS) {
-      const int c = i / ((NB - B) * 8), r = B + (i / 8) % (NB - B), j = i % 8;
-      *reinterpret_cast<uint4*>(hb + c * B_BYTES + r * 128 + j * 16) = make_uint4(0u, 0u, 0u, 0u);
-    }
-    fence_proxy_async();
-  }
   __syncthreads();
   cluster_sync_all();                                     // the peer's mbarriers are initialised
   const int kc0 = rank * NKR;                             // first K chunk (of H/64) of this CTA
@@ -1757,7 +1617,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
         tma_load_3d(smem + c * AW + 64 * 128, &p.tmW[d], wbar, (kc0 + c) * 64, U0 + UT, 0);
       }
       uint8_t* hbuf = smem + NKR * AW;
-      for (int step = 1; !LL && step < T; ++step) {       // LL: the epilogue warps fetch h_{t-1} themselves (below)
+      for (int step = 1; step < T; ++step) {
         const int t = d == 0 ? step : T - 1 - step;
         const int tp = d == 0 ? t - 1 : t + 1;
         grid_wait_counter(ctr, n_arrive * (unsigned int)step, p.err);
@@ -1849,7 +1709,6 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
     auto st4 = [](float* dst, const float (&v)[4]) { *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]); };
     uint32_t acc_phase = 0, part_phase = 0;
     const bool single = B <= 32;
-    int step_for_trace = 0;
     for (int step = 0; step < T; ++step) {
       const int t = d == 0 ? step : T - 1 - step;
       // input projections of this thread's cells: independent of the recurrence, fetched before the MMA wait
@@ -1952,9 +1811,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
         uint2 pk;
         pk.x = *reinterpret_cast<const unsigned int*>(&lo);
         pk.y = *reinterpret_cast<const unsigned int*>(&hi);
-        __half* hdst = p.h16 + (((size_t)d * T + t) * B + b) * H + u0 + uq;
-        if (LL) st_relaxed_v2(hdst, pk.x, pk.y);          // the values are their own ready flags (|h| < 1: never 0xFFFF)
-        else *reinterpret_cast<uint2*>(hdst) = pk;
+        *reinterpret_cast<uint2*>(p.h16 + (((size_t)d * T + t) * B + b) * H + u0 + uq) = pk;
       };
       auto store4 = [&](int b, const float (&o)[6][4]) {
         const size_t so = (((size_t)d * T + t) * B + b) * H + u0 + uq;
@@ -1966,42 +1823,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
         }
         st4(p.hseq + so, o[5]);
       };
-      // LL: fetch h_t of ALL units of this CTA's K half (written by the 32 owner CTAs of those units) into the
-      // swizzled K-major tile of the next step's MMA.  Called by the 128 epilogue threads after accum_bar of this
-      // step completed, i.e. when the MMAs that read the tile are done.  One 16-byte packet = 8 consecutive k of
-      // one batch row; consecutive threads take consecutive packets of a row (512 contiguous bytes per warp
-      // instruction); up to 8 polls in flight per thread; a group of 4 K chunks is handed to the MMA thread as soon
-      // as it is complete (fence.proxy.async: generic-proxy stores -> async-proxy reads of wgmma).
-      auto fetch_h = [&](int t_src) {
-        const __half* src = p.h16 + ((size_t)d * T + t_src) * B * H + (size_t)kc0 * 64;
-        const uint32_t hb = smem_u32(smem + NKR * AW);
-        for (int g = 0; g < NG; ++g) {
-          const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
-          const int npk = (c1 - c0) * 8, total = B * npk;
-          for (int base = 0; base < total; base += 128 * 8) {
-            uint4 v[8];
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const int idx = base + k * 128 + e;
-              if (idx < total) v[k] = ld_relaxed_v4(src + (size_t)(idx / npk) * H + (size_t)(c0 * 8 + idx % npk) * 8);
-            }
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-              const int idx = base + k * 128 + e;
-              if (idx < total) {
-                const int row = idx / npk, pc = c0 * 8 + idx % npk;
-                ll_wait(v[k], src + (size_t)row * H + (size_t)pc * 8, p.err);
-                st_shared_v4(hb + (uint32_t)((pc >> 3) * B_BYTES + row * 128 + (((pc & 7) ^ (row & 7)) << 4)), v[k]);
-              }
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(full + g);
-          if (e == 0 && g == 0) trace_stamp(p.trace, p.T, step_for_trace, 1);
-        }
-      };
-      const bool defer = LL || (p.defer && single);
+      const bool defer = p.defer && single;
       float sv[6][4];
       if (single) {
         if (b_own < B) {
@@ -2017,28 +1839,18 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
         }
       }
       if (e == 0) trace_stamp(p.trace, p.T, step, 8);
-      if (!LL) {
-        named_bar_sync(1, 128);        // CTA-scope: every epilogue thread's stores happen-before thread 0's release
-        if (e == 0) {
-          trace_stamp(p.trace, p.T, step, 9);
-          fence_proxy_async_global();
-          trace_stamp(p.trace, p.T, step, 10);
-          red_release(ctr, 1u);
-          trace_stamp(p.trace, p.T, step, 11);
-          trace_stamp_ns(p.trace, p.T, step, 12);
-        }
-      } else if (e == 0) {
+      named_bar_sync(1, 128);          // CTA-scope: every epilogue thread's stores happen-before thread 0's release
+      if (e == 0) {
+        trace_stamp(p.trace, p.T, step, 9);
+        fence_proxy_async_global();
+        trace_stamp(p.trace, p.T, step, 10);
+        red_release(ctr, 1u);
         trace_stamp(p.trace, p.T, step, 11);
         trace_stamp_ns(p.trace, p.T, step, 12);
       }
-      if (defer && single) {
+      if (defer) {
         if (b_own < B) store4(b_own, sv);
         if (e == 0) trace_stamp(p.trace, p.T, step, 13);
-      }
-      if (LL && step + 1 < T) {        // the other CTAs' h_t lands while the fp32 stores above drain
-        step_for_trace = step + 1;
-        if (e == 0) trace_stamp(p.trace, p.T, step + 1, 0);
-        fetch_h(t);
       }
     }
   }
@@ -2054,93 +1866,23 @@ static size_t fwd_splitk_smem_bytes(int NB, int H) {
 }
 
 // returns 1 when the shape / device does not take this variant (the caller then uses the 16-unit resident kernel)
-template <int RNN, bool LL>
+template <int RNN>
 static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
-  using namespace rp;
   constexpr int G = RNN == DS2_RNN_LSTM ? 4 : 3;
   if (a.H % 128 != 0 || a.H / 128 > 32) return 1;
   if (!vec_ok(a.gates, a.hseq, a.aux) || !a.aux) return 1;
   if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
-  PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32;
+  PersistParams p = sweep_params(a, 32, "DS2_TRACE_FWD", ws);
   if (p.NB > 64) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  p.H = a.H; p.D = a.D; p.NT = a.H / 32; p.G = G;
-  p.training = a.training;
-  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux;
-  p.trace = trace_ptr_from_env("DS2_TRACE_FWD");
-  p.defer = sweep_defer_default();
-  set_acc_layout(p);
-  p.err = static_cast<int*>(ws);
-  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + 128);
-  __half* w16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096);
-  p.h16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096 + align_up((size_t)a.D * G * a.H * a.H * 2, 256));
   const size_t smem = one_cta_per_sm(fwd_splitk_smem_bytes(p.NB, a.H));
   if (smem > 227 * 1024) return 1;
-  auto kern = (a.H == 1024) ? rnn_fwd_splitk_kernel<RNN, LL, 8> : rnn_fwd_splitk_kernel<RNN, LL, 0>;   // H = 1024: unrolled issue loop
+  // H = 1024: unrolled issue loop
+  const SweepKernel kern = a.H == 1024 ? rnn_fwd_splitk_kernel<RNN, 8> : rnn_fwd_splitk_kernel<RNN, 0>;
   static DeviceOnce attr_once;
-  if (attr_once.first()) {   // BOTH instantiations: whichever shape comes first must not leave the other without its opt-in
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_fwd_splitk_kernel<RNN, LL, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_fwd_splitk_kernel<RNN, LL, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_once.done();
-  }
-  int grid = a.D * p.NT * 2, launches = 1;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attrs[2];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = 2; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-  attrs[1].id = cudaLaunchAttributeCooperative;
-  attrs[1].val.cooperative = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = noncoop_cluster_launch() ? 1 : 2;     // see the backward launcher (Nsight Compute)
-  int max_clusters = 0;
-  cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg);
-  if (oe != cudaSuccess) { (void)cudaGetLastError(); return 1; }
-  if (max_clusters * 2 < grid) {
-    if (max_clusters * 2 < p.NT * 2) return 1;
-    grid = p.NT * 2;
-    launches = a.D;
-    cfg.gridDim = dim3(grid);
-  }
-  const size_t wn = (size_t)G * a.H * a.H;
-  for (int d = 0; d < a.D; ++d) {
-    p.b_ih[d] = a.b_ih[d];
-    p.b_hh[d] = a.b_hh[d];
-    DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
-    int rc = make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
-    if (rc) return rc;
-    rc = make_tmap_f16(&p.tmV[d], p.h16 + (size_t)d * a.T * a.B * a.H, 2, a.H, a.T * a.B, 1, (size_t)a.H, 0, 64, a.B, 1);
-    if (rc) return rc;
-    p.box3 = (a.H / 128) % 4 == 0;
-    if (p.box3) {
-      rc = make_tmap_f16(&p.tmV3[d], p.h16 + (size_t)d * a.T * a.B * a.H, 3, 64, a.T * a.B, a.H / 64, (size_t)a.H, 64, 64,
-                         p.NB, 4);
-      if (rc) return rc;
-    }
-  }
-  DS2_CHECK_CUDA(cudaMemsetAsync(ws, 0, 4096, st));
-  if (LL)   // every 2-byte element of the h stream is its own "not yet written" flag
-    DS2_CHECK_CUDA(cudaMemsetAsync(p.h16, 0xFF, (size_t)a.D * a.T * a.B * a.H * sizeof(__half), st));
-  for (int li = 0; li < launches; ++li) {
-    p.d0 = li;
-    cudaError_t le = cudaLaunchKernelEx(&cfg, kern, p);
-    if (le != cudaSuccess) {
-      (void)cudaGetLastError();
-      if (li == 0) {
-        fprintf(stderr, "ds2_b200: WARNING split-K forward sweep launch failed (%s); using the 16-unit kernel\n",
-                cudaGetErrorString(le));
-        return 1;
-      }
-      set_error("split-K forward sweep: second launch failed: %s", cudaGetErrorString(le));
-      return DS2_ERR_CUDA;
-    }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
-  return DS2_OK;
+  if (int rc = opt_in_smem(attr_once, {rnn_fwd_splitk_kernel<RNN, 8>, rnn_fwd_splitk_kernel<RNN, 0>})) return rc;
+  const int fit = cluster_fit(kern, 2, a.D * p.NT * 2, smem, st);
+  return launch_sweep(kern, 2, p.NT * 2, smem, fit, true, 4096, "split-K forward sweep", "the 16-unit kernel", p, st,
+                      [&] { return f16_weight_maps(a, p, ws, a.H / 128, st); });
 }
 
 static size_t splitk_smem_bytes(int NB, int CL) {
@@ -2148,16 +1890,6 @@ static size_t splitk_smem_bytes(int NB, int CL) {
   size_t NBp = NB + 1;
   return 1024 + (size_t)STAGES * ((size_t)UT * CL * 128 + (size_t)NB * 128) +
          ((size_t)CL * xt_slice(UT, NB) + UT * NBp + NB + 16) * sizeof(float) + (2 * STAGES + 3) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
-}
-
-// max |x| over n floats -> atomicMax on float bits (x >= 0 after fabs)
-__global__ void absmax_kernel(size_t n, const float* __restrict__ x, unsigned int* __restrict__ out) {
-  float m = 0.f;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    m = fmaxf(m, fabsf(x[i]));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if (threadIdx.x % 32 == 0) atomicMax(out, __float_as_uint(m));
 }
 
 // out[t] = float bits of max |x[t, :]| over the n floats of row t (one CTA per row, x >= 0 after fabs -> uint order)
@@ -2186,9 +1918,8 @@ static size_t splitk_res_smem_bytes(int NB, int Kc, int CL) {
   return 1024 + (size_t)(Kc / 64) * ((size_t)UT * CL * 128 + (size_t)NB * 128) +
          ((size_t)CL * xt_slice(UT, NB) + UT * NBp + NB + 16) * sizeof(float) + (32 + STAGES + 3) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
-// workspace of the resident backward: [4 KB control][gmax D*(T+1) uints][W^T fp16: D*H*GH][dg16: T*B*D*GH]
-// (+ [dymax: T uints][gmeta: D*T*(H/16)*4 uints] after gmax: H/16 CTAs per direction, 4 epilogue warps each)
-// (+ [xbuf: D*H/16 CTAs x 4 sources x 2 parities partial tiles] after dg16: the 4-CTA L2 exchange)
+// workspace of the resident backward: [4 KB control][gmax D*(T+1) uints][dymax: T uints][W^T fp16: D*H*GH]
+// [dg16: T*B*D*GH][xbuf: D*H/16 CTAs x 4 sources x 2 parities partial tiles, the 4-CTA L2 exchange]
 // The control block holds err (offset 0), the step counters (128) and the L2 exchange's xcnt (1024: <= 768 CTAs).
 constexpr size_t XCNT_OFFSET = 1024;
 constexpr int XCNT_MAX = (4096 - (int)XCNT_OFFSET) / 4;
@@ -2198,11 +1929,11 @@ static size_t splitk_xbuf_bytes(int B, int H, int D) {
 static size_t splitk_res_ws_bytes(int G, int T, int B, int H, int D) {
   const size_t GH = (size_t)G * H;
   return 4096 + align_up((size_t)D * (T + 1) * 4, 256) + align_up((size_t)T * 4, 256) +
-         align_up((size_t)D * T * (H / 16) * 4 * 4, 256) + align_up((size_t)D * H * GH * 2, 256) +
-         align_up((size_t)T * B * D * GH * 2, 256) + align_up(splitk_xbuf_bytes(B, H, D), 256);
+         align_up((size_t)D * H * GH * 2, 256) + align_up((size_t)T * B * D * GH * 2, 256) +
+         align_up(splitk_xbuf_bytes(B, H, D), 256);
 }
 
-template <int RNN, int CL, bool LL>
+template <int RNN, int CL>
 static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
   using namespace rp;
   const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
@@ -2212,13 +1943,8 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
   if (CL == 8 && ((a.B + 7) / 8 * 8) % 16 != 0) return 1;                                       // M = 128: N % 16 == 0
   if (!vec_ok(a.gates, a.hseq, a.aux, a.dy)) return 1;
   if (ws_bytes < splitk_res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
-  PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UM; p.G = G;
+  PersistParams p = sweep_params(a, UM, "DS2_TRACE_BWD", ws);
   if (p.NB > (CL == 8 ? 64 : 128)) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  p.training = 1;
-  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
-  p.trace = trace_ptr_from_env("DS2_TRACE_BWD");
-  p.defer = sweep_defer_default();
   for (int d = 0; d < a.D; ++d) { p.dbias[d] = a.dbias[d]; p.dbias_hn[d] = a.dbias_hn[d]; }
   if (a.f16_dg && a.f16_dgT && a.f16_scale && (RNN != DS2_RNN_GRU || a.f16_auxT)) {
     p.dgn16 = static_cast<__half*>(a.f16_dg);
@@ -2226,16 +1952,10 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
     p.auxn16T = static_cast<__half*>(a.f16_auxT);
     p.nscale = a.f16_scale;
   }
-  set_acc_layout(p);
   char* base = static_cast<char*>(ws);
-  p.err = reinterpret_cast<int*>(base);
-  p.bar = reinterpret_cast<unsigned int*>(base + 128);
   size_t off = 4096;
   p.gmax = reinterpret_cast<unsigned int*>(base + off); off += align_up((size_t)a.D * (a.T + 1) * 4, 256);
   p.dymax = reinterpret_cast<unsigned int*>(base + off); off += align_up((size_t)a.T * 4, 256);
-  p.gmeta = reinterpret_cast<unsigned int*>(base + off);
-  const size_t gmeta_bytes = (size_t)a.D * a.T * (a.H / 16) * 4 * 4;
-  off += align_up(gmeta_bytes, 256);
   __half* wT16 = reinterpret_cast<__half*>(base + off); off += align_up((size_t)a.D * a.H * GH * 2, 256);
   p.dg16 = reinterpret_cast<__half*>(base + off); off += align_up((size_t)a.T * a.B * a.D * GH * 2, 256);
   p.xbuf = reinterpret_cast<float*>(base + off);
@@ -2245,117 +1965,71 @@ static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_byte
   // DS2_SPLITK_XCHG=cluster|global: force the partial-tile exchange through distributed shared memory or through L2
   const char* xe = getenv("DS2_SPLITK_XCHG");
   const bool force_cluster = xe && !strcmp(xe, "cluster"), force_global = xe && !strcmp(xe, "global");
-  if (force_global && (CL != 4 || LL)) return 1;   // only the 4-CTA non-LL variant has the L2 exchange
+  if (force_global && CL != 4) return 1;   // only the 4-CTA variant has the L2 exchange
   // H = 1024 (the BASELINE shapes): compile-time chunk count -> unrolled issue loop
   constexpr int NKU = (G * 1024 / CL) / 64;   // chunks per CTA at H = 1024: 16 / 12 / 4 (CL 4), 8 / 6 / 2 (CL 8)
-  constexpr bool HAS_XG = CL == 4 && !LL;
-  auto kern = (!LL && a.H == 1024) ? rnn_bwd_splitk_kernel<RNN, true, CL, LL, NKU> : rnn_bwd_splitk_kernel<RNN, true, CL, LL, 0>;
-  auto kern_xg = kern;
-  if constexpr (HAS_XG)
-    kern_xg = a.H == 1024 ? rnn_bwd_splitk_kernel<RNN, true, CL, false, NKU, true> : rnn_bwd_splitk_kernel<RNN, true, CL, false, 0, true>;
+  SweepKernel kern = a.H == 1024 ? rnn_bwd_splitk_kernel<RNN, true, CL, NKU> : rnn_bwd_splitk_kernel<RNN, true, CL, 0>;
   static DeviceOnce attr_once;
-  if (attr_once.first()) {   // ALL instantiations (see the forward launcher)
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, LL, NKU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, LL, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    if constexpr (HAS_XG) {
-      DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, false, NKU, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      DS2_CHECK_CUDA(cudaFuncSetAttribute(rnn_bwd_splitk_kernel<RNN, true, CL, false, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    }
-    attr_once.done();
-  }
-  int grid = a.D * p.NT * CL, launches = 1;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attrs[2];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = CL; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-  attrs[1].id = cudaLaunchAttributeCooperative;
-  attrs[1].val.cooperative = 1;
-  cfg.attrs = attrs;
-  // Nsight Compute cannot replay a cooperative cluster launch: DS2_SPLITK_NONCOOP=1 (profiling only) drops the
-  // cooperative attribute; co-residency is still checked with cudaOccupancyMaxActiveClusters below.
-  cfg.numAttrs = noncoop_cluster_launch() ? 1 : 2;
-  int max_clusters = 0;
-  cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg);
-  if (oe != cudaSuccess) { (void)cudaGetLastError(); return 1; }
+  int rc;
+  if constexpr (CL == 4)
+    rc = opt_in_smem(attr_once, {rnn_bwd_splitk_kernel<RNN, true, CL, NKU>, rnn_bwd_splitk_kernel<RNN, true, CL, 0>,
+                                 rnn_bwd_splitk_kernel<RNN, true, CL, NKU, true>, rnn_bwd_splitk_kernel<RNN, true, CL, 0, true>});
+  else
+    rc = opt_in_smem(attr_once, {rnn_bwd_splitk_kernel<RNN, true, CL, NKU>, rnn_bwd_splitk_kernel<RNN, true, CL, 0>});
+  if (rc) return rc;
   // Path, from what the device reports: (1) every cluster of the grid co-resident: cluster exchange, one launch.
   // (2) Otherwise the plain cooperative grid co-resident (a cluster cannot span two GPCs, so clusters of 4 can fail
   // where single CTAs fit: 32 clusters of 4 on a 132-SM H100): L2 exchange, one launch.  (3) Otherwise one launch
-  // per direction with the cluster exchange.
-  bool xg = false;
-  int fit = max_clusters * CL;                           // CTAs of the chosen path that can be co-resident
+  // per direction with the cluster exchange; never with 8-CTA clusters, which are only worth it when both
+  // directions run concurrently.
+  const int grid = a.D * p.NT * CL;
+  int cluster = CL;
+  int fit = cluster_fit(kern, CL, grid, smem, st);
+  if (fit < 0) return 1;
   if (force_global || (fit < grid && !force_cluster)) {
-    if constexpr (HAS_XG) {
-      int per_sm = 0;
-      DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern_xg, THREADS, smem));
-      const int resident = per_sm * device_sm_count();
+    if constexpr (CL == 4) {
+      const SweepKernel kern_xg =
+          a.H == 1024 ? rnn_bwd_splitk_kernel<RNN, true, CL, NKU, true> : rnn_bwd_splitk_kernel<RNN, true, CL, 0, true>;
+      int resident = 0;
+      if ((rc = coop_fit(kern_xg, smem, &resident))) return rc;
       if (grid <= XCNT_MAX && (resident >= grid || force_global)) {
-        xg = true;
-        fit = resident;
         kern = kern_xg;
-        cfg.attrs = attrs + 1;                           // cooperative, no cluster dimension
-        cfg.numAttrs = 1;
+        cluster = 1;
+        fit = resident;
       }
     }
-    if (force_global && !xg) return 1;
+    if (force_global && cluster != 1) return 1;
   }
-  if (fit < grid) {
-    // 8-CTA clusters are only worth it when both directions run concurrently (otherwise the two directions run
-    // back to back)
-    if (CL == 8 || fit < p.NT * CL) return 1;
-    grid = p.NT * CL;
-    launches = a.D;
-    cfg.gridDim = dim3(grid);
-  }
-  DS2_CHECK_CUDA(cudaMemsetAsync(ws, 0, 4096 + align_up((size_t)a.D * (a.T + 1) * 4, 256), st));
-  const size_t wn = (size_t)a.H * GH;
-  const bool cached = a.w_hhT16[0] && (a.D == 1 || a.w_hhT16[1]);   // fp16 W_hh^T left by the forward pass
-  if (!cached) {
-    int rc = materialize_w_hh(a, st);
-    if (rc) return rc;
-  }
-  for (int d = 0; d < a.D; ++d) {
-    const __half* wsrc = static_cast<const __half*>(a.w_hhT16[d]);
+  // the control block and gmax are zeroed
+  rc = launch_sweep(kern, cluster, p.NT * CL, smem, fit, CL != 8, 4096 + align_up((size_t)a.D * (a.T + 1) * 4, 256),
+                    "resident split-K backward sweep", CL == 8 ? nullptr : "a slower variant", p, st, [&]() -> int {
+    const size_t wn = (size_t)a.H * GH;
+    const bool cached = a.w_hhT16[0] && (a.D == 1 || a.w_hhT16[1]);   // fp16 W_hh^T left by the forward pass
     if (!cached) {
-      DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], wT16 + (size_t)d * wn);
-      wsrc = wT16 + (size_t)d * wn;
+      int mrc = materialize_w_hh(a, st);
+      if (mrc) return mrc;
     }
-    int rc = make_tmap_f16(&p.tmW[d], wsrc, 2, GH, a.H, 1, (size_t)GH, 0, 64, UM, 1);
-    if (rc) return rc;
-    rc = make_tmap_f16(&p.tmV[d], p.dg16, 2, a.D * GH, a.T * a.B, 1, (size_t)a.D * GH, 0, 64, a.B, 1);
-    if (rc) return rc;
-    p.box3 = ((GH / CL) / 64) % 4 == 0;
-    if (p.box3) {
-      rc = make_tmap_f16(&p.tmV3[d], p.dg16, 3, 64, a.T * a.B, a.D * GH / 64, (size_t)a.D * GH, 64, 64, p.NB, 4);
-      if (rc) return rc;
-    }
-  }
-  // per-time-step max |dY[t]|: the step-0 scale, and part of every later step's scale (spiky upstream gradients)
-  DS2_LAUNCH(absmax_rows_kernel, a.T, 256, 0, st, (size_t)a.B * a.H, a.dy, p.dymax);
-  if (LL) {   // every 2-byte element of the gate-gradient stream / every word of the maxima is its own ready flag
-    DS2_CHECK_CUDA(cudaMemsetAsync(p.gmeta, 0xFF, gmeta_bytes, st));
-    DS2_CHECK_CUDA(cudaMemsetAsync(p.dg16, 0xFF, (size_t)a.T * a.B * a.D * GH * sizeof(__half), st));
-  }
-  for (int li = 0; li < launches; ++li) {
-    p.d0 = li;
-    cudaError_t le = cudaLaunchKernelEx(&cfg, kern, p);
-    if (le != cudaSuccess) {
-      (void)cudaGetLastError();
-      if (li == 0) {
-        if (CL != 8)
-          fprintf(stderr, "ds2_b200: WARNING resident split-K backward sweep launch failed (%s); using a slower variant\n",
-                  cudaGetErrorString(le));
-        return 1;
+    for (int d = 0; d < a.D; ++d) {
+      const __half* wsrc = static_cast<const __half*>(a.w_hhT16[d]);
+      if (!cached) {
+        DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], wT16 + (size_t)d * wn);
+        wsrc = wT16 + (size_t)d * wn;
       }
-      set_error("resident split-K backward sweep: second launch failed: %s", cudaGetErrorString(le));
-      return DS2_ERR_CUDA;
+      int trc = make_tmap_f16(&p.tmW[d], wsrc, 2, GH, a.H, 1, (size_t)GH, 0, 64, UM, 1);
+      if (trc) return trc;
+      trc = make_tmap_f16(&p.tmV[d], p.dg16, 2, a.D * GH, a.T * a.B, 1, (size_t)a.D * GH, 0, 64, a.B, 1);
+      if (trc) return trc;
+      p.box3 = ((GH / CL) / 64) % 4 == 0;
+      if (p.box3) {
+        trc = make_tmap_f16(&p.tmV3[d], p.dg16, 3, 64, a.T * a.B, a.D * GH / 64, (size_t)a.D * GH, 64, 64, p.NB, 4);
+        if (trc) return trc;
+      }
     }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
+    // per-time-step max |dY[t]|: the step-0 scale, and part of every later step's scale (spiky upstream gradients)
+    DS2_LAUNCH(absmax_rows_kernel, a.T, 256, 0, st, (size_t)a.B * a.H, a.dy, p.dymax);
+    return DS2_OK;
+  });
+  if (rc != DS2_OK) return rc;
   if (a.dbias_done && a.dbias[0]) *a.dbias_done = 1;
   if (a.f16_done && p.dgn16) *a.f16_done = 1;
   return DS2_OK;
@@ -2367,10 +2041,7 @@ static int launch_bwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
   const int GH = G * a.H;
   if (!getenv("DS2_NO_RESIDENT")) {
-    // DS2_BWD_LL=1: flag-in-data exchange instead of grid barrier + TMA of dGh[t_next] (measured slower, see the
-    // forward launcher)
-    int rc = env_flag("DS2_BWD_LL", 0) ? launch_bwd_splitk_resident<RNN, CL, true>(a, ws, ws_bytes, st)
-                                       : launch_bwd_splitk_resident<RNN, CL, false>(a, ws, ws_bytes, st);
+    int rc = launch_bwd_splitk_resident<RNN, CL>(a, ws, ws_bytes, st);
     if (rc != 1) return rc;
   }
   constexpr int UM = UT * CL;
@@ -2378,72 +2049,28 @@ static int launch_bwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   { int mrc = materialize_w_hh(a, st); if (mrc) return mrc; }   // this kernel streams the fp32 W_hh^T
   if (CL == 8 && ((a.B + 7) / 8 * 8) % 16 != 0) return 1;
   if (!vec_ok(a.gates, a.hseq, a.aux, a.dy)) return 1;
-  PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UM; p.G = G;
+  PersistParams p = sweep_params(a, UM, "DS2_TRACE_BWD", ws);
   if (p.NB > (CL == 8 ? 64 : 128)) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  p.training = 1;
-  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
-  p.trace = trace_ptr_from_env("DS2_TRACE_BWD");
   if (ws_bytes < 4096) return 1;
-  set_acc_layout(p);
-  p.err = static_cast<int*>(ws);
-  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + 128);
   const size_t smem = one_cta_per_sm(splitk_smem_bytes(p.NB, CL));
   if (smem > 227 * 1024) return 1;
-  auto kern = rnn_bwd_splitk_kernel<RNN, false, CL>;
+  const SweepKernel kern = rnn_bwd_splitk_kernel<RNN, false, CL>;
   static DeviceOnce attr_once;
-  if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_once.done();
-  }
-  int grid = a.D * p.NT * CL, launches = 1;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attrs[2];
-  attrs[0].id = cudaLaunchAttributeClusterDimension;
-  attrs[0].val.clusterDim.x = CL; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-  attrs[1].id = cudaLaunchAttributeCooperative;
-  attrs[1].val.cooperative = 1;
-  cfg.attrs = attrs;
-  // Nsight Compute cannot replay a cooperative cluster launch: DS2_SPLITK_NONCOOP=1 (profiling only) drops the
-  // cooperative attribute; co-residency is still checked with cudaOccupancyMaxActiveClusters below.
-  cfg.numAttrs = noncoop_cluster_launch() ? 1 : 2;
-  int max_clusters = 0;
-  cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg);
-  if (oe != cudaSuccess) { (void)cudaGetLastError(); return 1; }
-  if (max_clusters * CL < grid) {                        // all clusters must be co-resident (grid barrier)
-    if (CL == 8 || max_clusters * CL < p.NT * CL) return 1;
-    grid = p.NT * CL;                                    // one launch per direction
-    launches = a.D;
-    cfg.gridDim = dim3(grid);
-  }
-  for (int d = 0; d < a.D; ++d) {
-    int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, UM, BK);   // W_hh^T (H, G*H): UM unit rows per box
-    if (rc) return rc;
-    rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
-    if (rc) return rc;
-    if (RNN == DS2_RNN_GRU) {
-      rc = make_tmap_2d(&p.tmV2[d], a.aux + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
+  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
+  const int fit = cluster_fit(kern, CL, a.D * p.NT * CL, smem, st);
+  return launch_sweep(kern, CL, p.NT * CL, smem, fit, CL != 8, 4096, "split-K backward sweep", nullptr, p, st, [&] {
+    for (int d = 0; d < a.D; ++d) {
+      int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, UM, BK);   // W_hh^T (H, G*H): UM unit rows per box
       if (rc) return rc;
+      rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
+      if (rc) return rc;
+      if (RNN == DS2_RNN_GRU) {
+        rc = make_tmap_2d(&p.tmV2[d], a.aux + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
+        if (rc) return rc;
+      }
     }
-  }
-  DS2_CHECK_CUDA(cudaMemsetAsync(ws, 0, 4096, st));
-  for (int li = 0; li < launches; ++li) {
-    p.d0 = li;
-    cudaError_t le = cudaLaunchKernelEx(&cfg, kern, p);
-    if (le != cudaSuccess) {
-      (void)cudaGetLastError();
-      if (li == 0) return 1;                             // e.g. cooperative+cluster launch refused: 16-unit kernel
-      set_error("split-K backward sweep: second launch failed: %s", cudaGetErrorString(le));
-      return DS2_ERR_CUDA;
-    }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
-  return DS2_OK;
+    return 0;
+  });
 }
 
 template <int RNN>
@@ -2452,55 +2079,31 @@ static int launch_bwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t 
   const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
   const int GH = G * a.H;
   { int mrc = materialize_w_hh(a, st); if (mrc) return mrc; }   // fp32 W_hh^T through TMA
-  PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / UT; p.G = G;
+  PersistParams p = sweep_params(a, UT, "DS2_TRACE_BWD", ws);
   if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  p.training = 1;
-  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
-  p.trace = trace_ptr_from_env("DS2_TRACE_BWD");
   if (ws_bytes < 4096) return 1;
-  set_acc_layout(p);
-  p.err = static_cast<int*>(ws);
-  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + 128);
   const size_t smem = one_cta_per_sm(fwd_smem_bytes(p.NB));
-  auto kern = rnn_bwd_persist_kernel<RNN>;
-  static DeviceOnce attr_once;
-  const int num_sms = device_sm_count();
-  if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_once.done();
-  }
   if (smem > 227 * 1024) return 1;
-  int max_blocks_per_sm = 0;
-  DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&max_blocks_per_sm, kern, THREADS, smem));
-  int grid = a.D * p.NT, launches = 1;
-  if (max_blocks_per_sm < 1) return 1;
-  if (grid > max_blocks_per_sm * num_sms) {           // both directions do not fit: one launch per direction
-    if (p.NT > max_blocks_per_sm * num_sms) return 1;
-    grid = p.NT;
-    launches = a.D;
-  }
-  for (int d = 0; d < a.D; ++d) {
-    // a.w_hh[d] is the transposed recurrent matrix (H, G*H) here
-    int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, UT, BK);
-    if (rc) return rc;
-    // gate gradients: rows (t,b), full row width D*GH (the direction offset is a coordinate)
-    rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
-    if (rc) return rc;
-    if (RNN == DS2_RNN_GRU) {
-      rc = make_tmap_2d(&p.tmV2[d], a.aux + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
+  const SweepKernel kern = rnn_bwd_persist_kernel<RNN>;
+  static DeviceOnce attr_once;
+  int fit = 0;
+  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
+  if (int rc = coop_fit(kern, smem, &fit)) return rc;
+  return launch_sweep(kern, 0, p.NT, smem, fit, true, 4096, nullptr, nullptr, p, st, [&] {
+    for (int d = 0; d < a.D; ++d) {
+      // a.w_hh[d] is the transposed recurrent matrix (H, G*H) here
+      int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, UT, BK);
       if (rc) return rc;
+      // gate gradients: rows (t,b), full row width D*GH (the direction offset is a coordinate)
+      rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
+      if (rc) return rc;
+      if (RNN == DS2_RNN_GRU) {
+        rc = make_tmap_2d(&p.tmV2[d], a.aux + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
+        if (rc) return rc;
+      }
     }
-  }
-  DS2_CHECK_CUDA(cudaMemsetAsync(ws, 0, 4096, st));
-  for (int li = 0; li < launches; ++li) {
-    p.d0 = li;
-    void* args[] = {&p};
-    DS2_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3(grid), dim3(THREADS), args, smem, st));
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
-  return DS2_OK;
+    return 0;
+  });
 }
 
 int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {

@@ -341,15 +341,14 @@ def _one_layer(rnn, T, B, In, H, seed):
 
 @pytest.mark.parametrize("rnn,B", [("lstm", 32), ("lstm", 20), ("gru", 20), ("lstm", 40), ("gru", 48)])
 def test_tf32_sweep_variants_agree_with_the_fp32_path(rnn, B, monkeypatch):
-    """forward: 2-CTA split-K clusters vs 16-unit CTAs; backward: 8- vs 4-CTA clusters (LSTM, B = 32); grid barrier + TMA
-    (default) vs the flag-in-data exchange (DS2_FWD_LL / DS2_BWD_LL = 1); stores deferred past the barrier or not.  H = 256 takes every variant; B = 20 exercises the N padding (24 / 32 columns),
+    """forward: 2-CTA split-K clusters vs 16-unit CTAs; backward: 8- vs 4-CTA clusters (LSTM, B = 32); stores deferred
+    past the barrier or not.  H = 256 takes every variant; B = 20 exercises the N padding (24 / 32 columns),
     B > 32 the second pass of the epilogues over the batch columns."""
     run = _one_layer(rnn, T=33, B=B, In=192, H=256, seed=11)
     ds.set_precision("fp32")
     ref = run()
     ds.set_precision("tf32")
     variants = [{}, {"DS2_FWD_SPLITK": "0"}, {"DS2_SPLITK_CL": "4"}, {"DS2_SWEEP_DEFER": "0"},
-                {"DS2_FWD_LL": "1"}, {"DS2_BWD_LL": "1"}, {"DS2_FWD_LL": "1", "DS2_BWD_LL": "1", "DS2_SPLITK_CL": "4"},
                 {"DS2_FWD_SPLITK": "0", "DS2_SPLITK_CL": "4", "DS2_SWEEP_DEFER": "0"}]
     for env in variants:
         for k_, v in env.items():
