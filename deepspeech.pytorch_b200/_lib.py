@@ -58,6 +58,7 @@ PROTOTYPES = {
     "ds2_gemm_workspace_bytes": (sz, [i32] * 5),
     "ds2_gemm": (i32, [i32] * 5 + [f32, vp, i32, vp, i32, f32, vp, i32, vp, sz, vp]),
     "ds2_gemm_f16": (i32, [i32] * 3 + [f32, vp, i32, vp, i32, f32, vp, i32, vp]),
+    "ds2_gemm_f16_scaled": (i32, [i32] * 3 + [f32, vp, i32, vp, i32, f32, vp, i32, vp, vp]),
 }
 
 _lib = None

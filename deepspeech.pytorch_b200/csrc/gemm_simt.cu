@@ -172,11 +172,16 @@ int ds2_gemm(int transA, int transB, int M, int N, int K, float alpha, const flo
 
 // fp16-operand GEMM of the precision-16 mode, exported for tests / the roofline bench: A16 (M,K), B16 (N,K) K-major
 // halfs on the device, C fp32.  DS2_ERR_INVALID when the shape / alignment is not eligible (no fallback here).
-int ds2_gemm_f16(int M, int N, int K, float alpha, const void* A16, int lda, const void* B16, int ldb, float beta,
-                 float* C, int ldc, void* stream) {
+int ds2_gemm_f16_scaled(int M, int N, int K, float alpha, const void* A16, int lda, const void* B16, int ldb,
+                        float beta, float* C, int ldc, const float* alpha_dev, void* stream) {
   DS2_REQUIRE(M > 0 && N > 0 && K > 0 && A16 && B16 && C, "ds2_gemm_f16: bad arguments");
-  int r = ds2::gemm_tc_f16(M, N, K, alpha, A16, lda, B16, ldb, beta, C, ldc, nullptr, ds2::as_stream(stream));
+  int r = ds2::gemm_tc_f16(M, N, K, alpha, A16, lda, B16, ldb, beta, C, ldc, alpha_dev, ds2::as_stream(stream));
   DS2_REQUIRE(r != 1, "ds2_gemm_f16: shape %dx%dx%d / alignment not eligible for the fp16 tensor-core kernel", M, N, K);
   return r;
+}
+
+int ds2_gemm_f16(int M, int N, int K, float alpha, const void* A16, int lda, const void* B16, int ldb, float beta,
+                 float* C, int ldc, void* stream) {
+  return ds2_gemm_f16_scaled(M, N, K, alpha, A16, lda, B16, ldb, beta, C, ldc, nullptr, stream);
 }
 }

@@ -1,8 +1,9 @@
-// wgmma TF32 GEMM:  C[M,N] = alpha * A[M,K] . B[N,K]^T + beta * C   (both operands K-major).
+// wgmma TF32 / fp16 GEMM:  C[M,N] = alpha * A[M,K] . B[N,K]^T + beta * C   (both operands K-major).
 //
 //   warp 0       TMA producer: cp.async.bulk.tensor 2-D tiles (128B swizzle) of A (128 x 32 fp32) and
-//                B (128 x 32 fp32) into a 6-stage shared-memory ring, mbarrier complete_tx signalling
-//   warps 4..11  two MMA warpgroups: wgmma.mma_async m64n128k8 (tf32) x4 per stage on their 64-row half of
+//                B (BN x 32 fp32) into a 6-stage (BN = 128) or 4-stage (BN = 256) shared-memory ring, mbarrier
+//                complete_tx signalling
+//   warps 4..11  two MMA warpgroups: wgmma.mma_async m64nBNk8 (tf32) x4 per stage on their 64-row half of
 //                the A tile, fp32 accumulators in registers; the epilogue stores them (alpha / beta) to global
 //
 // Operands that are not K-major in memory (transA / !transB) are first transposed into the workspace.
@@ -144,13 +145,24 @@ int make_tmap_f16(CUtensorMap* out, const void* base, int rank, int d0, int d1, 
   return DS2_OK;
 }
 
-// ---- kernel ---------------------------------------------------------------------------------------
-// 128 x 128 output tile per CTA; a 128-byte swizzle row holds 32 fp32 (or 64 fp16) of K, one stage = one row of K
-// for both operand tiles (32 KB), six stages in flight.
+// ---- kernel ----------------------------------------------------------------------------------------
+// 128 x BN output tile per CTA; a 128-byte swizzle row holds 32 fp32 (or 64 fp16) of K, one stage = one row of K
+// for both operand tiles.  Two configurations, chosen on the host from N (`tile_n`):
+//   BN = 128: six 32 KB stages, wgmma m64n128 per warpgroup (N <= 128: the fc head, small shapes)
+//   BN = 256: four 48 KB stages (A 16 KB + B 32 KB), wgmma m64n256 per warpgroup (the recurrent stack's GEMMs):
+//             half the shared-memory operand reads per MMA of the 128 x 128 tile
 namespace gtc {
-constexpr int BM = 128, BN = 128, BK = 32, THREADS = 384, STAGES = 6;
-constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int BM = 128, BK = 32, THREADS = 384;
+// registers per thread after the producer warpgroup hands its surplus to the two MMA warpgroups: 128 x 40 + 256 x 232
+// = 384 x 168, the whole allotment of one CTA of 384 threads
+constexpr int PRODUCER_REGS = 40, MMA_REGS = 232;
+template <int BN>
+struct Cfg {
+  static constexpr int STAGES = BN == 256 ? 4 : 6;
+  static constexpr int A_BYTES = BM * 128, B_BYTES = BN * 128, STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+};
+static_assert(Cfg<256>::SMEM_BYTES <= 227 * 1024 && Cfg<128>::SMEM_BYTES <= 227 * 1024, "shared memory");
 }  // namespace gtc
 
 // gridDim.z > 1: split-K, every CTA adds its partial tile into C with vector atomics (C holds beta * C_old,
@@ -158,12 +170,16 @@ constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*b
 // F16 (precision-16 mode): fp16 operands, the same 128-byte rows hold 64 halfs, wgmma k16 instead of tf32 k8;
 // accumulation and C stay fp32.  `alpha_dev` (optional) multiplies alpha by a device-resident factor (the inverse of
 // the power-of-two scale of a scaled fp16 operand).
-template <bool F16>
+// The MMA warpgroups keep one wgmma group in flight: stage s is released once stage s + 1's group is issued and
+// stage s's has completed, so the tensor pipe does not drain between stages.  The products still reach every
+// accumulator in ascending K, one k-step after the other.
+template <bool F16, int BN>
 __global__ void __launch_bounds__(gtc::THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N, int K,
                float alpha, float beta, float* __restrict__ C, int ldc, const float* __restrict__ alpha_dev) {
   using namespace gtc;
   using namespace tc;
+  constexpr int STAGES = Cfg<BN>::STAGES, A_BYTES = Cfg<BN>::A_BYTES, STAGE_BYTES = Cfg<BN>::STAGE_BYTES;
   constexpr int BK = F16 ? 2 * gtc::BK : gtc::BK;         // K elements per stage (shadows gtc::BK)
   if (alpha_dev) alpha *= __ldg(alpha_dev);
   extern __shared__ uint8_t smem_raw[];
@@ -184,9 +200,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   __syncthreads();
 
-  if (warp == 0) {
-    // TMA producer
-    if (lane == 0) {
+  if (warp < 4) {
+    // TMA producer (one thread of warpgroup 0)
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
       for (int it = 0; it < nk; ++it) {
         const int kb = kb0 + it, s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
@@ -197,12 +214,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         tma_load_2d(sa + A_BYTES, &tmB, &full[s], kb * BK, n0);
       }
     }
-  } else if (warp >= 4) {
+  } else {
     // two MMA warpgroups, 64 rows of the tile each; the accumulators stay in registers for the epilogue
+    setmaxnreg_inc<MMA_REGS>();
     const int wg = warp / 4 - 1;
-    float acc[64];
+    const bool leader = (threadIdx.x & 127) == 0;
+    float acc[BN / 2];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     for (int it = 0; it < nk; ++it) {
       const int s = it % STAGES;
       mbar_wait(&full[s], (it / STAGES) & 1);
@@ -212,8 +231,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
       for (int k = 0; k < 4; ++k)          // four 32-byte k-steps per 128-byte row (K = 8 tf32 / 16 fp16)
         Wgmma<BN, F16>::mma(acc, adesc + 2 * k, bdesc + 2 * k, 1u);
-      wg_release(&empty[s]);
+      wg_commit();
+      wg_wait<1>();                        // the previous stage's group has read its operands
+      if (it > 0 && leader) mbar_arrive(&empty[(it - 1) % STAGES]);
     }
+    wg_wait<0>();
+    if (nk > 0 && leader) mbar_arrive(&empty[(nk - 1) % STAGES]);
     if (nk > 0) {
       // fragment: rows 16 w + l/4 (+8), column pairs 8 i + 2 (l%4)
       const int w = warp % 4;
@@ -299,20 +322,31 @@ static int choose_splits(const char* env, float beta) {
   return 1;
 }
 
-template <bool F16>
+// columns of the output tile: 256 wherever N needs more than one 128-column tile
+static int tile_n(int N) { return N > 128 ? 256 : 128; }
+
+template <bool F16, int BN>
 static int launch_gemm_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, float alpha, float beta,
-                          float* C, int ldc, int splits, cudaStream_t st, const float* alpha_dev = nullptr) {
-  auto kern = gemm_tc_kernel<F16>;
+                          float* C, int ldc, int splits, cudaStream_t st, const float* alpha_dev) {
+  auto kern = gemm_tc_kernel<F16, BN>;
+  constexpr int smem = gtc::Cfg<BN>::SMEM_BYTES;
   static DeviceOnce attr_once;
   if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, gtc::SMEM_BYTES));
+    DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_once.done();
   }
   if (splits > 1 && beta == 0.f)
     DS2_CHECK_CUDA(cudaMemset2DAsync(C, (size_t)ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, st));
-  dim3 grid(cdiv(N, gtc::BN), cdiv(M, gtc::BM), splits);
-  DS2_LAUNCH(kern, grid, gtc::THREADS, gtc::SMEM_BYTES, st, tmA, tmB, M, N, K, alpha, beta, C, ldc, alpha_dev);
+  dim3 grid(cdiv(N, BN), cdiv(M, gtc::BM), splits);
+  DS2_LAUNCH(kern, grid, gtc::THREADS, smem, st, tmA, tmB, M, N, K, alpha, beta, C, ldc, alpha_dev);
   return DS2_OK;
+}
+
+template <bool F16>
+static int launch_gemm_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, float alpha, float beta,
+                          float* C, int ldc, int splits, cudaStream_t st, const float* alpha_dev = nullptr) {
+  if (tile_n(N) == 256) return launch_gemm_tc<F16, 256>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st, alpha_dev);
+  return launch_gemm_tc<F16, 128>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st, alpha_dev);
 }
 
 // TF32 wgmma reads both operands K-major: an operand stored the other way round (transA / !transB) is first
@@ -347,7 +381,7 @@ int gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const floa
   CUtensorMap tmA, tmB;
   int rc = make_tmap_2d(&tmA, Ak, M, K, ldak, gtc::BM, gtc::BK);
   if (rc) return rc;
-  rc = make_tmap_2d(&tmB, Bk, N, K, ldbk, gtc::BN, gtc::BK);
+  rc = make_tmap_2d(&tmB, Bk, N, K, ldbk, tile_n(N), gtc::BK);
   if (rc) return rc;
   return launch_gemm_tc<false>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st);
 }
@@ -362,7 +396,7 @@ int gemm_tc_f16(int M, int N, int K, float alpha, const void* A16, int lda, cons
   CUtensorMap tmA, tmB;
   int rc = make_tmap_f16(&tmA, A16, 2, K, M, 1, (size_t)lda, 0, 64, gtc::BM, 1);
   if (rc) return rc;
-  rc = make_tmap_f16(&tmB, B16, 2, K, N, 1, (size_t)ldb, 0, 64, gtc::BN, 1);
+  rc = make_tmap_f16(&tmB, B16, 2, K, N, 1, (size_t)ldb, 0, 64, tile_n(N), 1);
   if (rc) return rc;
   return launch_gemm_tc<true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st, alpha_dev);
 }

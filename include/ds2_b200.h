@@ -261,6 +261,10 @@ int ds2_gemm(int transA, int transB, int M, int N, int K, float alpha, const flo
  * device, C = alpha * A16 . B16^T + beta * C in fp32.  lda / ldb multiples of 8, 16-byte aligned bases.       */
 int ds2_gemm_f16(int M, int N, int K, float alpha, const void* A16, int lda, const void* B16, int ldb, float beta,
                  float* C, int ldc, void* stream);
+/* the same with alpha multiplied by *alpha_dev, a float on the device (the layers pass the inverse of the
+ * power-of-two scale of a scaled fp16 operand this way); alpha_dev may be NULL.                                */
+int ds2_gemm_f16_scaled(int M, int N, int K, float alpha, const void* A16, int lda, const void* B16, int ldb,
+                        float beta, float* C, int ldc, const float* alpha_dev, void* stream);
 
 #ifdef __cplusplus
 }
