@@ -1,44 +1,70 @@
 // BatchNorm over the rows of a (rows, F) matrix: the SequenceWise(BatchNorm1d) of the reference
 // (model.py:18-33, :86 per RNN layer, :196 in the fc head).  Statistics are over ALL T*B rows,
-// padded rows included (SURVEY.md §8c quirks).  Column sums are accumulated in double to avoid
-// E[x^2]-E[x]^2 cancellation.
+// padded rows included (SURVEY.md §8c quirks).
+//
+// Forward statistics: E[x^2] - E[x]^2 from raw sums (fp32 partials of 64 rows, flushed into double) cancels on
+// near-constant features, which is what saturated LSTM units feed the next layer (the sum of the two directions of h
+// sits near +-2 with a tiny spread): for mean 10 and std 0.001 the variance is 1e-8 of E[x^2], below fp32 rounding.
+// So the forward pass also sums (x - K) and (x - K)^2 in double per element, with K = the feature's first row:
+// mean = K + S1/n, var = S2/n - (S1/n)^2, where S2/n stays within a small factor of (S1/n)^2.  The raw result is kept
+// wherever it is accurate, E[x^2] <= RAW_MAX_CANCEL * var (raw variance error there: about 1e-6 relative, typical),
+// so a well-conditioned feature gets exactly the bits it always had: a last-bit change in the statistics, carried
+// through fp16 operand copies and AdamW, moves the loss of the benchmark step by 0.1 % after 11 steps.  Every feature
+// of the benchmark's model is well-conditioned (E[x^2] / var <= 18).  The FP64 adds are hidden under the loads.
 #include "common.cuh"
 
 namespace ds2 {
 
+constexpr double RAW_MAX_CANCEL = 256.0;
+
 // blockDim = (32, 8): 32 consecutive features x 8 row lanes; grid = (ceil(F/32), row_chunks)
 __global__ void bn_colsum_kernel(int rows, int F, const float* __restrict__ a, const float* __restrict__ b,
-                                 double* __restrict__ sums) {
+                                 const float* __restrict__ pivot, double* __restrict__ sums) {
   // sums[0..F) += sum_r a ; sums[F..2F) += sum_r a*b   (b == a for the forward statistics)
-  __shared__ double s1[8][33], s2[8][33];
+  // with a pivot (forward statistics): sums[2F..3F) += sum_r (a - K), sums[3F..4F) += sum_r (a - K)^2, K = pivot[f]
+  __shared__ double s[4][8][33];
   int f = blockIdx.x * 32 + threadIdx.x;
   int rows_per = cdiv_dev(rows, gridDim.y);
   int r0 = blockIdx.y * rows_per, r1 = min(rows, r0 + rows_per);
   float p1 = 0.f, p2 = 0.f;
-  double d1 = 0.0, d2 = 0.0;
+  double d1 = 0.0, d2 = 0.0, e1 = 0.0, e2 = 0.0;
   int cnt = 0;
   if (f < F) {
+    const double k = pivot ? (double)pivot[f] : 0.0;
     for (int r = r0 + threadIdx.y; r < r1; r += 8) {
       float va = a[(size_t)r * F + f], vb = b[(size_t)r * F + f];
       p1 += va;
       p2 = fmaf(va, vb, p2);
+      if (pivot) {
+        const double d = (double)va - k;
+        e1 += d;
+        e2 = fma(d, d, e2);
+      }
       if (++cnt == 64) {  // flush the fp32 partials into double every 64 rows
         d1 += p1; d2 += p2; p1 = p2 = 0.f; cnt = 0;
       }
     }
     d1 += p1; d2 += p2;
   }
-  s1[threadIdx.y][threadIdx.x] = d1;
-  s2[threadIdx.y][threadIdx.x] = d2;
+  s[0][threadIdx.y][threadIdx.x] = d1;
+  s[1][threadIdx.y][threadIdx.x] = d2;
+  s[2][threadIdx.y][threadIdx.x] = e1;
+  s[3][threadIdx.y][threadIdx.x] = e2;
   __syncthreads();
   if (threadIdx.y == 0 && f < F) {
-    for (int i = 1; i < 8; ++i) { d1 += s1[i][threadIdx.x]; d2 += s2[i][threadIdx.x]; }
+    for (int i = 1; i < 8; ++i) { d1 += s[0][i][threadIdx.x]; d2 += s[1][i][threadIdx.x]; }
     atomicAdd(&sums[f], d1);
     atomicAdd(&sums[F + f], d2);
+    if (pivot) {
+      for (int i = 1; i < 8; ++i) { e1 += s[2][i][threadIdx.x]; e2 += s[3][i][threadIdx.x]; }
+      atomicAdd(&sums[2 * F + f], e1);
+      atomicAdd(&sums[3 * F + f], e2);
+    }
   }
 }
 
-__global__ void bn_finalize_kernel(int F, double count, const double* __restrict__ sums, float* __restrict__ rmean,
+__global__ void bn_finalize_kernel(int F, double count, const double* __restrict__ sums,
+                                   const float* __restrict__ pivot, float* __restrict__ rmean,
                                    float* __restrict__ rvar, int training, float momentum, float eps,
                                    float* __restrict__ mean_invstd) {
   int f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -48,6 +74,13 @@ __global__ void bn_finalize_kernel(int F, double count, const double* __restrict
     double m = sums[f] / count;
     double v = sums[F + f] / count - m * m;
     if (v < 0.0) v = 0.0;
+    const double ms = sums[2 * F + f] / count;  // mean - K
+    double vs = sums[3 * F + f] / count - ms * ms;
+    if (vs < 0.0) vs = 0.0;
+    if (!(sums[F + f] / count <= RAW_MAX_CANCEL * vs)) {  // the raw sums cancel: take the pivoted ones
+      m = (double)pivot[f] + ms;
+      v = vs;
+    }
     mean = (float)m;
     var = (float)v;
     double unbiased = count > 1.0 ? v * count / (count - 1.0) : v;
@@ -104,11 +137,11 @@ int bn_rows_fwd(int rows, int F, const float* x, const float* gamma, const float
                 int training, float momentum, float eps, float* y, float* xhat, float* mean_invstd,
                 double* ws_sums, cudaStream_t st) {
   if (training) {
-    DS2_CHECK_CUDA(cudaMemsetAsync(ws_sums, 0, sizeof(double) * 2 * F, st));
+    DS2_CHECK_CUDA(cudaMemsetAsync(ws_sums, 0, sizeof(double) * 4 * F, st));
     dim3 grid(cdiv(F, 32), colsum_grid_y(rows)), block(32, 8);
-    DS2_LAUNCH(bn_colsum_kernel, grid, block, 0, st, rows, F, x, x, ws_sums);
+    DS2_LAUNCH(bn_colsum_kernel, grid, block, 0, st, rows, F, x, x, x /* pivot: row 0 */, ws_sums);
   }
-  DS2_LAUNCH(bn_finalize_kernel, cdiv(F, 128), 128, 0, st, F, (double)rows, ws_sums, rmean, rvar, training, momentum,
+  DS2_LAUNCH(bn_finalize_kernel, cdiv(F, 128), 128, 0, st, F, (double)rows, ws_sums, x, rmean, rvar, training, momentum,
              eps, mean_invstd);
   size_t total = (size_t)rows * F;
   int blocks = (int)((total + 1023) / 1024);
@@ -132,7 +165,7 @@ int bn_rows_bwd(int rows, int F, const float* xhat, const float* gamma, const fl
                 float* dx, float* dgamma, float* dbeta, double* ws_sums, cudaStream_t st) {
   DS2_CHECK_CUDA(cudaMemsetAsync(ws_sums, 0, sizeof(double) * 2 * F, st));
   dim3 grid(cdiv(F, 32), colsum_grid_y(rows)), block(32, 8);
-  DS2_LAUNCH(bn_colsum_kernel, grid, block, 0, st, rows, F, dy, xhat, ws_sums);
+  DS2_LAUNCH(bn_colsum_kernel, grid, block, 0, st, rows, F, dy, xhat, nullptr, ws_sums);
   DS2_LAUNCH(bn_bwd_params_kernel, cdiv(F, 128), 128, 0, st, F, ws_sums, dgamma, dbeta);
   size_t total = (size_t)rows * F;
   int blocks = (int)((total + 1023) / 1024);

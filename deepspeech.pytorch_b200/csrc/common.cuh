@@ -140,7 +140,7 @@ int pow2_scale_for(int rows, int cols, const float* x, size_t ld, unsigned int* 
 // y = (x-mean)*invstd*gamma+beta ; xhat optionally stored.
 int bn_rows_fwd(int rows, int F, const float* x, const float* gamma, const float* beta, float* rmean, float* rvar,
                 int training, float momentum, float eps, float* y, float* xhat, float* mean_invstd /*2F*/,
-                double* ws_sums /*2F doubles*/, cudaStream_t st);
+                double* ws_sums /*4F doubles*/, cudaStream_t st);
 // y / xhat again from saved statistics (backward recomputation)
 int bn_rows_reapply(int rows, int F, const float* x, const float* gamma, const float* beta,
                     const float* mean_invstd, float* y, float* xhat, cudaStream_t st);

@@ -251,7 +251,7 @@ int ds2_lookahead_bwd(int T, int B, int H, int ctx, const float* x, const float*
 }
 
 size_t ds2_fc_head_workspace_bytes(int rows, int H, int C) {
-  return align_up((size_t)rows * H * 4, 256) + align_up((size_t)2 * H * 8, 256) +
+  return align_up((size_t)rows * H * 4, 256) + align_up((size_t)4 * H * 8, 256) +
          ds2_gemm_workspace_bytes(1, 0, C, H, rows) + 4096;
 }
 
@@ -264,7 +264,7 @@ int ds2_fc_head_fwd(int rows, int H, int C, const float* x, const float* g, cons
   Arena ar(ws, ws_bytes);
   DS2_PROF("fc_fwd", st);
   float* xbn = ar.take<float>((size_t)rows * H);
-  double* sums = ar.take<double>(2 * (size_t)H);
+  double* sums = ar.take<double>(4 * (size_t)H);
   int r = bn_rows_fwd(rows, H, x, g, b, rmean, rvar, training, momentum, eps, xbn, xhat, stats, sums, st);
   if (r) return r;
   r = ds2_gemm(0, 1, rows, C, H, 1.f, xbn, H, w, H, 0.f, logits, C, ar.base + ar.off, ar.cap - ar.off, stream);

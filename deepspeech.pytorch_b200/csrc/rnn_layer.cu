@@ -320,7 +320,7 @@ size_t ds2_rnn_workspace_bytes(const ds2_rnn_desc* d) {
   const size_t TB = (size_t)d->T * d->B, GH = G * d->H;
   size_t n = 0;
   n += 3 * align_up(TB * d->In * 4, 256);                 // xbn, xhat, dxbn
-  n += align_up(2 * (size_t)d->In * 8, 256);              // BN double sums
+  n += align_up(4 * (size_t)d->In * 8, 256);              // BN double sums
   n += D * align_up(GH * d->H * 4, 256);                  // W_hh^T per direction
   n += align_up(D * (size_t)d->B * d->H * 4, 256);        // carry
   if (f16_gemm_mode()) {
@@ -357,7 +357,7 @@ int ds2_rnn_layer_fwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
   const float* xin = x;
   if (bn_gamma) {
     float* xbn = ar.take<float>((size_t)TB * In);
-    double* sums = ar.take<double>(2 * (size_t)In);
+    double* sums = ar.take<double>(4 * (size_t)In);
     rc = bn_rows_fwd(TB, In, x, bn_gamma, bn_beta, bn_rmean, bn_rvar, d->training, d->bn_momentum, d->bn_eps, xbn,
                      nullptr, R.bnstats, sums, st);
     if (rc) return rc;

@@ -305,7 +305,7 @@ def ctc_loss_and_grad(logits: np.ndarray, targets: np.ndarray, input_lengths, ta
             for t in range(1, Tb):
                 a0 = la[t - 1]
                 a1 = np.concatenate(([-np.inf], a0[:-1]))
-                a2 = np.where(can_skip, np.concatenate(([-np.inf, -np.inf], a0[:-2])), -np.inf)
+                a2 = np.where(can_skip, np.concatenate(([-np.inf, -np.inf], a0))[:S], -np.inf)   # [:S]: also S = 1
                 la[t] = _lse(a0, a1, a2) + lp[t, b, ext]
             ll = _lse(la[Tb - 1, S - 1], la[Tb - 1, S - 2] if S > 1 else np.float64(-np.inf))
             nll[b] = -float(ll)
@@ -324,7 +324,7 @@ def ctc_loss_and_grad(logits: np.ndarray, targets: np.ndarray, input_lengths, ta
         for t in range(Tb - 2, -1, -1):
             b0 = lb[t + 1]
             b1 = np.concatenate((b0[1:], [-np.inf]))
-            b2 = np.where(skip_fwd, np.concatenate((b0[2:], [-np.inf, -np.inf])), -np.inf)
+            b2 = np.where(skip_fwd, np.concatenate((b0[2:], [-np.inf, -np.inf]))[:S], -np.inf)
             lb[t] = _lse(b0, b1, b2) + lp[t, b, ext]
         # posterior[t,c] = sum_{s: ext[s]=c} exp(la+lb - lp[t,c] + nll)
         lab = la + lb
@@ -365,7 +365,7 @@ def train_step(inputs, targets, input_percentages, target_sizes, P, cfg: OracleC
 
 
 # ----------------------------------------------------------------------------- greedy decode (N2)
-def greedy_path(probs: torch.Tensor, sizes) -> List[Tuple[List[int], List[int]]]:
+def greedy_path(probs: torch.Tensor, sizes, blank: int = 0) -> List[Tuple[List[int], List[int]]]:
     """reference decoder.py:144-181 as integers: argmax -> drop blank -> collapse repeats;
     returns per utterance (label indices, frame offsets)."""
     am = probs.argmax(2)
@@ -375,7 +375,7 @@ def greedy_path(probs: torch.Tensor, sizes) -> List[Tuple[List[int], List[int]]]
         lab, offs = [], []
         for i in range(n):
             c = int(am[b, i])
-            if c != 0 and not (i != 0 and c == int(am[b, i - 1])):
+            if c != blank and not (i != 0 and c == int(am[b, i - 1])):
                 lab.append(c), offs.append(i)
         res.append((lab, offs))
     return res
