@@ -4,7 +4,7 @@ python >= 3.11 (the reference's mutable dataclass defaults at :41,:87-89 are not
 without hydra/omegaconf installed."""
 from dataclasses import dataclass, field
 
-from .enums import RNNType, SpectrogramWindow
+from .enums import DecoderType, RNNType, SpectrogramWindow
 
 
 @dataclass
@@ -65,6 +65,20 @@ class DataConfig:
     spect: SpectConfig = field(default_factory=SpectConfig)
     augmentation: AugmentationConfig = field(default_factory=AugmentationConfig)
     prepare_data_per_node: bool = True
+
+
+@dataclass
+class LMConfig:
+    """deepspeech_pytorch/configs/inference_config.py:7-16 (the decoder settings of evaluation and transcription)"""
+    decoder_type: DecoderType = DecoderType.greedy
+    lm_path: str = ''           # KenLM model for beam search: not supported here (BeamCTCDecoder raises)
+    top_paths: int = 1          # number of beams to return
+    alpha: float = 0.0          # language-model weight (no effect without a language model)
+    beta: float = 0.0           # word bonus (no effect without a language model)
+    cutoff_top_n: int = 40      # characters with the highest probabilities considered per frame
+    cutoff_prob: float = 1.0    # cumulative-probability pruning; 1.0 = none
+    beam_width: int = 10
+    lm_workers: int = 4         # ctcdecode's CPU worker count; ignored by the GPU decoder
 
 
 def cfg_type(cfg):

@@ -1,0 +1,506 @@
+// Prefix beam search for CTC without a language model (row N5): what the reference's BeamCTCDecoder
+// (decoder.py:56-118) gets from ctcdecode.CTCBeamDecoder with an empty lm_path, on the GPU.
+//
+// The decoder is defined by these rules (oracle/beam_oracle.py and DESIGN.md §5.7 carry the same text; ctcdecode's
+// algorithm with ext_scorer == nullptr, deviating only where its behaviour is order-dependent or degenerate, (!)):
+//
+// All path arithmetic is in float64 log space, with lp[c] = log((double) p[c]) and log 0 = -inf.  lse(a, b) is a
+// log-sum-exp that returns -inf when both arguments are -inf, and never NaN.  (!) ctcdecode keeps path probabilities
+// in fp32; fp64 here makes GPU and oracle agree to rounding of the last bits, so list order can be tested exactly.
+//  1. State.  An ordered list of at most W prefixes, each with log_b, log_nb and score = lse(log_b, log_nb).  Before
+//     frame 0 the list is {empty prefix: log_b = 0, log_nb = -inf}.
+//  2. Prefix identity is by content: the same label sequence is never in the list twice.  A prefix that falls out of
+//     the list and is produced again later is the same prefix: its probabilities restart from the new contributions,
+//     but it keeps its timestep record (rule 7) -- ctcdecode's trie node coming back with exists_ = true.  A prefix's
+//     parent is its sequence minus the last label.
+//  3. Character pruning per frame.  If cutoff_prob < 1 or cutoff_top_n < C: order the characters by (p desc, index
+//     asc).  With cutoff_prob < 1, take characters in that order, accumulating p in fp64, until the cumulative sum is
+//     >= cutoff_prob or cutoff_top_n characters are taken; otherwise take the first cutoff_top_n characters.  In all
+//     other cases the kept set K is every character.  The blank can be pruned; it then contributes nothing that frame.
+//  4. Candidates at frame t.  For each listed prefix j, with last label l_j, and its parent pi if the parent is in the
+//     list, the stay candidate is  b' = lp[blank] + score_j if blank in K, else -inf;
+//     nb' = lse(lp[l_j] + nb_j, lp[l_j] + (b_pi if l_pi = l_j else score_pi)), each term present only if l_j in K, and
+//     the second only if pi is listed (the empty prefix has no nb terms).  For each listed prefix i and each c in K,
+//     c != blank, where i + c is not in the list, the new candidate is  b' = -inf, nb' = lp[c] + (b_i if c = l_i else
+//     score_i).
+//  5. Selection.  Drop candidates whose score is -inf ((!) ctcdecode can return -inf prefixes when fewer than W finite
+//     ones exist).  Order the rest by (score desc, origin asc), the origin being (j, -1) for the stay candidate of list
+//     position j and (i, c) for a new candidate ((!) a total order, so ties are defined).  The first W candidates
+//     become the new list, in that order.
+//  6. Output.  Per utterance, the final list in its order, with each prefix's labels and per-label timesteps; its
+//     reported score is -lse(log_b, log_nb) (ctcdecode's sign: a negative log-likelihood, lower is better).
+//     n_beams[b] <= W; unused slots have length 0 and score +inf.  sizes[b] = 0 gives one empty beam with score 0.
+//  7. Timesteps.  A label's timestep is the frame at which its prefix was first created, with best = that frame's lp.
+//     It moves to a later frame t when, at t, the listed parent is extended by the same label with a strictly larger
+//     lp than the recorded best (ctcdecode's get_path_trie rule as we read it; not verifiable here).
+// Read where the rules leave room (as the oracle does): "created" = first entry into the list; the rule-7 move is
+// checked for listed prefixes with a listed parent and l_j in K (the stay candidate's second term), whether or not the
+// stay survives selection, and a returning prefix keeps its record unchanged; reported timesteps are the records of
+// the prefix's ancestors at the end of the utterance (ctcdecode's get_path_vec walk).  NaN scores count as -inf.
+//
+// Kernel: one CTA per utterance, the list in shared memory.  Per frame:
+//  A. warp 0 loads the C <= 64 probabilities, takes logs and prunes (ranks by (p desc, index asc); the cutoff_prob
+//     sum is one sequential fp64 loop in that order, as in the oracle, so both round alike);
+//  B. every candidate gets a 64-bit key at a dense position e = i * S + s (S = 1 + |K \ {blank}|, s = 0 the stay of i,
+//     s >= 1 the s-th kept non-blank character in ascending index), so e ascending IS origin ascending.  The key is the
+//     order-reversing 64-bit image of the fp64 score (ascending key = descending score), all ones for a dropped
+//     candidate.  "Is i + c listed?" is a per-slot 64-bit child mask rebuilt each frame from the parent slots;
+//  C. the W smallest (key, e) pairs are found by an MSB-first radix select (8 bits per pass over the key, then 7 + 7
+//     over e; it stops as soon as the boundary bucket is taken whole, usually after 2-4 passes), then ranked by
+//     counting (<= W^2 comparisons) into list order;
+//  D. the new list: a new candidate looks up (parent node, label) in the utterance's hash, so a returning prefix finds
+//     its old node (rule 2); otherwise it takes the next node of the pool (ids in list order).  Parent slots and child
+//     masks of the new list come from a W x W node comparison.
+// Nothing is decided by an atomic: shared atomics only count (histograms, compaction before the rank sort, child
+// masks), and the hash's slot claims do not change what a lookup returns.  The final beams are written by walking
+// parent pointers through the pool.
+
+#include <math_constants.h>
+
+#include "common.cuh"
+
+namespace ds2 {
+
+namespace {
+
+constexpr int BEAM_THREADS = 512;
+constexpr int BEAM_MAX_W = 128, BEAM_MAX_C = 64;
+constexpr unsigned long long KEY_DROPPED = ~0ull;
+
+// Per-utterance node pool (NP = T*W + 1 nodes, node 0 = the empty prefix) and (parent, label) -> node hash.
+struct BeamPool {
+  int* parent;
+  int* label;
+  int* ts;
+  int* depth;
+  double* best;
+  unsigned long long* hkey;   // 0 = empty slot
+  int* hval;
+  long long NP, HC;           // HC: power of two >= 2 NP
+};
+
+void pool_sizes(int T, int W, long long* NP, long long* HC) {
+  *NP = (long long)T * W + 1;
+  long long h = 1;
+  while (h < 2 * *NP) h <<= 1;
+  *HC = h;
+}
+
+size_t dyn_smem_bytes(int W, int C) {
+  return (size_t)W * C * 8          // keys
+         + (size_t)W * 8 * 8        // lb, lnb, sc, sb, snb, b2, nb2, child masks
+         + (size_t)W * 4 * 10;      // lab, node, pnode, pslot, lab2, node2, pnode2, sel, rnk, ord
+}
+
+__device__ __forceinline__ double lse(double a, double b) {
+  const double m = fmax(a, b);
+  if (m == -CUDART_INF) return -CUDART_INF;
+  return m + log1p(exp(-fabs(a - b)));
+}
+
+// ascending key = descending score; +0 and -0 map alike
+__device__ __forceinline__ unsigned long long score_key(double s) {
+  if (!(s > -CUDART_INF)) return KEY_DROPPED;                      // -inf and NaN are dropped (rule 5)
+  const unsigned long long u = (unsigned long long)__double_as_longlong(s + 0.0);
+  const unsigned long long asc = (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+  return ~asc;
+}
+
+__device__ __forceinline__ unsigned long long hash_key(int pnode, int c) {
+  return (((unsigned long long)pnode << 6) | (unsigned)c) + 1ull;
+}
+__device__ __forceinline__ long long hash_slot(unsigned long long k, long long HC) {
+  k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
+  return (long long)(k & (unsigned long long)(HC - 1));
+}
+
+__global__ void __launch_bounds__(BEAM_THREADS)
+beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t* __restrict__ out_len, int blank,
+                   int W, int top_n, float cutoff_prob, int32_t* __restrict__ labels, int32_t* __restrict__ timesteps,
+                   int32_t* __restrict__ lengths, double* __restrict__ scores, int32_t* __restrict__ n_beams,
+                   BeamPool pool) {
+  const int u = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  unsigned long long* key = reinterpret_cast<unsigned long long*>(smem_raw);
+  double* lb = reinterpret_cast<double*>(key + (size_t)W * C);
+  double* lnb = lb + W;
+  double* sc = lnb + W;
+  double* sb = sc + W;
+  double* snb = sb + W;
+  double* b2 = snb + W;
+  double* nb2 = b2 + W;
+  unsigned long long* kids = reinterpret_cast<unsigned long long*>(nb2 + W);
+  int* lab = reinterpret_cast<int*>(kids + W);
+  int* node = lab + W;
+  int* pnode = node + W;
+  int* pslot = pnode + W;
+  int* lab2 = pslot + W;
+  int* node2 = lab2 + W;
+  int* pnode2 = node2 + W;
+  int* sel = pnode2 + W;
+  int* rnk = sel + W;
+  int* ord = rnk + W;
+
+  __shared__ double lp[BEAM_MAX_C];
+  __shared__ float pf[BEAM_MAX_C];
+  __shared__ int ordc[BEAM_MAX_C];
+  __shared__ int knb[BEAM_MAX_C];
+  __shared__ int hist[256];
+  __shared__ unsigned warp_new[BEAM_MAX_W / 32];
+  __shared__ unsigned long long kmask, pre_hi;
+  __shared__ int n_list, nK, n_valid, n_sel, need, passes, done, pre_e, pool_next;
+
+  const long long NP = pool.NP, HC = pool.HC;
+  int* P_par = pool.parent + (size_t)u * NP;
+  int* P_lab = pool.label + (size_t)u * NP;
+  int* P_ts = pool.ts + (size_t)u * NP;
+  int* P_depth = pool.depth + (size_t)u * NP;
+  double* P_best = pool.best + (size_t)u * NP;
+  unsigned long long* hk = pool.hkey + (size_t)u * HC;
+  int* hv = pool.hval + (size_t)u * HC;
+
+  for (long long i = tid; i < HC; i += BEAM_THREADS) hk[i] = 0ull;
+  const int Tu = out_len ? min(max(out_len[u], 0), T) : T;
+  if (tid == 0) {
+    P_par[0] = -1; P_lab[0] = -1; P_ts[0] = 0; P_depth[0] = 0; P_best[0] = -CUDART_INF;
+    lb[0] = 0.0; lnb[0] = -CUDART_INF; sc[0] = 0.0;
+    lab[0] = -1; node[0] = 0; pnode[0] = -1; pslot[0] = -1; kids[0] = 0ull;
+    n_list = 1; pool_next = 1;
+  }
+  __syncthreads();
+
+  const bool prune = cutoff_prob < 1.f || top_n < C;
+  for (int t = 0; t < Tu; ++t) {
+    // ---- A. probabilities, logs, the kept set K (rule 3)
+    if (warp == 0) {
+      const float* p = probs + ((size_t)u * T + t) * C;
+      for (int c = lane; c < C; c += 32) {
+        const float v = p[c];
+        pf[c] = v;
+        lp[c] = log((double)v);
+      }
+      __syncwarp();
+      bool keep0 = true, keep1 = true;
+      if (prune) {
+        int r0 = 0, r1 = 0;
+        const int c0 = lane, c1 = lane + 32;
+        const float v0 = c0 < C ? pf[c0] : 0.f, v1 = c1 < C ? pf[c1] : 0.f;
+        for (int k = 0; k < C; ++k) {
+          const float w = pf[k];
+          r0 += (w > v0 || (w == v0 && k < c0));
+          r1 += (w > v1 || (w == v1 && k < c1));
+        }
+        if (c0 < C) ordc[r0] = c0;
+        if (c1 < C) ordc[r1] = c1;
+        __syncwarp();
+        int nkeep = min(top_n, C);
+        if (cutoff_prob < 1.f) {
+          if (lane == 0) {
+            const double thr = (double)cutoff_prob;
+            double cum = 0.0;
+            int m = 0;
+            while (m < C) {
+              cum += (double)pf[ordc[m]];
+              ++m;
+              if (cum >= thr || m >= top_n) break;
+            }
+            nkeep = m;
+          }
+          nkeep = __shfl_sync(0xffffffffu, nkeep, 0);
+        }
+        keep0 = r0 < nkeep;
+        keep1 = r1 < nkeep;
+      }
+      const unsigned m0 = __ballot_sync(0xffffffffu, lane < C && keep0);
+      const unsigned m1 = __ballot_sync(0xffffffffu, lane + 32 < C && keep1);
+      const unsigned long long km = ((unsigned long long)m1 << 32) | m0;
+      const unsigned long long nbm = km & ~(1ull << blank);
+      const unsigned long long lt = (1ull << lane) - 1ull;
+      if ((nbm >> lane) & 1ull) knb[__popcll(nbm & lt)] = lane;
+      if ((nbm >> (lane + 32)) & 1ull) knb[__popcll(nbm & ((lt << 32) | 0xffffffffull))] = lane + 32;
+      if (lane == 0) {
+        kmask = km;
+        nK = __popcll(nbm);
+        n_valid = 0;
+        n_sel = 0;
+      }
+    }
+    if (tid < W) rnk[tid] = 0;
+    __syncthreads();
+
+    // ---- B. candidate keys (rule 4); the timestep move of rule 7
+    const int n = n_list, S = 1 + nK, N = n * S;
+    const unsigned long long km = kmask;
+    const bool blank_in = (km >> blank) & 1ull;
+    int valid = 0;
+    for (int e = tid; e < N; e += BEAM_THREADS) {
+      const int i = e / S, s = e - i * S;
+      double v;
+      if (s == 0) {
+        const double bb = blank_in ? lp[blank] + sc[i] : -CUDART_INF;
+        double nn = -CUDART_INF;
+        const int l = lab[i];
+        if (l >= 0 && ((km >> l) & 1ull)) {
+          const double lpl = lp[l];
+          nn = lpl + lnb[i];
+          const int pi = pslot[i];
+          if (pi >= 0) {
+            nn = lse(nn, lpl + (lab[pi] == l ? lb[pi] : sc[pi]));
+            const int nd = node[i];
+            if (lpl > P_best[nd]) { P_best[nd] = lpl; P_ts[nd] = t; }
+          }
+        }
+        sb[i] = bb;
+        snb[i] = nn;
+        v = lse(bb, nn);
+      } else {
+        const int c = knb[s - 1];
+        v = ((kids[i] >> c) & 1ull) ? -CUDART_INF : lp[c] + (c == lab[i] ? lb[i] : sc[i]);
+      }
+      const unsigned long long k = score_key(v);
+      key[e] = k;
+      valid += (k != KEY_DROPPED);
+    }
+    valid = __reduce_add_sync(0xffffffffu, valid);
+    if (lane == 0 && valid) atomicAdd(&n_valid, valid);
+    __syncthreads();
+
+    // ---- C. the W smallest (key, e), in order (rule 5)
+    const int nv = n_valid, Wsel = min(W, nv);
+    bool all_valid = nv <= W;
+    if (!all_valid) {
+      if (tid == 0) { need = Wsel; pre_hi = 0ull; pre_e = 0; done = 0; passes = 0; }
+      for (int p = 0; p < 10; ++p) {
+        if (tid < 256) hist[tid] = 0;
+        __syncthreads();
+        const unsigned long long ph = pre_hi;
+        const int pe = pre_e;
+        for (int e = tid; e < N; e += BEAM_THREADS) {
+          const unsigned long long k = key[e];
+          bool in;
+          int d;
+          if (p < 8) {
+            in = p == 0 || (k >> (64 - 8 * p)) == (ph >> (64 - 8 * p));
+            d = (int)((k >> (56 - 8 * p)) & 255ull);
+          } else if (p == 8) {
+            in = k == ph;
+            d = e >> 7;
+          } else {
+            in = k == ph && (e >> 7) == pe;
+            d = e & 127;
+          }
+          if (in) atomicAdd(&hist[d], 1);
+        }
+        __syncthreads();
+        if (warp == 0) {
+          int h[8], sum = 0;
+#pragma unroll
+          for (int q = 0; q < 8; ++q) { h[q] = hist[lane * 8 + q]; sum += h[q]; }
+          int incl = sum;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += y;
+          }
+          const int nd = need, excl = incl - sum;
+          const unsigned hit = __ballot_sync(0xffffffffu, excl < nd && nd <= incl);
+          if (lane == __ffs(hit) - 1) {
+            int before = excl, bsel = lane * 8;
+            while (before + hist[bsel] < nd) before += hist[bsel++];
+            const int rem = nd - before;
+            if (p < 8) pre_hi = ph | ((unsigned long long)bsel << (56 - 8 * p));
+            else if (p == 8) pre_e = bsel;
+            else pre_e = (pe << 7) | bsel;
+            need = rem;
+            done = rem == hist[bsel];
+            passes = p + 1;
+          }
+        }
+        __syncthreads();
+        if (done) break;
+      }
+    }
+    {
+      const int ps = all_valid ? 0 : passes;
+      const unsigned long long ph = pre_hi;
+      const int pe = pre_e;
+      for (int e = tid; e < N; e += BEAM_THREADS) {
+        const unsigned long long k = key[e];
+        bool s;
+        if (all_valid) s = k != KEY_DROPPED;
+        else if (ps <= 8) s = (k >> (64 - 8 * ps)) <= (ph >> (64 - 8 * ps));
+        else if (ps == 9) s = k < ph || (k == ph && (e >> 7) <= pe);
+        else s = k < ph || (k == ph && e <= pe);
+        if (s) {
+          const int at = atomicAdd(&n_sel, 1);   // at < Wsel: the select takes exactly Wsel candidates
+          if (at < W) sel[at] = e;
+        }
+      }
+    }
+    __syncthreads();
+    for (int x = tid; x < Wsel * Wsel; x += BEAM_THREADS) {
+      const int a = x / Wsel, o = x - a * Wsel;
+      const int ea = sel[a], eo = sel[o];
+      const unsigned long long ka = key[ea], ko = key[eo];
+      if (ko < ka || (ko == ka && eo < ea)) atomicAdd(&rnk[a], 1);
+    }
+    __syncthreads();
+    if (tid < Wsel) ord[rnk[tid]] = sel[tid];
+    __syncthreads();
+
+    // ---- D. the new list; returning prefixes find their node (rule 2), new ones take the next pool nodes
+    bool is_new = false;
+    long long hs = 0;
+    unsigned long long hkey_new = 0ull;
+    if (tid < Wsel) {
+      const int e = ord[tid], i = e / S, s = e - i * S;
+      if (s == 0) {
+        b2[tid] = sb[i]; nb2[tid] = snb[i]; lab2[tid] = lab[i]; node2[tid] = node[i]; pnode2[tid] = pnode[i];
+      } else {
+        const int c = knb[s - 1];
+        b2[tid] = -CUDART_INF;
+        nb2[tid] = lp[c] + (c == lab[i] ? lb[i] : sc[i]);
+        lab2[tid] = c;
+        pnode2[tid] = node[i];
+        hkey_new = hash_key(node[i], c);
+        hs = hash_slot(hkey_new, HC);
+        int found = -1;
+        for (;;) {
+          const unsigned long long x = hk[hs];
+          if (x == hkey_new) { found = hv[hs]; break; }
+          if (x == 0ull) break;
+          hs = (hs + 1) & (HC - 1);
+        }
+        node2[tid] = found;
+        is_new = found < 0;
+      }
+    }
+    if (tid < BEAM_MAX_W) {
+      const unsigned m = __ballot_sync(0xffffffffu, is_new);
+      if (lane == 0) warp_new[warp] = m;
+    }
+    // pool_next is read here, one barrier before thread 0 advances it below: no thread may see the advanced value
+    const int first_new = pool_next;
+    __syncthreads();
+    if (tid < Wsel) {
+      if (is_new) {
+        int id = first_new + __popc(warp_new[warp] & ((1u << lane) - 1u));
+        for (int w = 0; w < warp; ++w) id += __popc(warp_new[w]);
+        const int pn = pnode2[tid], c = lab2[tid];
+        P_par[id] = pn; P_lab[id] = c; P_ts[id] = t; P_best[id] = lp[c]; P_depth[id] = P_depth[pn] + 1;
+        for (;;) {                                       // hs: the empty slot the lookup stopped at, or later
+          const unsigned long long prev = atomicCAS(&hk[hs], 0ull, hkey_new);
+          if (prev == 0ull) { hv[hs] = id; break; }
+          hs = (hs + 1) & (HC - 1);
+        }
+        node2[tid] = id;
+      }
+      lb[tid] = b2[tid]; lnb[tid] = nb2[tid]; sc[tid] = lse(b2[tid], nb2[tid]);
+      lab[tid] = lab2[tid]; node[tid] = node2[tid]; pnode[tid] = pnode2[tid];
+      pslot[tid] = -1; kids[tid] = 0ull;
+    }
+    if (tid == 0) {
+      int added = 0;
+      for (int w = 0; w < BEAM_MAX_W / 32; ++w) added += __popc(warp_new[w]);
+      pool_next = first_new + added;
+      n_list = Wsel;
+    }
+    __syncthreads();
+    for (int x = tid; x < Wsel * Wsel; x += BEAM_THREADS) {
+      const int j = x / Wsel, k = x - j * Wsel;
+      if (node[k] == pnode[j]) {
+        pslot[j] = k;
+        atomicOr(&kids[k], 1ull << lab[j]);
+      }
+    }
+    __syncthreads();
+  }
+
+  // ---- output (rule 6): zero the rows, then walk each beam's parent chain
+  const size_t row0 = (size_t)u * W * T;
+  for (size_t x = tid; x < (size_t)W * T; x += BEAM_THREADS) {
+    labels[row0 + x] = 0;
+    timesteps[row0 + x] = 0;
+  }
+  __syncthreads();
+  if (tid < W) {
+    const size_t o = (size_t)u * W + tid;
+    if (tid < n_list) {
+      int nd = node[tid];
+      const int len = P_depth[nd];
+      lengths[o] = len;
+      scores[o] = -sc[tid] + 0.0;
+      int32_t* L = labels + row0 + (size_t)tid * T;
+      int32_t* S = timesteps + row0 + (size_t)tid * T;
+      for (int pos = len - 1; pos >= 0; --pos) {
+        L[pos] = P_lab[nd];
+        S[pos] = P_ts[nd];
+        nd = P_par[nd];
+      }
+    } else {
+      lengths[o] = 0;
+      scores[o] = CUDART_INF;
+    }
+  }
+  if (tid == 0) n_beams[u] = n_list;
+}
+
+}  // namespace
+}  // namespace ds2
+
+extern "C" {
+using namespace ds2;
+
+size_t ds2_beam_decode_workspace_bytes(int B, int T, int C, int beam_width) {
+  (void)C;
+  if (B <= 0 || T <= 0 || beam_width <= 0) return 0;
+  long long NP, HC;
+  pool_sizes(T, beam_width, &NP, &HC);
+  const size_t n = (size_t)B * NP, h = (size_t)B * HC;
+  return 4 * align_up(n * 4, 256) + align_up(n * 8, 256) + align_up(h * 8, 256) + align_up(h * 4, 256);
+}
+
+int ds2_beam_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank, int beam_width,
+                    int cutoff_top_n, float cutoff_prob, int32_t* labels, int32_t* timesteps, int32_t* lengths,
+                    double* scores, int32_t* n_beams, void* workspace, size_t workspace_bytes, void* stream) {
+  DS2_REQUIRE(B > 0 && T > 0, "ds2_beam_decode: bad shape B=%d T=%d", B, T);
+  DS2_REQUIRE(C >= 2 && C <= BEAM_MAX_C, "ds2_beam_decode: C=%d outside [2, %d]", C, BEAM_MAX_C);
+  DS2_REQUIRE(blank >= 0 && blank < C, "ds2_beam_decode: blank=%d outside [0, C=%d)", blank, C);
+  DS2_REQUIRE(beam_width >= 1 && beam_width <= BEAM_MAX_W, "ds2_beam_decode: beam_width=%d outside [1, %d]",
+              beam_width, BEAM_MAX_W);
+  DS2_REQUIRE(cutoff_top_n >= 1, "ds2_beam_decode: cutoff_top_n=%d < 1", cutoff_top_n);
+  DS2_REQUIRE(cutoff_prob > 0.f && cutoff_prob <= 1.f, "ds2_beam_decode: cutoff_prob=%g outside (0, 1]",
+              (double)cutoff_prob);
+  DS2_REQUIRE((long long)T * beam_width < (1ll << 31) - 1, "ds2_beam_decode: T*beam_width too large for the node pool");
+  DS2_REQUIRE(probs && labels && timesteps && lengths && scores && n_beams, "ds2_beam_decode: null pointer");
+  DS2_REQUIRE(workspace && workspace_bytes >= ds2_beam_decode_workspace_bytes(B, T, C, beam_width),
+              "ds2_beam_decode: workspace too small (%zu < %zu bytes)", workspace_bytes,
+              ds2_beam_decode_workspace_bytes(B, T, C, beam_width));
+  long long NP, HC;
+  pool_sizes(T, beam_width, &NP, &HC);
+  const size_t n = (size_t)B * NP, h = (size_t)B * HC;
+  Arena ar(workspace, workspace_bytes);
+  BeamPool pool;
+  pool.parent = ar.take<int>(n);
+  pool.label = ar.take<int>(n);
+  pool.ts = ar.take<int>(n);
+  pool.depth = ar.take<int>(n);
+  pool.best = ar.take<double>(n);
+  pool.hkey = ar.take<unsigned long long>(h);
+  pool.hval = ar.take<int>(h);
+  pool.NP = NP;
+  pool.HC = HC;
+  static DeviceOnce attr_once;
+  if (attr_once.first()) {
+    DS2_CHECK_CUDA(cudaFuncSetAttribute(beam_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)dyn_smem_bytes(BEAM_MAX_W, BEAM_MAX_C)));
+    attr_once.done();
+  }
+  cudaStream_t st = as_stream(stream);
+  DS2_PROF("beam_decode", st);
+  DS2_LAUNCH(beam_decode_kernel, B, BEAM_THREADS, dyn_smem_bytes(beam_width, C), st, T, C, probs, out_len, blank,
+             beam_width, cutoff_top_n, cutoff_prob, labels, timesteps, lengths, scores, n_beams, pool);
+  return DS2_OK;
+}
+
+}  // extern "C"

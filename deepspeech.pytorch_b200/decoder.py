@@ -1,6 +1,11 @@
-"""Greedy CTC decoding on the GPU (SURVEY.md §8f row N2): argmax -> collapse repeats -> drop blank,
-with per-character frame offsets — the integer result of the reference's
-deepspeech_pytorch/decoder.py:121-181 (GreedyDecoder), bit-exact."""
+"""CTC decoding on the GPU.
+
+GreedyDecoder (SURVEY.md §8f row N2): argmax -> collapse repeats -> drop blank, with per-character frame offsets — the
+integer result of the reference's deepspeech_pytorch/decoder.py:121-181 (GreedyDecoder), bit-exact.
+
+BeamCTCDecoder (row N5): prefix beam search without a language model, with the reference's constructor and return
+shapes (decoder.py:56-118) and `load_decoder` (utils.py:37-54).  The search is defined by the rules in
+csrc/beam_decode.cu (DESIGN.md §5.7); ctcdecode itself is not pinned."""
 import torch
 
 from . import _lib
@@ -61,3 +66,90 @@ class GreedyDecoder:
             strings.append([''.join(self.int_to_char[int(c)] for c in labels[b, :n])])
             offs.append([offsets[b, :n].clone()])
         return strings, offs
+
+
+class BeamCTCDecoder:
+    """decoder.py:56-118 on the GPU (`ds2_beam_decode`).  `alpha` / `beta` have no effect without a language model,
+    as in ctcdecode without a scorer; `num_processes` is ignored; a non-empty `lm_path` is refused."""
+
+    def __init__(self, labels, lm_path=None, alpha=0, beta=0, cutoff_top_n=40, cutoff_prob=1.0, beam_width=100,
+                 num_processes=4, blank_index=0):
+        if lm_path:
+            raise _lib.Ds2Error(f"BeamCTCDecoder: language-model scoring (lm_path={lm_path!r}) is not supported; "
+                                "use lm_path=None or '' for beam search without a language model")
+        self.labels = list(labels)
+        self.int_to_char = dict(enumerate(self.labels))
+        self.blank_index = blank_index
+        self.space_index = self.labels.index(' ') if ' ' in self.labels else len(self.labels)
+        self.alpha, self.beta, self.num_processes = alpha, beta, num_processes
+        self.cutoff_top_n, self.cutoff_prob, self.beam_width = int(cutoff_top_n), float(cutoff_prob), int(beam_width)
+
+    def decode_beams(self, probs, sizes=None):
+        """probs (B,T,C) fp32 probabilities (a CPU tensor is copied to the current CUDA device) -> on the CPU:
+        labels (B,W,T) int32, scores (B,W) float64 (-log-likelihood, +inf for unused slots), timesteps (B,W,T) int32,
+        lengths (B,W) int32, n_beams (B) int32"""
+        import ctypes as C
+        if probs.dim() != 3:
+            raise _lib.Ds2Error(f"BeamCTCDecoder: probs must be (B, T, C), got {tuple(probs.shape)}")
+        if sizes is not None:                                # the kernel reads one length per utterance
+            sizes = torch.as_tensor(sizes)
+            if sizes.dim() != 1 or sizes.numel() != probs.size(0):
+                raise _lib.Ds2Error(f"BeamCTCDecoder: sizes must hold one length per utterance (B = {probs.size(0)}),"
+                                    f" got shape {tuple(sizes.shape)}")
+        dev = probs.device if probs.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        probs = probs.to(device=dev, dtype=torch.float32).contiguous()
+        B, T, Cn = probs.shape
+        W = self.beam_width
+        lib = get_lib()
+        with torch.cuda.device(dev):                         # launches bind to the current device
+            Wa = max(W, 1)                                   # the library refuses a bad width with a message
+            nws = lib.ds2_beam_decode_workspace_bytes(B, T, Cn, W)
+            ws = torch.empty(max(nws, 1), dtype=torch.uint8, device=dev)
+            labels = torch.empty(B, Wa, T, dtype=torch.int32, device=dev)
+            timesteps = torch.empty_like(labels)
+            lengths = torch.empty(B, Wa, dtype=torch.int32, device=dev)
+            scores = torch.empty(B, Wa, dtype=torch.float64, device=dev)
+            n_beams = torch.empty(B, dtype=torch.int32, device=dev)
+            sz = None if sizes is None else sizes.to(device=dev, dtype=torch.int32).contiguous()
+            check(lib.ds2_beam_decode(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
+                                      self.cutoff_prob, ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores),
+                                      ptr(n_beams), ptr(ws), nws, C.c_void_p(torch.cuda.current_stream().cuda_stream)),
+                  "ds2_beam_decode")
+        return labels.cpu(), scores.cpu(), timesteps.cpu(), lengths.cpu(), n_beams.cpu()
+
+    def convert_to_strings(self, out, seq_len):
+        """decoder.py:79-91: [[str]] over utterances and beams, '' where the length is 0"""
+        results = []
+        for b, batch in enumerate(out):
+            utterances = []
+            for p, utt in enumerate(batch):
+                size = int(seq_len[b][p])
+                utterances.append(''.join(self.int_to_char[int(x)] for x in utt[0:size]) if size > 0 else '')
+            results.append(utterances)
+        return results
+
+    def convert_tensor(self, offsets, sizes):
+        """decoder.py:93-104: [[IntTensor]], empty where the length is 0"""
+        results = []
+        for b, batch in enumerate(offsets):
+            utterances = []
+            for p, utt in enumerate(batch):
+                size = int(sizes[b][p])
+                utterances.append(utt[0:size] if size > 0 else torch.tensor([], dtype=torch.int))
+            results.append(utterances)
+        return results
+
+    def decode(self, probs, sizes=None):
+        """same return shape as the reference: (strings [[W str]], offsets [[W IntTensor]]), best beam first"""
+        out, _, offsets, seq_lens, _ = self.decode_beams(probs, sizes)
+        return self.convert_to_strings(out, seq_lens), self.convert_tensor(offsets, seq_lens)
+
+
+def load_decoder(labels, cfg):
+    """utils.py:37-54 without hydra: `cfg` is an LMConfig (this package's or the reference's)"""
+    kind = getattr(cfg.decoder_type, "value", cfg.decoder_type)
+    if kind == "beam":
+        return BeamCTCDecoder(labels=labels, lm_path=cfg.lm_path, alpha=cfg.alpha, beta=cfg.beta,
+                              cutoff_top_n=cfg.cutoff_top_n, cutoff_prob=cfg.cutoff_prob, beam_width=cfg.beam_width,
+                              num_processes=cfg.lm_workers, blank_index=labels.index('_'))
+    return GreedyDecoder(labels=labels, blank_index=labels.index('_'))

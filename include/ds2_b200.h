@@ -191,6 +191,22 @@ int ds2_ctc_loss_fwd_bwd(int T, int B, int C, const float* logits, const int64_t
 int ds2_greedy_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
                       int32_t* labels, int32_t* offsets, int32_t* counts, void* stream);
 
+/* ---- beam-search decode (row N5): CTC prefix beam search without a language model, what decoder.py:56-118
+ * (BeamCTCDecoder) gets from ctcdecode with an empty lm_path; the rules are in csrc/beam_decode.cu.
+ *   probs (B,T,C) fp32 probabilities; out_len (B) or NULL (= T), clamped to [0, T]
+ *   1 <= beam_width W <= 128, 2 <= C <= 64, 0 <= blank < C, cutoff_top_n >= 1, 0 < cutoff_prob <= 1
+ *   labels/timesteps (B,W,T) int32 (zero past each beam's length), lengths (B,W) int32, scores (B,W) fp64
+ *   (-log-likelihood, +inf for unused slots), n_beams (B) int32 -- ctcdecode's (beam_results, beam_scores,
+ *   timesteps, out_lens).  Deterministic; no allocation, no synchronisation; one launch.
+ *   Workspace: per utterance a node pool of T*W + 1 nodes (24 B each) and a hash of the next power of two
+ *   >= 2 (T*W + 1) slots (12 B each), which the call clears: ~2.8 MB at T = 500, W = 100; ~98 MB at T = 20000. */
+size_t ds2_beam_decode_workspace_bytes(int B, int T, int C, int beam_width);
+int ds2_beam_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
+                    int beam_width, int cutoff_top_n, float cutoff_prob,
+                    int32_t* labels, int32_t* timesteps, int32_t* lengths,
+                    double* scores, int32_t* n_beams,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- optimizer on flat fp32 buffers (row N1): clip_grad_norm_(max_norm) + AdamW / SGD-Nesterov,
  * model.py:273-297, configs/librispeech.yaml:12.  grad_scale multiplies g first (1/world for DDP
  * mean).  norm_ws: >= ds2_optim_workspace_bytes(); grad_norm_out (1 float, device) gets the
