@@ -10,6 +10,7 @@
 //   warps 0-3  epilogue: accumulator image -> registers, + input projection + biases, gate non-linearities,
 //              cell update (c / h state stays in shared memory for the whole sweep), masked stores of h_t (and
 //              the saved tensors for backward)
+// (rnn_fwd_splitk_kernel differs: its MMA warpgroup finishes the step from its registers, see there.)
 // Steps are separated by a per-direction grid barrier (monotonic counter in global memory, release / acquire,
 // bounded spin so that a fault cannot hang the GPU).  All CTAs of a launch must be co-resident: launch_sweep checks
 // occupancy and launches cooperatively; shapes that do not fit return 1 (FFMA step kernels).
@@ -678,7 +679,10 @@ static size_t res_ws_bytes(int G, int T, int B, int H, int D) {
 
 // Resident forward variants: the fp16 copy of W_hh (in the workspace) and the tensor maps of it and of the fp16 h
 // sequence.  `chunks`: 64-wide K chunks a CTA streams per step; a multiple of 4 takes one 3-D box per group of 4.
-static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chunks, cudaStream_t st) {
+// A box of W_hh holds 16 units; its rows are [gate][unit], or with `unit_major` [unit][4 gate rows] (a (k, gate, unit)
+// map, the GRU's fourth row of a unit is zero fill).
+static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chunks, cudaStream_t st,
+                           bool unit_major = false) {
   using namespace rp;
   const int G = a.G;
   __half* w16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096);
@@ -687,7 +691,9 @@ static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chu
   p.box3 = chunks % 4 == 0;
   for (int d = 0; d < a.D; ++d) {
     DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
-    int rc = make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
+    int rc = unit_major
+                 ? make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, G, a.H, (size_t)a.H * a.H, (size_t)a.H, 64, 4, UT)
+                 : make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
     if (rc) return rc;
     rc = make_tmap_f16(&p.tmV[d], p.h16 + (size_t)d * a.T * a.B * a.H, 2, a.H, a.T * a.B, 1, (size_t)a.H, 0, 64, a.B, 1);
     if (rc) return rc;
@@ -1553,15 +1559,59 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
 }
 
 // ------------------------------------------------------------------------------------------------
-// Forward sweep, split-K variant (LSTM / GRU, resident fp16 weights).  A 2-CTA cluster owns 32 hidden units of
-// one direction; CTA `rank` multiplies the G*32 gate rows (MMA M = 128, rows ordered [owner CTA][gate][unit])
-// with its half of K = H, so a step issues H/32 MMAs instead of H/16 — the single-thread MMA issue chain is the
-// longest part of a step.  accumulator-image lanes 0..63 hold the rows CTA 0 finishes, lanes 64..127 those of CTA 1: every
-// epilogue warp pushes its 32 accumulator rows into the owner's shared memory with st.async (complete_tx on
-// the owner's mbarrier); the owner adds the two partial tiles, the input projection and the biases, and runs
-// gates + cell update for its 16 units in one pass (thread = 4 consecutive units x one batch column).
+// Forward sweep, split-K variant (LSTM / GRU, resident fp16 weights).  A 2-CTA cluster owns 32 hidden units of one
+// direction; CTA `rank` multiplies the G*32 gate rows (MMA M = 128) with its half of K = H, so a step issues H/32 MMAs
+// instead of H/16 — the single-thread MMA issue chain is the longest part of a step.  The MMA warpgroup finishes the
+// step itself, from its accumulator registers: m-block 0 holds the rows of the 16 units this CTA owns, m-block 1 those
+// of the peer's 16 units.  After its last MMA the warpgroup pushes m-block 1 into the peer's `part` tile with st.async
+// (complete_tx on the peer's mbarrier), waits for the peer's tile of its own rows, adds it, the input projection and
+// the biases, and runs gates + cell update.  Warps 0-3 only store the fp32 outputs that later kernels read (B <= 32,
+// deferred saves), so that the warpgroup goes from a step's barrier arrival straight to the next step's MMAs.
+//
+// Rows of an m-block are ordered row = 4 * unit + gate: tmW is a (k, gate, unit) map and the GRU's fourth gate row of
+// a unit is the map's zero fill.  Thread l of warp w of the warpgroup holds accumulator rows 16 w + l/4 + 8 hh, i.e.
+// gate (l >> 2) & 3 of units 4 w + l/16 + 2 hh, at columns 8 i + 2 (l & 3) + e of every 32-column chunk.  A transpose
+// across the four lanes l ^ {0, 4, 8, 12} (quad_transpose) leaves each lane all gates of four cells: units
+// 4 w + l/16 + 2 hh, columns 8 ((l >> 2) & 3) + 2 (l & 3) + e (fwd_cell_unit / fwd_cell_col).
 // NKR_T: compile-time number of K chunks per CTA (0 = runtime): with constant chunk offsets the MMA descriptors are
 // "uniform base + immediate" and the issue loop needs no vector arithmetic / R2UR per instruction.
+__device__ __forceinline__ int fwd_cell_unit(int tid, int k) { return 4 * (tid >> 5) + ((tid >> 4) & 1) + 2 * (k >> 1); }
+__device__ __forceinline__ int fwd_cell_col(int tid, int k) { return 8 * ((tid >> 2) & 3) + 2 * (tid & 3) + (k & 1); }
+
+// The four cells' values of a thread (k = 2 hh + e: unit 4 w + ub + 2 hh, column e, ub = (tid >> 4) & 1) regrouped
+// with lane tid ^ 16: u4[j] = unit 4 w + j at column ub (fwd_store_col)
+__device__ __forceinline__ int fwd_store_col(int tid) { return 8 * ((tid >> 2) & 3) + 2 * (tid & 3) + ((tid >> 4) & 1); }
+__device__ __forceinline__ void fwd_units4(const float (&v)[4], float (&u4)[4]) {
+  const bool ub = (threadIdx.x >> 4) & 1;
+  const float r0 = __shfl_xor_sync(0xffffffffu, ub ? v[0] : v[1], 16);   // the partner's column, units of hh = 0
+  const float r1 = __shfl_xor_sync(0xffffffffu, ub ? v[2] : v[3], 16);   //   ... hh = 1
+  u4[0] = ub ? r0 : v[0];
+  u4[1] = ub ? v[1] : r0;
+  u4[2] = ub ? r1 : v[2];
+  u4[3] = ub ? v[3] : r1;
+}
+
+// Blocks of 4 floats, v[4 i .. 4 i + 3] = block i, transposed across the lanes x = (lane >> 2) & 3 of a group
+// l ^ {0, 4, 8, 12}: block i of lane x ends as block x of lane i (one shfl.xor round per lane bit; exact moves).
+__device__ __forceinline__ void quad_transpose(float (&v)[16]) {
+  const int x = (threadIdx.x >> 2) & 3;
+#pragma unroll
+  for (int bit = 0; bit < 2; ++bit) {
+    const bool hi = (x >> bit) & 1;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      if (i & (1 << bit)) continue;
+      const int i1 = i | (1 << bit);   // of the pair (i, i1) a lane sends the block whose bit differs from its own
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float r = __shfl_xor_sync(0xffffffffu, hi ? v[4 * i + k] : v[4 * i1 + k], 4 << bit);
+        if (hi) v[4 * i + k] = r;
+        else v[4 * i1 + k] = r;
+      }
+    }
+  }
+}
+
 template <int RNN, int NKR_T = 0>
 __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __grid_constant__ PersistParams p) {
   using namespace rp;
@@ -1572,17 +1622,16 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned, still __shared__
   const int NB = p.NB, B = p.B, T = p.T, H = p.H, D = p.D;
   const int B_BYTES = NB * 128;
-  const int NBp = NB + 1;
   const int NKR = NKR_T ? NKR_T : H / 128;               // 64-wide fp16 chunks of this CTA's K half
   const int NG = grp_count(NKR);
-  float* part = reinterpret_cast<float*>(smem + NKR * (AW + B_BYTES));   // [2 sources] 64-row partial tiles (xt_* layout)
-  float* cst = part + 2 * xt_slice(64, NB);                              // [16][NBp] cell (LSTM) / hidden (GRU) state
-  int* lens_s = reinterpret_cast<int*>(cst + UT * NBp);
-  uint64_t* full = reinterpret_cast<uint64_t*>(lens_s + ((NB + 1) & ~1));   // one per group of 4 chunks (<= 8)
+  // the peer's partial sums of this CTA's rows, in the accumulator's fragment order: [32-column chunk][4][thread]
+  float4* part = reinterpret_cast<float4*>(smem + NKR * (AW + B_BYTES));
+  // B <= 32 with deferred saves: the MMA warpgroup hands a step's fp32 outputs ([6][thread]) to warps 0-3 here
+  const bool stage_saves = p.defer && NB == 32;
+  float4* stage = part + NB * 16;
+  uint64_t* full = reinterpret_cast<uint64_t*>(stage + (stage_saves ? 6 * 128 : 0));   // one per group of 4 chunks (<= 8)
   uint64_t* wbar = full + 8;
-  uint64_t* accum_bar = wbar + 1;
-  uint64_t* part_bar = accum_bar + 1;
-  float* acc_img = reinterpret_cast<float*>(part_bar + 1);   // accumulator image (tc::wg_store_acc)
+  uint64_t* part_bar = wbar + 1;
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int rank = blockIdx.x & 1, cl = blockIdx.x >> 1;
@@ -1598,28 +1647,26 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
     tma_prefetch_desc(&p.tmV[d]);
     for (int i = 0; i < 8; ++i) mbar_init(&full[i], 1);
     mbar_init(wbar, 1);
-    mbar_init(accum_bar, 1);
     mbar_init(part_bar, 1);
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < UT * NBp; i += THREADS) cst[i] = 0.f;
-  for (int i = threadIdx.x; i < NB; i += THREADS) lens_s[i] = i < B ? p.len[i] : 0;
   __syncthreads();
   cluster_sync_all();                                     // the peer's mbarriers are initialised
   const int kc0 = rank * NKR;                             // first K chunk (of H/64) of this CTA
 
   if (warp == 8) {                                        // TMA producer
     if (lane == 0) {
-      // weights once: per chunk the rows of the two owners, [gate][16 units] each (rows >= 16 G of a half unused)
-      mbar_arrive_expect_tx(wbar, (uint32_t)(NKR * 2 * G * UT * 128));
+      // weights once: per chunk 64 rows (16 units x 4 gate rows) of this CTA's units, then 64 of the peer's
+      mbar_arrive_expect_tx(wbar, (uint32_t)(NKR * 2 * 64 * 128));
       for (int c = 0; c < NKR; ++c) {
-        tma_load_3d(smem + c * AW, &p.tmW[d], wbar, (kc0 + c) * 64, U0, 0);
-        tma_load_3d(smem + c * AW + 64 * 128, &p.tmW[d], wbar, (kc0 + c) * 64, U0 + UT, 0);
+        tma_load_3d(smem + c * AW, &p.tmW[d], wbar, (kc0 + c) * 64, 0, u0);
+        tma_load_3d(smem + c * AW + 64 * 128, &p.tmW[d], wbar, (kc0 + c) * 64, 0, U0 + (rank ^ 1) * UT);
       }
       uint8_t* hbuf = smem + NKR * AW;
       for (int step = 1; step < T; ++step) {
         const int t = d == 0 ? step : T - 1 - step;
         const int tp = d == 0 ? t - 1 : t + 1;
+        // every CTA has finished the previous step, this one included: its MMAs no longer read hbuf
         grid_wait_counter(ctr, n_arrive * (unsigned int)step, p.err);
         fence_proxy_async_global();
         trace_stamp(p.trace, p.T, step, 0);
@@ -1638,231 +1685,275 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
       }
     }
   } else if (warp >= 4) {
-    // MMA warpgroup: accumulators in registers, handed to the epilogue warps as an image in shared memory; the
-    // accumulator width (batch padded to 32 * NCH) is chosen once, outside the step loop
+    // MMA warpgroup: the accumulator width (batch padded to 32 * NCH) is chosen once, outside the step loop
     with_nch<2>(NB, [&](auto nch) {
-      WgAcc<2, decltype(nch)::value> acc;
-      {
-        const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
-        const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * AW)));
-        const uint64_t a_step = (uint64_t)(AW >> 4), b_step = (uint64_t)(B_BYTES >> 4);
-        mbar_wait(wbar, 0);
-        uint32_t ph = 0;
-        for (int step = 1; step < T; ++step) {
+      constexpr int NCH = decltype(nch)::value;
+      const int tid = threadIdx.x - 128;
+      // biases of the cells' two units (k >> 1): x-side + h-side summed, except the GRU n gate (r multiplies the h side)
+      float bsum[G][2], bhn[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int u = u0 + fwd_cell_unit(tid, 2 * hh);
+#pragma unroll
+        for (int g = 0; g < G; ++g) {
+          const float bx = p.b_ih[d][g * H + u], bh = p.b_hh[d][g * H + u];
+          bsum[g][hh] = (RNN == DS2_RNN_GRU && g == 2) ? bx : bx + bh;
+          if (RNN == DS2_RNN_GRU && g == 2) bhn[hh] = bh;
+        }
+        if (RNN != DS2_RNN_GRU) bhn[hh] = 0.f;
+      }
+      float cs[NCH][4];                                  // cell (LSTM) / hidden (GRU) state of the cells
+#pragma unroll
+      for (int c = 0; c < NCH; ++c)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) cs[c][k] = 0.f;
+      const uint32_t dst_part = mapa_u32(smem_u32(part + tid), (uint32_t)(rank ^ 1));
+      const uint32_t dst_bar = mapa_u32(smem_u32(part_bar), (uint32_t)(rank ^ 1));
+      const uint32_t part_tx = (uint32_t)(64 * NB * 4);
+      const uint64_t a_base = warp_uniform(smem_desc_sw128(smem_u32(smem)));
+      const uint64_t b_base = warp_uniform(smem_desc_sw128(smem_u32(smem + NKR * AW)));
+      const uint64_t a_step = (uint64_t)(AW >> 4), b_step = (uint64_t)(B_BYTES >> 4);
+      const bool defer = stage_saves;                   // two chunks: stored before the arrival
+      mbar_wait(wbar, 0);
+      uint32_t ph = 0, part_phase = 0;
+      for (int step = 0; step < T; ++step) {
+        const int t = d == 0 ? step : T - 1 - step;
+        // input projections of the cells of column chunk c: independent of the recurrence, so with one chunk they
+        // are loaded before the MMA chain and land while it runs (with two, both chunks' accumulators and
+        // projections would not fit in the registers together: each chunk's are loaded just before its cells)
+        float gx[NCH][G][4];
+        auto load_gx = [&](int c) {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int b = 32 * c + fwd_cell_col(tid, k);
+            const float* src = p.gates + (((size_t)t * B + b) * D + d) * GH + u0 + fwd_cell_unit(tid, k);
+#pragma unroll
+            for (int g = 0; g < G; ++g) gx[c][g][k] = b < B ? src[(size_t)g * H] : 0.f;
+          }
+        };
+        if (NCH == 1) load_gx(0);
+        // s[c][4 g + k]: recurrent sum of gate g of cell k (zero at the first step: h_{-1} = 0)
+        float s[NCH][16];
+        if (step > 0) {
+          if (tid == 0) mbar_arrive_expect_tx(part_bar, part_tx);   // arm this step's phase (the peer may already have sent)
+          WgAcc<2, NCH> acc;                             // live from the first MMA of the step to the partial sums only
           if constexpr (NKR_T > 0) {
             constexpr int NGT = (NKR_T + 3) / 4;
-  #pragma unroll
+#pragma unroll
             for (int g = 0; g < NGT; ++g) {
               mbar_wait(full + g, ph);
-              if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-              if (g == NGT - 1 && lane == 0) trace_stamp(p.trace, p.T, step, 3);
-  #pragma unroll
+              if (g == 0 && tid == 0) trace_stamp(p.trace, p.T, step, 2);
+              if (g == NGT - 1 && tid == 0) trace_stamp(p.trace, p.T, step, 3);
+#pragma unroll
               for (int c = 4 * g; c < (4 * g + 4 < NKR_T ? 4 * g + 4 : NKR_T); ++c) {
                 const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
                 wg_mma4<true>(acc, ad, bd, c > 0);
               }
             }
           } else {
-            for (int g = 0; g < NG; ++g) {
-              mbar_wait(full + g, ph);
-              if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
-              const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
-              if (c1 == NKR && lane == 0) trace_stamp(p.trace, p.T, step, 3);
-              for (int c = c0; c < c1; ++c) {
-                const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
-                wg_mma4<true>(acc, ad, bd, c > 0);
+            for (int c = 0; c < NKR; ++c) {
+              if (c % 4 == 0) {                          // first chunk of a group
+                mbar_wait(full + c / 4, ph);
+                if (c == 0 && tid == 0) trace_stamp(p.trace, p.T, step, 2);
+                if (c + 4 >= NKR && tid == 0) trace_stamp(p.trace, p.T, step, 3);
               }
+              const uint64_t ad = a_base + (uint64_t)c * a_step, bd = b_base + (uint64_t)c * b_step;
+              wg_mma4<true>(acc, ad, bd, c > 0);
             }
           }
-          wg_publish(acc, acc_img, accum_bar);
-          if (lane == 0) trace_stamp(p.trace, p.T, step, 4);
+          wg_commit();
+          wg_wait<0>();
           ph ^= 1;
+          if (tid == 0) trace_stamp(p.trace, p.T, step, 4);
+          // the peer's rows, straight from the registers: thread tid of the peer reads back exactly these 16 values
+#pragma unroll
+          for (int c = 0; c < NCH; ++c)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+              st_async_v4(dst_part + (uint32_t)((4 * c + j) * 128 * 16), acc.r[1][c][4 * j], acc.r[1][c][4 * j + 1],
+                          acc.r[1][c][4 * j + 2], acc.r[1][c][4 * j + 3], dst_bar);
+          if (tid == 0) trace_stamp(p.trace, p.T, step, 6);
+          mbar_wait_cluster(part_bar, part_phase, p.err);   // the peer's partial tile of this CTA's rows has landed
+          part_phase ^= 1;
+          if (tid == 0) trace_stamp(p.trace, p.T, step, 7);
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) {
+            // pr[rank] + pr[rank ^ 1]: IEEE addition is commutative, so this is pr[0] + pr[1] bit for bit
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const float4 pv = part[(4 * c + j) * 128 + tid];
+              s[c][4 * j] = acc.r[0][c][4 * j] + pv.x;
+              s[c][4 * j + 1] = acc.r[0][c][4 * j + 1] + pv.y;
+              s[c][4 * j + 2] = acc.r[0][c][4 * j + 2] + pv.z;
+              s[c][4 * j + 3] = acc.r[0][c][4 * j + 3] + pv.w;
+            }
+            quad_transpose(s[c]);
+          }
+        } else {
+#pragma unroll
+          for (int c = 0; c < NCH; ++c)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) s[c][i] = 0.f;
+        }
+        // ---- gates + cell update of 4 cells: o[0..G-1] saved gate values, o[4] aux (LSTM c / GRU h_n + b_hn), o[5] h
+        auto cell4 = [&](int c, const float (&x)[G][4], const float (&r4)[16], float (&cp)[4], float (&o)[6][4]) {
+          float pre[G][4], hn[4], hval[4];
+          bool valid[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int b = 32 * c + fwd_cell_col(tid, k);
+            valid[k] = b < B && t < p.len[b];
+          }
+#pragma unroll
+          for (int g = 0; g < G; ++g)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float r = r4[4 * g + k];
+              if (RNN == DS2_RNN_GRU && g == 2) { hn[k] = r + bhn[k >> 1]; pre[g][k] = x[g][k] + bsum[g][k >> 1]; }
+              else pre[g][k] = (x[g][k] + r) + bsum[g][k >> 1];
+            }
+          if (RNN == DS2_RNN_LSTM) {
+            float a[4][4], cval[4], th[4];
+            // i, f, o: sigmoid; g: tanh = 2 sigmoid(2x) - 1  (one EX2 + one RCP per value, stage by stage)
+#pragma unroll
+            for (int g = 0; g < 4; ++g)
+#pragma unroll
+              for (int k = 0; k < 4; ++k) a[g][k] = ex2_ftz((g == 2 ? -2.f * LOG2E : -LOG2E) * pre[g][k]);
+#pragma unroll
+            for (int g = 0; g < 4; ++g)
+#pragma unroll
+              for (int k = 0; k < 4; ++k) a[g][k] = rcp_ftz(1.f + a[g][k]);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              a[2][k] = fmaf(2.f, a[2][k], -1.f);
+              cval[k] = valid[k] ? fmaf(a[1][k], cp[k], a[0][k] * a[2][k]) : 0.f;
+            }
+#pragma unroll
+            for (int k = 0; k < 4; ++k) th[k] = ex2_ftz(-2.f * LOG2E * cval[k]);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) th[k] = rcp_ftz(1.f + th[k]);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              hval[k] = valid[k] ? a[3][k] * fmaf(2.f, th[k], -1.f) : 0.f;
+              if (valid[k]) cp[k] = cval[k];
+#pragma unroll
+              for (int g = 0; g < 4; ++g) o[g][k] = valid[k] ? a[g][k] : 0.f;
+              o[4][k] = cval[k];
+            }
+          } else {
+            float a[2][4], nv[4];
+#pragma unroll
+            for (int g = 0; g < 2; ++g)
+#pragma unroll
+              for (int k = 0; k < 4; ++k) a[g][k] = ex2_ftz(-LOG2E * pre[g][k]);
+#pragma unroll
+            for (int g = 0; g < 2; ++g)
+#pragma unroll
+              for (int k = 0; k < 4; ++k) a[g][k] = rcp_ftz(1.f + a[g][k]);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) nv[k] = ex2_ftz(-2.f * LOG2E * fmaf(a[0][k], hn[k], pre[2][k]));
+#pragma unroll
+            for (int k = 0; k < 4; ++k) nv[k] = rcp_ftz(1.f + nv[k]);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const float nval = valid[k] ? fmaf(2.f, nv[k], -1.f) : 0.f;
+              hval[k] = valid[k] ? fmaf(a[1][k], cp[k] - nval, nval) : 0.f;
+              if (valid[k]) cp[k] = hval[k];
+              o[0][k] = valid[k] ? a[0][k] : 0.f; o[1][k] = valid[k] ? a[1][k] : 0.f; o[2][k] = nval; o[3][k] = 0.f;
+              o[4][k] = valid[k] ? hn[k] : 0.f;
+            }
+          }
+#pragma unroll
+          for (int k = 0; k < 4; ++k) o[5][k] = hval[k];
+        };
+        // the fp32 saves that only later kernels read (gates when training, aux, the sequence output)
+        // Outputs of a chunk's cells regrouped by one shfl.xor(16) round (fwd_units4): the lane with
+        // ub = (tid >> 4) & 1 ends with column e = ub of the four consecutive units 4 w .. 4 w + 3, so every global
+        // store of a thread is one 16-byte (fp32) or 8-byte (fp16) vector; scattered 4-byte stores cost more memory
+        // transactions, and the release at the step barrier waits for them.
+        const int bs = fwd_store_col(tid);               // + 32 c
+        const int us = u0 + 4 * (tid >> 5);
+        auto store4 = [&](int c, const float (&o)[6][4]) {
+          const int b = 32 * c + bs;
+          if (b < B) {
+            const size_t so = (((size_t)d * T + t) * B + b) * H + us;
+            float* gp = p.gates + (((size_t)t * B + b) * D + d) * GH + us;
+            *reinterpret_cast<float4*>(p.aux + so) = make_float4(o[4][0], o[4][1], o[4][2], o[4][3]);
+            if (p.training) {
+#pragma unroll
+              for (int g = 0; g < G; ++g)
+                *reinterpret_cast<float4*>(gp + (size_t)g * H) = make_float4(o[g][0], o[g][1], o[g][2], o[g][3]);
+            }
+            *reinterpret_cast<float4*>(p.hseq + so) = make_float4(o[5][0], o[5][1], o[5][2], o[5][3]);
+          }
+        };
+        float sv[NCH][6][4];
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+          if (NCH > 1) load_gx(c);
+          float o[6][4];
+          cell4(c, gx[c], s[c], cs[c], o);
+#pragma unroll
+          for (int q = 0; q < 6; ++q)
+            if (q < G || q >= 4) fwd_units4(o[q], sv[c][q]);
+          const int b = 32 * c + bs;
+          if (b < B) {                                   // fp16 h_t: the MMA operand of the next step
+            const __half2 lo = __floats2half2_rn(sv[c][5][0], sv[c][5][1]), hi = __floats2half2_rn(sv[c][5][2], sv[c][5][3]);
+            uint2 pk;
+            pk.x = *reinterpret_cast<const unsigned int*>(&lo);
+            pk.y = *reinterpret_cast<const unsigned int*>(&hi);
+            *reinterpret_cast<uint2*>(p.h16 + (((size_t)d * T + t) * B + b) * H + us) = pk;
+          }
+          if (!defer) store4(c, sv[c]);
+        }
+        if (tid == 0) trace_stamp(p.trace, p.T, step, 8);
+        named_bar_sync(1, 128);          // CTA-scope: every thread's h16 stores happen-before thread 0's release
+        if (tid == 0) {
+          trace_stamp(p.trace, p.T, step, 9);
+          fence_proxy_async_global();
+          trace_stamp(p.trace, p.T, step, 10);
+          red_release(ctr, 1u);
+          trace_stamp(p.trace, p.T, step, 11);
+          trace_stamp_ns(p.trace, p.T, step, 12);
+        }
+        if (defer) {                     // after the arrival: hand the saves to warps 0-3 (stage_saves)
+          named_bar_sync(4, 256);        // they have stored the previous step's
+#pragma unroll
+          for (int q = 0; q < 6; ++q)
+            if (q < G || q >= 4) stage[q * 128 + tid] = make_float4(sv[0][q][0], sv[0][q][1], sv[0][q][2], sv[0][q][3]);
+          asm volatile("bar.arrive 3, 256;" ::: "memory");
         }
       }
     });
-  } else {                                                // warps 0..3: epilogue
-    const int q = warp % 4;
-    const int e = threadIdx.x;          // 0..127
-    // accumulator-image lane (= row) 32q + lane belongs to CTA q/2; inside that CTA's 64-row slice it is row 32 (q&1) + lane
-    const int dst_cta = q >> 1;
-    const int my_row = 32 * (q & 1) + lane;
-    const uint32_t dst_row = mapa_u32(smem_u32(part), (uint32_t)dst_cta) + (uint32_t)(rank * xt_slice(64, NB) * 4);
-    const uint32_t dst_bar = mapa_u32(smem_u32(part_bar), (uint32_t)dst_cta);
-    const uint32_t part_tx = (uint32_t)(2 * 64 * NB * 4);
-    const int uq = 4 * (e & 3), b_own = e >> 2;
-    // biases of this thread's 4 units: x-side + h-side summed, except the GRU n gate (r multiplies the h side)
-    float bsum[G][4], bhn[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-#pragma unroll
-      for (int g = 0; g < G; ++g) {
-        const float bx = p.b_ih[d][g * H + u0 + uq + j], bh = p.b_hh[d][g * H + u0 + uq + j];
-        bsum[g][j] = (RNN == DS2_RNN_GRU && g == 2) ? bx : bx + bh;
-        if (RNN == DS2_RNN_GRU && g == 2) bhn[j] = bh;
-      }
-      if (RNN != DS2_RNN_GRU) bhn[j] = 0.f;
-    }
-    auto ld4 = [](const float* src, float (&v)[4]) {
-      const float4 x = *reinterpret_cast<const float4*>(src);
-      v[0] = x.x; v[1] = x.y; v[2] = x.z; v[3] = x.w;
-    };
-    auto st4 = [](float* dst, const float (&v)[4]) { *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]); };
-    uint32_t acc_phase = 0, part_phase = 0;
-    const bool single = B <= 32;
+  } else if (stage_saves) {
+    // warps 0-3: the fp32 saves (gates, aux, sequence output) of the cells of MMA-warpgroup thread threadIdx.x, off
+    // the warpgroup's path from one step's arrival to the next step's MMAs
+    const int tid = threadIdx.x;
+    const int b = fwd_store_col(tid), us = u0 + 4 * (tid >> 5);
     for (int step = 0; step < T; ++step) {
       const int t = d == 0 ? step : T - 1 - step;
-      // input projections of this thread's cells: independent of the recurrence, fetched before the MMA wait
-      float gx[G][4];
-      if (single && b_own < B) {
-#pragma unroll
-        for (int g = 0; g < G; ++g) ld4(p.gates + (((size_t)t * B + b_own) * D + d) * GH + (size_t)g * H + u0 + uq, gx[g]);
-      }
-      if (step > 0) {
-        if (e == 0) mbar_arrive_expect_tx(part_bar, part_tx);   // arm this step's phase (the peer may already have sent)
-        mbar_wait(accum_bar, acc_phase);
-        if (e == 0) trace_stamp(p.trace, p.T, step, 5);
-        for (int cb = 0; cb < NB; cb += 32) {
-          float acc[32];
-          tmem_ld32(acc_img, acc_pitch(NB), ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int c0 = cb + 4 * i;                    // NB is a multiple of 8: a group of 4 columns is in or out
-            if (c0 < NB)
-              st_async_v4(dst_row + (uint32_t)(xt_off(64, my_row, c0) * 4), acc[4 * i], acc[4 * i + 1], acc[4 * i + 2], acc[4 * i + 3], dst_bar);
-          }
-        }
-        acc_phase ^= 1;
-        if (e == 0) trace_stamp(p.trace, p.T, step, 6);
-        mbar_wait_cluster(part_bar, part_phase, p.err);   // both partial tiles of this CTA's rows have landed
-        part_phase ^= 1;
-      }
-      if (e == 0) trace_stamp(p.trace, p.T, step, 7);
-      // ---- gates + cell update: o[0..G-1] saved gate values, o[4] aux (LSTM c / GRU h_n + b_hn), o[5] h
-      auto cell4 = [&](int b, const float (&x)[G][4], float (&o)[6][4]) {
-        const bool valid = t < lens_s[b];
-        float pre[G][4], hn[4], hval[4];
-#pragma unroll
-        for (int g = 0; g < G; ++g)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float r = 0.f;
-            if (step > 0) {
-              const float* pr = part + xt_off(64, g * UT + uq + j, b);
-              r = pr[0] + pr[xt_slice(64, NB)];
-            }
-            if (RNN == DS2_RNN_GRU && g == 2) { hn[j] = r + bhn[j]; pre[g][j] = x[g][j] + bsum[g][j]; }
-            else pre[g][j] = (x[g][j] + r) + bsum[g][j];
-          }
-        if (RNN == DS2_RNN_LSTM) {
-          float a[4][4], cval[4], th[4];
-          // i, f, o: sigmoid; g: tanh = 2 sigmoid(2x) - 1  (one EX2 + one RCP per value, stage by stage)
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) a[g][j] = ex2_ftz((g == 2 ? -2.f * LOG2E : -LOG2E) * pre[g][j]);
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) a[g][j] = rcp_ftz(1.f + a[g][j]);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            a[2][j] = fmaf(2.f, a[2][j], -1.f);
-            cval[j] = valid ? fmaf(a[1][j], cst[(uq + j) * NBp + b], a[0][j] * a[2][j]) : 0.f;
-          }
-#pragma unroll
-          for (int j = 0; j < 4; ++j) th[j] = ex2_ftz(-2.f * LOG2E * cval[j]);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) th[j] = rcp_ftz(1.f + th[j]);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            hval[j] = valid ? a[3][j] * fmaf(2.f, th[j], -1.f) : 0.f;
-            if (valid) cst[(uq + j) * NBp + b] = cval[j];
-#pragma unroll
-            for (int g = 0; g < 4; ++g) o[g][j] = valid ? a[g][j] : 0.f;
-            o[4][j] = cval[j];
-          }
-        } else {
-          float a[2][4], nv[4];
-#pragma unroll
-          for (int g = 0; g < 2; ++g)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) a[g][j] = ex2_ftz(-LOG2E * pre[g][j]);
-#pragma unroll
-          for (int g = 0; g < 2; ++g)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) a[g][j] = rcp_ftz(1.f + a[g][j]);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) nv[j] = ex2_ftz(-2.f * LOG2E * fmaf(a[0][j], hn[j], pre[2][j]));
-#pragma unroll
-          for (int j = 0; j < 4; ++j) nv[j] = rcp_ftz(1.f + nv[j]);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float nval = valid ? fmaf(2.f, nv[j], -1.f) : 0.f;
-            const float hprev = cst[(uq + j) * NBp + b];
-            hval[j] = valid ? fmaf(a[1][j], hprev - nval, nval) : 0.f;
-            if (valid) cst[(uq + j) * NBp + b] = hval[j];
-            o[0][j] = valid ? a[0][j] : 0.f; o[1][j] = valid ? a[1][j] : 0.f; o[2][j] = nval; o[3][j] = 0.f;
-            o[4][j] = valid ? hn[j] : 0.f;
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o[5][j] = hval[j];
-        const __half2 lo = __floats2half2_rn(hval[0], hval[1]), hi = __floats2half2_rn(hval[2], hval[3]);
-        uint2 pk;
-        pk.x = *reinterpret_cast<const unsigned int*>(&lo);
-        pk.y = *reinterpret_cast<const unsigned int*>(&hi);
-        *reinterpret_cast<uint2*>(p.h16 + (((size_t)d * T + t) * B + b) * H + u0 + uq) = pk;
-      };
-      auto store4 = [&](int b, const float (&o)[6][4]) {
-        const size_t so = (((size_t)d * T + t) * B + b) * H + u0 + uq;
-        float* gp = p.gates + (((size_t)t * B + b) * D + d) * GH + u0 + uq;
-        st4(p.aux + so, o[4]);
+      asm volatile("bar.arrive 4, 256;" ::: "memory");   // the staging buffer is free
+      named_bar_sync(3, 256);                            // this step's outputs are in it
+      if (b < B) {
+        const size_t so = (((size_t)d * T + t) * B + b) * H + us;
+        float* gp = p.gates + (((size_t)t * B + b) * D + d) * GH + us;
+        *reinterpret_cast<float4*>(p.aux + so) = stage[4 * 128 + tid];
         if (p.training) {
 #pragma unroll
-          for (int g = 0; g < G; ++g) st4(gp + g * H, o[g]);
+          for (int g = 0; g < G; ++g) *reinterpret_cast<float4*>(gp + (size_t)g * H) = stage[g * 128 + tid];
         }
-        st4(p.hseq + so, o[5]);
-      };
-      const bool defer = p.defer && single;
-      float sv[6][4];
-      if (single) {
-        if (b_own < B) {
-          cell4(b_own, gx, sv);
-          if (!defer) store4(b_own, sv);
-        }
-      } else {
-        for (int b = b_own; b < B; b += 32) {
-#pragma unroll
-          for (int g = 0; g < G; ++g) ld4(p.gates + (((size_t)t * B + b) * D + d) * GH + (size_t)g * H + u0 + uq, gx[g]);
-          cell4(b, gx, sv);
-          store4(b, sv);
-        }
+        *reinterpret_cast<float4*>(p.hseq + so) = stage[5 * 128 + tid];
       }
-      if (e == 0) trace_stamp(p.trace, p.T, step, 8);
-      named_bar_sync(1, 128);          // CTA-scope: every epilogue thread's stores happen-before thread 0's release
-      if (e == 0) {
-        trace_stamp(p.trace, p.T, step, 9);
-        fence_proxy_async_global();
-        trace_stamp(p.trace, p.T, step, 10);
-        red_release(ctr, 1u);
-        trace_stamp(p.trace, p.T, step, 11);
-        trace_stamp_ns(p.trace, p.T, step, 12);
-      }
-      if (defer) {
-        if (b_own < B) store4(b_own, sv);
-        if (e == 0) trace_stamp(p.trace, p.T, step, 13);
-      }
+      if (tid == 0) trace_stamp(p.trace, p.T, step, 13);
     }
   }
   __syncthreads();
   cluster_sync_all();                                     // nobody exits while the peer may still write into its tile
 }
 
-static size_t fwd_splitk_smem_bytes(int NB, int H) {
-  using namespace rp;
-  size_t NBp = NB + 1;
-  return 1024 + (size_t)(H / 128) * (128 * 128 + (size_t)NB * 128) + (2 * xt_slice(64, NB) + UT * NBp + NB + 4) * sizeof(float) +
-         12 * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
+static size_t fwd_splitk_smem_bytes(int NB, int H, bool defer) {
+  return 1024 + (size_t)(H / 128) * (128 * 128 + (size_t)NB * 128) + (size_t)64 * NB * sizeof(float) +
+         (defer && NB == 32 ? 6 * 128 * 16 : 0) + 10 * sizeof(uint64_t) + 64;
 }
 
 // returns 1 when the shape / device does not take this variant (the caller then uses the 16-unit resident kernel)
@@ -1874,7 +1965,7 @@ static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
   PersistParams p = sweep_params(a, 32, "DS2_TRACE_FWD", ws);
   if (p.NB > 64) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  const size_t smem = one_cta_per_sm(fwd_splitk_smem_bytes(p.NB, a.H));
+  const size_t smem = one_cta_per_sm(fwd_splitk_smem_bytes(p.NB, a.H, p.defer));
   if (smem > 227 * 1024) return 1;
   // H = 1024: unrolled issue loop
   const SweepKernel kern = a.H == 1024 ? rnn_fwd_splitk_kernel<RNN, 8> : rnn_fwd_splitk_kernel<RNN, 0>;
@@ -1882,7 +1973,7 @@ static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   if (int rc = opt_in_smem(attr_once, {rnn_fwd_splitk_kernel<RNN, 8>, rnn_fwd_splitk_kernel<RNN, 0>})) return rc;
   const int fit = cluster_fit(kern, 2, a.D * p.NT * 2, smem, st);
   return launch_sweep(kern, 2, p.NT * 2, smem, fit, true, 4096, "split-K forward sweep", "the 16-unit kernel", p, st,
-                      [&] { return f16_weight_maps(a, p, ws, a.H / 128, st); });
+                      [&] { return f16_weight_maps(a, p, ws, a.H / 128, st, true); });
 }
 
 static size_t splitk_smem_bytes(int NB, int CL) {
