@@ -50,6 +50,11 @@ PROTOTYPES = {
     "ds2_greedy_decode": (i32, [i32, i32, i32, vp, vp, i32, vp, vp, vp, vp]),
     "ds2_beam_decode_workspace_bytes": (sz, [i32] * 4),
     "ds2_beam_decode": (i32, [i32, i32, i32, vp, vp, i32, i32, i32, f32] + [vp] * 6 + [sz, vp]),
+    "ds2_lm_bytes": (sz, [i32, vp, i64]),
+    "ds2_lm_build": (i32, [i32, vp, vp, vp, vp, i32, i32, i64, vp, vp, vp, vp, sz, vp]),
+    "ds2_beam_decode_lm_workspace_bytes": (sz, [i32] * 4),
+    "ds2_beam_decode_lm": (i32, [i32, i32, i32, vp, vp, i32, i32, i32, f32, vp, i32, C.c_double, C.c_double, i32]
+                           + [vp] * 6 + [sz, vp]),
     "ds2_spectrogram_workspace_bytes": (sz, [i32]),
     "ds2_spectrogram_batch": (i32, [i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, vp, i32, vp, sz, vp]),
     "ds2_spec_augment_workspace_bytes": (sz, [i32]),

@@ -71,7 +71,7 @@ class DataConfig:
 class LMConfig:
     """deepspeech_pytorch/configs/inference_config.py:7-16 (the decoder settings of evaluation and transcription)"""
     decoder_type: DecoderType = DecoderType.greedy
-    lm_path: str = ''           # KenLM model for beam search: not supported here (BeamCTCDecoder raises)
+    lm_path: str = ''           # ARPA n-gram model (.arpa or .arpa.gz) for beam search; KenLM binaries are refused
     top_paths: int = 1          # number of beams to return
     alpha: float = 0.0          # language-model weight (no effect without a language model)
     beta: float = 0.0           # word bonus (no effect without a language model)

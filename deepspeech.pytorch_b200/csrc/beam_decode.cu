@@ -54,10 +54,55 @@
 // Nothing is decided by an atomic: shared atomics only count (histograms, compaction before the rank sort, child
 // masks), and the hash's slot claims do not change what a lookup returns.  The final beams are written by walking
 // parent pointers through the pool.
+//
+// With an ARPA n-gram language model (row N6, ds2_beam_decode_lm), rules 1-7 hold with these additions: ctcdecode's
+// algorithm with a word-level Scorer (PaddlePaddle's ctc_beam_search_decoder with ext_scorer set,
+// fill_dictionary(true), OOV_SCORE = -1000).  Parity with ctcdecode and KenLM is unpinned: neither is available here.
+//  L0. Model.  An ARPA text file, plain or gzip'd; values parsed to fp32 (as KenLM stores them), an unwritten backoff
+//      is 0; word ids in the file's unigram order.  Refused (host side, deepspeech.pytorch_b200/lm.py): a missing
+//      file, a file that is not ARPA (a KenLM binary), counts that differ from the \data\ header, duplicate n-grams,
+//      order > 5 or >= 2^24 words, no <s> unigram, labels without ' ', a character-based model (every word one
+//      character), and a model none of whose words can be spelled with the labels.
+//  L1. Vocabulary V and dictionary constraint.  V = the unigrams other than <s>, </s>, <unk> whose every character is
+//      a label other than the blank's and the space's ((!) ctcdecode would also map the blank's character).  A prefix
+//      splits at spaces into completed words and its partial word (the run after the last space, maybe empty).  A new
+//      candidate (i, c), c != blank, exists only if c != space and partial(i)+c is a prefix of a word of V, or
+//      c = space and partial(i) is in V.  Leading and double spaces are impossible.  (!) ctcdecode's FST matcher also
+//      rejects the first character after a space in the frame where it resets its state; which character that hits
+//      depends on the visiting order, so it is not reproduced.
+//  L2. LM value.  lm(w | u_1..u_k) is the ARPA conditional log10 probability of w with the context the last N-1 items
+//      of (<s>^(N-1), u_1, ..., u_k): the longest listed n-gram plus the backoffs of the longer unlisted contexts (0 for
+//      a context that is not listed), the fp32 values summed in fp64 from the longest context down.  A word outside
+//      the ARPA vocabulary gets lm = -1000 (LM_OOV).  a(w) = alpha * lm + beta.  (!) The value is used in log10,
+//      unconverted (LM_SCALE, lm.cuh): how we read ctcdecode's get_log_cond_prob, not verifiable here.
+//  L3. a(w) enters on the path from "...w" to "...w ": the new candidate (i, space) has
+//      nb' = lp[space] + score_i + a(partial(i) | ctx(i)), and a listed prefix ending in a space whose parent pi is
+//      listed adds it to the second nb term of its stay candidate.  The first nb term gets none.  Scores carry every
+//      LM term from then on.
+//  L4. Full-beam filter (ctcdecode's min_cutoff).  When the list holds W prefixes at the start of frame t, let
+//      m = score of the last listed prefix + log p[blank] - max(0, beta), p[blank] unpruned.  Every contribution from a
+//      prefix x through a character c with lp[c] + score_x < m is dropped: the blank term of a stay (x = j), both nb
+//      terms of a stay (x = j, then x = pi, c = l_j), a new candidate (x = i).  A dropped contribution does not move a
+//      timestep under rule 7.
+//  L5. End of utterance.  Each listed prefix that is non-empty and does not end in a space gets
+//      score += a(partial | ctx), lm = -1000 for a partial word not in V.  The list is reordered by (score desc, list
+//      position asc) and -score is reported.  (!) ctcdecode orders by this score but reports an "approx_ctc" that
+//      subtracts beta per character and alpha times a sentence probability including </s>, a term the search never
+//      added; here the reported score is the one the beams are ordered by.  sizes[b] = 0 gives one empty beam, 0.
+// Kernel (LM = true): per list slot in shared memory the trie node of the partial word, the allowed-extension mask
+// (trie children, plus the space when the node is a word) and the N-1 context word ids; per pool node the lm value of
+// its partial word, so a returning prefix needs no new lookup.  Pass B drops a new candidate that fails L1 or L4 with
+// KEY_DROPPED and adds a(w) to a space candidate; pass D looks up lm for each new node whose partial is a word (<= W
+// lookups per frame, each <= 2N - 1 hash probes runs).  The L5 term and the reorder (a W x W counting rank) happen
+// before the beams are written.  a(w) is computed with __dmul_rn / __dadd_rn, never contracted, so it rounds as the
+// oracle's does.
 
 #include <math_constants.h>
 
+#include <cmath>
+
 #include "common.cuh"
+#include "lm.cuh"
 
 namespace ds2 {
 
@@ -76,8 +121,18 @@ struct BeamPool {
   double* best;
   unsigned long long* hkey;   // 0 = empty slot
   int* hval;
+  double* lm;                 // LM only: lm value of the node's partial word (rule L2), if that word is in V
   long long NP, HC;           // HC: power of two >= 2 NP
 };
+
+// LM only: the tables of ds2_lm_build and the scorer's parameters
+struct BeamLm {
+  const void* tables;
+  int order, space;
+  double alpha, beta;
+};
+
+constexpr int LM_CTX = LM_MAX_ORDER - 1;   // context word ids per list slot
 
 void pool_sizes(int T, int W, long long* NP, long long* HC) {
   *NP = (long long)T * W + 1;
@@ -86,10 +141,16 @@ void pool_sizes(int T, int W, long long* NP, long long* HC) {
   *HC = h;
 }
 
-size_t dyn_smem_bytes(int W, int C) {
+size_t dyn_smem_bytes(int W, int C, bool lm) {
   return (size_t)W * C * 8          // keys
          + (size_t)W * 8 * 8        // lb, lnb, sc, sb, snb, b2, nb2, child masks
-         + (size_t)W * 4 * 10;      // lab, node, pnode, pslot, lab2, node2, pnode2, sel, rnk, ord
+         + (size_t)W * 4 * 10       // lab, node, pnode, pslot, lab2, node2, pnode2, sel, rnk, ord
+         + (lm ? (size_t)W * (8 + 8 + 4 + 4 * LM_CTX) : 0);   // LM: amask, lmv, tn, ctx
+}
+
+// a(w) = alpha * lm + beta (rule L2), rounded as written
+__device__ __forceinline__ double lm_term(const BeamLm& L, double lm) {
+  return __dadd_rn(__dmul_rn(L.alpha, lm), L.beta);
 }
 
 __device__ __forceinline__ double lse(double a, double b) {
@@ -114,11 +175,12 @@ __device__ __forceinline__ long long hash_slot(unsigned long long k, long long H
   return (long long)(k & (unsigned long long)(HC - 1));
 }
 
+template <bool LM>
 __global__ void __launch_bounds__(BEAM_THREADS)
 beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t* __restrict__ out_len, int blank,
                    int W, int top_n, float cutoff_prob, int32_t* __restrict__ labels, int32_t* __restrict__ timesteps,
                    int32_t* __restrict__ lengths, double* __restrict__ scores, int32_t* __restrict__ n_beams,
-                   BeamPool pool) {
+                   BeamPool pool, BeamLm lmp) {
   const int u = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* key = reinterpret_cast<unsigned long long*>(smem_raw);
@@ -140,6 +202,12 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
   int* sel = pnode2 + W;
   int* rnk = sel + W;
   int* ord = rnk + W;
+  // LM only (rules L1-L5): per slot the allowed extensions, the lm value of the partial word, its trie node, and
+  // the N-1 context word ids (oldest first)
+  unsigned long long* amask = reinterpret_cast<unsigned long long*>(ord + W);
+  double* lmv = reinterpret_cast<double*>(amask + W);
+  int* tn = reinterpret_cast<int*>(lmv + W);
+  int* ctx = tn + W;
 
   __shared__ double lp[BEAM_MAX_C];
   __shared__ float pf[BEAM_MAX_C];
@@ -166,6 +234,17 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
     lb[0] = 0.0; lnb[0] = -CUDART_INF; sc[0] = 0.0;
     lab[0] = -1; node[0] = 0; pnode[0] = -1; pslot[0] = -1; kids[0] = 0ull;
     n_list = 1; pool_next = 1;
+  }
+  LmView lmt;
+  const int order = LM ? lmp.order : 1, space = LM ? lmp.space : -1;
+  if constexpr (LM) {
+    lmt = lm_view(lmp.tables);
+    if (tid == 0) {
+      tn[0] = 0;                                     // the root: the empty partial word, not a word itself
+      amask[0] = lmt.mask[0];
+      lmv[0] = 0.0;
+      for (int k = 0; k < LM_CTX; ++k) ctx[k] = lmt.bos;
+    }
   }
   __syncthreads();
 
@@ -232,19 +311,36 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
     const int n = n_list, S = 1 + nK, N = n * S;
     const unsigned long long km = kmask;
     const bool blank_in = (km >> blank) & 1ull;
+    // L4: contributions with lp[c] + score_x < m are dropped; m = -inf (nothing dropped) unless the list is full
+    double m = -CUDART_INF;
+    if constexpr (LM) {
+      if (n == W) m = sc[n - 1] + lp[blank] - fmax(0.0, lmp.beta);
+    }
     int valid = 0;
     for (int e = tid; e < N; e += BEAM_THREADS) {
       const int i = e / S, s = e - i * S;
       double v;
       if (s == 0) {
-        const double bb = blank_in ? lp[blank] + sc[i] : -CUDART_INF;
+        double bb = blank_in ? lp[blank] + sc[i] : -CUDART_INF;
+        if constexpr (LM) {
+          if (bb < m) bb = -CUDART_INF;
+        }
         double nn = -CUDART_INF;
         const int l = lab[i];
         if (l >= 0 && ((km >> l) & 1ull)) {
           const double lpl = lp[l];
           nn = lpl + lnb[i];
           const int pi = pslot[i];
-          if (pi >= 0) {
+          if constexpr (LM) {
+            if (lpl + sc[i] < m) nn = -CUDART_INF;
+            if (pi >= 0 && !(lpl + sc[pi] < m)) {
+              double v2 = lpl + (lab[pi] == l ? lb[pi] : sc[pi]);
+              if (l == space) v2 = __dadd_rn(v2, lm_term(lmp, lmv[pi]));            // L3
+              nn = lse(nn, v2);
+              const int nd = node[i];
+              if (lpl > P_best[nd]) { P_best[nd] = lpl; P_ts[nd] = t; }
+            }
+          } else if (pi >= 0) {
             nn = lse(nn, lpl + (lab[pi] == l ? lb[pi] : sc[pi]));
             const int nd = node[i];
             if (lpl > P_best[nd]) { P_best[nd] = lpl; P_ts[nd] = t; }
@@ -255,7 +351,17 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
         v = lse(bb, nn);
       } else {
         const int c = knb[s - 1];
-        v = ((kids[i] >> c) & 1ull) ? -CUDART_INF : lp[c] + (c == lab[i] ? lb[i] : sc[i]);
+        if constexpr (LM) {
+          // L1 (allowed extensions), L4, then the L3 term of a space candidate
+          if (((kids[i] >> c) & 1ull) || !((amask[i] >> c) & 1ull) || lp[c] + sc[i] < m) {
+            v = -CUDART_INF;
+          } else {
+            v = lp[c] + (c == lab[i] ? lb[i] : sc[i]);
+            if (c == space) v = __dadd_rn(v, lm_term(lmp, lmv[i]));
+          }
+        } else {
+          v = ((kids[i] >> c) & 1ull) ? -CUDART_INF : lp[c] + (c == lab[i] ? lb[i] : sc[i]);
+        }
       }
       const unsigned long long k = score_key(v);
       key[e] = k;
@@ -352,14 +458,34 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
     bool is_new = false;
     long long hs = 0;
     unsigned long long hkey_new = 0ull;
+    int tn_new = 0, ctx_new[LM_CTX];   // LM: the new slot's trie node, context and lm value (written after the barrier)
+    double lmv_new = 0.0;
     if (tid < Wsel) {
       const int e = ord[tid], i = e / S, s = e - i * S;
+      if constexpr (LM) {
+        tn_new = tn[i];
+        lmv_new = lmv[i];
+#pragma unroll
+        for (int k = 0; k < LM_CTX; ++k) ctx_new[k] = ctx[i * LM_CTX + k];
+      }
       if (s == 0) {
         b2[tid] = sb[i]; nb2[tid] = snb[i]; lab2[tid] = lab[i]; node2[tid] = node[i]; pnode2[tid] = pnode[i];
       } else {
         const int c = knb[s - 1];
         b2[tid] = -CUDART_INF;
-        nb2[tid] = lp[c] + (c == lab[i] ? lb[i] : sc[i]);
+        double nb = lp[c] + (c == lab[i] ? lb[i] : sc[i]);
+        if constexpr (LM) {
+          if (c == space) {                                 // "...w" -> "...w ": w joins the context
+            nb = __dadd_rn(nb, lm_term(lmp, lmv[i]));
+#pragma unroll
+            for (int k = 0; k < LM_CTX - 1; ++k) ctx_new[k] = ctx_new[k + 1];
+            ctx_new[LM_CTX - 1] = lmt.word[tn_new];
+            tn_new = 0;
+          } else {
+            tn_new = lmt.first[tn_new] + __popcll(lmt.mask[tn_new] & ((1ull << c) - 1ull));
+          }
+        }
+        nb2[tid] = nb;
         lab2[tid] = c;
         pnode2[tid] = node[i];
         hkey_new = hash_key(node[i], c);
@@ -373,6 +499,9 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
         }
         node2[tid] = found;
         is_new = found < 0;
+        if constexpr (LM) {                                 // a returning prefix (rule 2) keeps its lm value;
+          lmv_new = is_new ? 0.0 : pool.lm[(size_t)u * NP + found];   // a new one is looked up below
+        }
       }
     }
     if (tid < BEAM_MAX_W) {
@@ -383,6 +512,13 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
     const int first_new = pool_next;
     __syncthreads();
     if (tid < Wsel) {
+      if constexpr (LM) {
+        // the slot's own context, written and then read by this thread only
+#pragma unroll
+        for (int k = 0; k < LM_CTX; ++k) ctx[tid * LM_CTX + k] = ctx_new[k];
+        if (is_new && lmt.word[tn_new] >= 0)
+          lmv_new = lm_logp(lmt, order, ctx + tid * LM_CTX + LM_CTX - (order - 1), lmt.word[tn_new]);
+      }
       if (is_new) {
         int id = first_new + __popc(warp_new[warp] & ((1u << lane) - 1u));
         for (int w = 0; w < warp; ++w) id += __popc(warp_new[w]);
@@ -394,10 +530,16 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
           hs = (hs + 1) & (HC - 1);
         }
         node2[tid] = id;
+        if constexpr (LM) pool.lm[(size_t)u * NP + id] = lmv_new;
       }
       lb[tid] = b2[tid]; lnb[tid] = nb2[tid]; sc[tid] = lse(b2[tid], nb2[tid]);
       lab[tid] = lab2[tid]; node[tid] = node2[tid]; pnode[tid] = pnode2[tid];
       pslot[tid] = -1; kids[tid] = 0ull;
+      if constexpr (LM) {
+        tn[tid] = tn_new;
+        lmv[tid] = lmv_new;
+        amask[tid] = lmt.mask[tn_new] | (lmt.word[tn_new] >= 0 ? 1ull << space : 0ull);
+      }
     }
     if (tid == 0) {
       int added = 0;
@@ -416,6 +558,24 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
     __syncthreads();
   }
 
+  // ---- LM: the end-of-utterance term and the reorder (rule L5); the final score goes to sb, the position to rnk
+  if constexpr (LM) {
+    const int n = n_list;
+    if (tid < n) {
+      double f = sc[tid];
+      const int l = lab[tid];
+      if (l >= 0 && l != space) f = __dadd_rn(f, lm_term(lmp, lmt.word[tn[tid]] >= 0 ? lmv[tid] : LM_OOV));
+      sb[tid] = f;
+      rnk[tid] = 0;
+    }
+    __syncthreads();
+    for (int x = tid; x < n * n; x += BEAM_THREADS) {
+      const int a = x / n, o = x - a * n;
+      if (sb[o] > sb[a] || (sb[o] == sb[a] && o < a)) atomicAdd(&rnk[a], 1);
+    }
+    __syncthreads();
+  }
+
   // ---- output (rule 6): zero the rows, then walk each beam's parent chain
   const size_t row0 = (size_t)u * W * T;
   for (size_t x = tid; x < (size_t)W * T; x += BEAM_THREADS) {
@@ -424,14 +584,15 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
   }
   __syncthreads();
   if (tid < W) {
-    const size_t o = (size_t)u * W + tid;
+    const int r = LM && tid < n_list ? rnk[tid] : tid;
+    const size_t o = (size_t)u * W + r;
     if (tid < n_list) {
       int nd = node[tid];
       const int len = P_depth[nd];
       lengths[o] = len;
-      scores[o] = -sc[tid] + 0.0;
-      int32_t* L = labels + row0 + (size_t)tid * T;
-      int32_t* S = timesteps + row0 + (size_t)tid * T;
+      scores[o] = -(LM ? sb[tid] : sc[tid]) + 0.0;
+      int32_t* L = labels + row0 + (size_t)r * T;
+      int32_t* S = timesteps + row0 + (size_t)r * T;
       for (int pos = len - 1; pos >= 0; --pos) {
         L[pos] = P_lab[nd];
         S[pos] = P_ts[nd];
@@ -445,37 +606,33 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
   if (tid == 0) n_beams[u] = n_list;
 }
 
-}  // namespace
-}  // namespace ds2
-
-extern "C" {
-using namespace ds2;
-
-size_t ds2_beam_decode_workspace_bytes(int B, int T, int C, int beam_width) {
+size_t beam_workspace_bytes(int B, int T, int C, int beam_width, bool lm) {
   (void)C;
   if (B <= 0 || T <= 0 || beam_width <= 0) return 0;
   long long NP, HC;
   pool_sizes(T, beam_width, &NP, &HC);
   const size_t n = (size_t)B * NP, h = (size_t)B * HC;
-  return 4 * align_up(n * 4, 256) + align_up(n * 8, 256) + align_up(h * 8, 256) + align_up(h * 4, 256);
+  return 4 * align_up(n * 4, 256) + align_up(n * 8, 256) + align_up(h * 8, 256) + align_up(h * 4, 256) +
+         (lm ? align_up(n * 8, 256) : 0);
 }
 
-int ds2_beam_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank, int beam_width,
-                    int cutoff_top_n, float cutoff_prob, int32_t* labels, int32_t* timesteps, int32_t* lengths,
-                    double* scores, int32_t* n_beams, void* workspace, size_t workspace_bytes, void* stream) {
-  DS2_REQUIRE(B > 0 && T > 0, "ds2_beam_decode: bad shape B=%d T=%d", B, T);
-  DS2_REQUIRE(C >= 2 && C <= BEAM_MAX_C, "ds2_beam_decode: C=%d outside [2, %d]", C, BEAM_MAX_C);
-  DS2_REQUIRE(blank >= 0 && blank < C, "ds2_beam_decode: blank=%d outside [0, C=%d)", blank, C);
-  DS2_REQUIRE(beam_width >= 1 && beam_width <= BEAM_MAX_W, "ds2_beam_decode: beam_width=%d outside [1, %d]",
-              beam_width, BEAM_MAX_W);
-  DS2_REQUIRE(cutoff_top_n >= 1, "ds2_beam_decode: cutoff_top_n=%d < 1", cutoff_top_n);
-  DS2_REQUIRE(cutoff_prob > 0.f && cutoff_prob <= 1.f, "ds2_beam_decode: cutoff_prob=%g outside (0, 1]",
-              (double)cutoff_prob);
-  DS2_REQUIRE((long long)T * beam_width < (1ll << 31) - 1, "ds2_beam_decode: T*beam_width too large for the node pool");
-  DS2_REQUIRE(probs && labels && timesteps && lengths && scores && n_beams, "ds2_beam_decode: null pointer");
-  DS2_REQUIRE(workspace && workspace_bytes >= ds2_beam_decode_workspace_bytes(B, T, C, beam_width),
-              "ds2_beam_decode: workspace too small (%zu < %zu bytes)", workspace_bytes,
-              ds2_beam_decode_workspace_bytes(B, T, C, beam_width));
+template <bool LM>
+int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
+                       int beam_width, int cutoff_top_n, float cutoff_prob, BeamLm lm, int32_t* labels,
+                       int32_t* timesteps, int32_t* lengths, double* scores, int32_t* n_beams, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  DS2_REQUIRE(B > 0 && T > 0, "%s: bad shape B=%d T=%d", fn, B, T);
+  DS2_REQUIRE(C >= 2 && C <= BEAM_MAX_C, "%s: C=%d outside [2, %d]", fn, C, BEAM_MAX_C);
+  DS2_REQUIRE(blank >= 0 && blank < C, "%s: blank=%d outside [0, C=%d)", fn, blank, C);
+  DS2_REQUIRE(beam_width >= 1 && beam_width <= BEAM_MAX_W, "%s: beam_width=%d outside [1, %d]", fn, beam_width,
+              BEAM_MAX_W);
+  DS2_REQUIRE(cutoff_top_n >= 1, "%s: cutoff_top_n=%d < 1", fn, cutoff_top_n);
+  DS2_REQUIRE(cutoff_prob > 0.f && cutoff_prob <= 1.f, "%s: cutoff_prob=%g outside (0, 1]", fn, (double)cutoff_prob);
+  DS2_REQUIRE((long long)T * beam_width < (1ll << 31) - 1, "%s: T*beam_width too large for the node pool", fn);
+  DS2_REQUIRE(probs && labels && timesteps && lengths && scores && n_beams, "%s: null pointer", fn);
+  const size_t need = beam_workspace_bytes(B, T, C, beam_width, LM);
+  DS2_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes,
+              need);
   long long NP, HC;
   pool_sizes(T, beam_width, &NP, &HC);
   const size_t n = (size_t)B * NP, h = (size_t)B * HC;
@@ -488,19 +645,64 @@ int ds2_beam_decode(int B, int T, int C, const float* probs, const int32_t* out_
   pool.best = ar.take<double>(n);
   pool.hkey = ar.take<unsigned long long>(h);
   pool.hval = ar.take<int>(h);
+  pool.lm = LM ? ar.take<double>(n) : nullptr;
   pool.NP = NP;
   pool.HC = HC;
   static DeviceOnce attr_once;
   if (attr_once.first()) {
-    DS2_CHECK_CUDA(cudaFuncSetAttribute(beam_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)dyn_smem_bytes(BEAM_MAX_W, BEAM_MAX_C)));
+    DS2_CHECK_CUDA(cudaFuncSetAttribute(beam_decode_kernel<LM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)dyn_smem_bytes(BEAM_MAX_W, BEAM_MAX_C, LM)));
     attr_once.done();
   }
   cudaStream_t st = as_stream(stream);
-  DS2_PROF("beam_decode", st);
-  DS2_LAUNCH(beam_decode_kernel, B, BEAM_THREADS, dyn_smem_bytes(beam_width, C), st, T, C, probs, out_len, blank,
-             beam_width, cutoff_top_n, cutoff_prob, labels, timesteps, lengths, scores, n_beams, pool);
+  DS2_PROF(LM ? "beam_decode_lm" : "beam_decode", st);
+  DS2_LAUNCH(beam_decode_kernel<LM>, B, BEAM_THREADS, dyn_smem_bytes(beam_width, C, LM), st, T, C, probs, out_len,
+             blank, beam_width, cutoff_top_n, cutoff_prob, labels, timesteps, lengths, scores, n_beams, pool, lm);
   return DS2_OK;
+}
+
+}  // namespace
+}  // namespace ds2
+
+extern "C" {
+using namespace ds2;
+
+size_t ds2_beam_decode_workspace_bytes(int B, int T, int C, int beam_width) {
+  return beam_workspace_bytes(B, T, C, beam_width, false);
+}
+
+size_t ds2_beam_decode_lm_workspace_bytes(int B, int T, int C, int beam_width) {
+  return beam_workspace_bytes(B, T, C, beam_width, true);
+}
+
+int ds2_beam_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank, int beam_width,
+                    int cutoff_top_n, float cutoff_prob, int32_t* labels, int32_t* timesteps, int32_t* lengths,
+                    double* scores, int32_t* n_beams, void* workspace, size_t workspace_bytes, void* stream) {
+  return beam_decode_launch<false>("ds2_beam_decode", B, T, C, probs, out_len, blank, beam_width, cutoff_top_n,
+                                   cutoff_prob, BeamLm{}, labels, timesteps, lengths, scores, n_beams, workspace,
+                                   workspace_bytes, stream);
+}
+
+int ds2_beam_decode_lm(int B, int T, int C, const float* probs, const int32_t* out_len, int blank, int beam_width,
+                       int cutoff_top_n, float cutoff_prob, const void* lm, int lm_order, double alpha, double beta,
+                       int space, int32_t* labels, int32_t* timesteps, int32_t* lengths, double* scores,
+                       int32_t* n_beams, void* workspace, size_t workspace_bytes, void* stream) {
+  DS2_REQUIRE(lm, "ds2_beam_decode_lm: null language model");
+  DS2_REQUIRE(lm_order >= 1 && lm_order <= LM_MAX_ORDER, "ds2_beam_decode_lm: order=%d outside [1, %d]", lm_order,
+              LM_MAX_ORDER);
+  DS2_REQUIRE(space >= 0 && space < C && space != blank && C <= BEAM_MAX_C,
+              "ds2_beam_decode_lm: space=%d outside [0, C=%d) or equal to blank=%d", space, C, blank);
+  DS2_REQUIRE(std::isfinite(alpha) && std::isfinite(beta), "ds2_beam_decode_lm: alpha=%g, beta=%g not finite", alpha,
+              beta);
+  BeamLm L;
+  L.tables = lm;
+  L.order = lm_order;
+  L.space = space;
+  L.alpha = alpha;
+  L.beta = beta;
+  return beam_decode_launch<true>("ds2_beam_decode_lm", B, T, C, probs, out_len, blank, beam_width, cutoff_top_n,
+                                  cutoff_prob, L, labels, timesteps, lengths, scores, n_beams, workspace,
+                                  workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -3,9 +3,9 @@
 GreedyDecoder (SURVEY.md §8f row N2): argmax -> collapse repeats -> drop blank, with per-character frame offsets — the
 integer result of the reference's deepspeech_pytorch/decoder.py:121-181 (GreedyDecoder), bit-exact.
 
-BeamCTCDecoder (row N5): prefix beam search without a language model, with the reference's constructor and return
-shapes (decoder.py:56-118) and `load_decoder` (utils.py:37-54).  The search is defined by the rules in
-csrc/beam_decode.cu (DESIGN.md §5.7); ctcdecode itself is not pinned."""
+BeamCTCDecoder (rows N5, N6): prefix beam search, without or with an ARPA n-gram language model (`lm_path`), with the
+reference's constructor and return shapes (decoder.py:56-118) and `load_decoder` (utils.py:37-54).  The search is
+defined by the rules in csrc/beam_decode.cu (DESIGN.md §5.7); ctcdecode and KenLM themselves are not pinned."""
 import torch
 
 from . import _lib
@@ -69,25 +69,33 @@ class GreedyDecoder:
 
 
 class BeamCTCDecoder:
-    """decoder.py:56-118 on the GPU (`ds2_beam_decode`).  `alpha` / `beta` have no effect without a language model,
-    as in ctcdecode without a scorer; `num_processes` is ignored; a non-empty `lm_path` is refused."""
+    """decoder.py:56-118 on the GPU.  Without `lm_path` this is `ds2_beam_decode` and `alpha` / `beta` have no
+    effect, as in ctcdecode without a scorer.  With `lm_path`, an ARPA n-gram model (plain or gzip'd) is parsed here
+    and the search is `ds2_beam_decode_lm` (rules L0-L5 of csrc/beam_decode.cu): words restricted to the model's
+    vocabulary, alpha * log10 p + beta added at every completed word.  `num_processes` is ignored."""
 
     def __init__(self, labels, lm_path=None, alpha=0, beta=0, cutoff_top_n=40, cutoff_prob=1.0, beam_width=100,
                  num_processes=4, blank_index=0):
-        if lm_path:
-            raise _lib.Ds2Error(f"BeamCTCDecoder: language-model scoring (lm_path={lm_path!r}) is not supported; "
-                                "use lm_path=None or '' for beam search without a language model")
         self.labels = list(labels)
         self.int_to_char = dict(enumerate(self.labels))
         self.blank_index = blank_index
         self.space_index = self.labels.index(' ') if ' ' in self.labels else len(self.labels)
-        self.alpha, self.beta, self.num_processes = alpha, beta, num_processes
+        self.alpha, self.beta, self.num_processes = float(alpha), float(beta), num_processes
         self.cutoff_top_n, self.cutoff_prob, self.beam_width = int(cutoff_top_n), float(cutoff_prob), int(beam_width)
+        self.lm = None
+        if lm_path:
+            from .lm import LanguageModel
+            self.lm = LanguageModel(lm_path, self.labels, blank_index)
+        self._decoder = self          # the reference's search_lm_params.py calls decoder._decoder.reset_params
+
+    def reset_params(self, alpha, beta):
+        """ctcdecode's CTCBeamDecoder.reset_params: the language-model weight and word bonus of later decodes"""
+        self.alpha, self.beta = float(alpha), float(beta)
 
     def decode_beams(self, probs, sizes=None):
         """probs (B,T,C) fp32 probabilities (a CPU tensor is copied to the current CUDA device) -> on the CPU:
         labels (B,W,T) int32, scores (B,W) float64 (-log-likelihood, +inf for unused slots), timesteps (B,W,T) int32,
-        lengths (B,W) int32, n_beams (B) int32"""
+        lengths (B,W) int32, n_beams (B) int32.  With a language model the scores include its terms (rule L5)"""
         import ctypes as C
         if probs.dim() != 3:
             raise _lib.Ds2Error(f"BeamCTCDecoder: probs must be (B, T, C), got {tuple(probs.shape)}")
@@ -103,7 +111,9 @@ class BeamCTCDecoder:
         lib = get_lib()
         with torch.cuda.device(dev):                         # launches bind to the current device
             Wa = max(W, 1)                                   # the library refuses a bad width with a message
-            nws = lib.ds2_beam_decode_workspace_bytes(B, T, Cn, W)
+            lm = None if self.lm is None else self.lm.device_tables(dev)
+            nws = (lib.ds2_beam_decode_workspace_bytes if lm is None else lib.ds2_beam_decode_lm_workspace_bytes)(
+                B, T, Cn, W)
             ws = torch.empty(max(nws, 1), dtype=torch.uint8, device=dev)
             labels = torch.empty(B, Wa, T, dtype=torch.int32, device=dev)
             timesteps = torch.empty_like(labels)
@@ -111,10 +121,16 @@ class BeamCTCDecoder:
             scores = torch.empty(B, Wa, dtype=torch.float64, device=dev)
             n_beams = torch.empty(B, dtype=torch.int32, device=dev)
             sz = None if sizes is None else sizes.to(device=dev, dtype=torch.int32).contiguous()
-            check(lib.ds2_beam_decode(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
-                                      self.cutoff_prob, ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores),
-                                      ptr(n_beams), ptr(ws), nws, C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                  "ds2_beam_decode")
+            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            if lm is None:
+                check(lib.ds2_beam_decode(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
+                                          self.cutoff_prob, ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores),
+                                          ptr(n_beams), ptr(ws), nws, stream), "ds2_beam_decode")
+            else:
+                check(lib.ds2_beam_decode_lm(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
+                                             self.cutoff_prob, ptr(lm), self.lm.order, self.alpha, self.beta,
+                                             self.lm.space, ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores),
+                                             ptr(n_beams), ptr(ws), nws, stream), "ds2_beam_decode_lm")
         return labels.cpu(), scores.cpu(), timesteps.cpu(), lengths.cpu(), n_beams.cpu()
 
     def convert_to_strings(self, out, seq_len):

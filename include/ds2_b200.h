@@ -207,6 +207,32 @@ int ds2_beam_decode(int B, int T, int C, const float* probs, const int32_t* out_
                     double* scores, int32_t* n_beams,
                     void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- ARPA n-gram language model for beam search (row N6): the tables of csrc/lm.cuh in a caller buffer.
+ *   order 1..5; counts[order] (host) the number of n-grams of each order, counts[0] = n_words < 2^24;
+ *   ids[n-1] (device) counts[n-1] x n int32 word ids, oldest first; logp[n-1] / backoff[n-1] (device) fp32 log10
+ *   values as written (a NULL backoff array = all 0); duplicate n-grams are the caller's to refuse; bos = id of <s>;
+ *   trie_mask / trie_first / trie_word (device, n_nodes each): the vocabulary trie, node 0 the root, children of a
+ *   node contiguous in label order from trie_first, trie_word = word id of the node's prefix or -1.
+ *   The build clears and fills the buffer on `stream` (a few launches); the inputs may be freed once it has run.
+ *   Bytes: 4 per hash slot (a power of two >= 2 x the n-gram count), 24 per n-gram, 16 per trie node. */
+size_t ds2_lm_bytes(int order, const int64_t* counts, int64_t n_nodes);
+int ds2_lm_build(int order, const int64_t* counts, const int32_t* const* ids, const float* const* logp,
+                 const float* const* backoff, int n_words, int bos, int64_t n_nodes, const uint64_t* trie_mask,
+                 const int32_t* trie_first, const int32_t* trie_word, void* buffer, size_t buffer_bytes,
+                 void* stream);
+
+/* ---- beam-search decode with the language model (rules L0-L5 in csrc/beam_decode.cu): the arguments of
+ * ds2_beam_decode plus the buffer of ds2_lm_build, its order, alpha, beta (fp64) and the space label, which must not
+ * be the blank.  Scores are -(CTC log-likelihood + alpha * sum lm + beta * #words), best first.  Workspace: that of
+ * ds2_beam_decode plus 8 B per pool node.  Deterministic; no allocation, no synchronisation; one launch. */
+size_t ds2_beam_decode_lm_workspace_bytes(int B, int T, int C, int beam_width);
+int ds2_beam_decode_lm(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
+                       int beam_width, int cutoff_top_n, float cutoff_prob,
+                       const void* lm, int lm_order, double alpha, double beta, int space,
+                       int32_t* labels, int32_t* timesteps, int32_t* lengths,
+                       double* scores, int32_t* n_beams,
+                       void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- optimizer on flat fp32 buffers (row N1): clip_grad_norm_(max_norm) + AdamW / SGD-Nesterov,
  * model.py:273-297, configs/librispeech.yaml:12.  grad_scale multiplies g first (1/world for DDP
  * mean).  norm_ws: >= ds2_optim_workspace_bytes(); grad_norm_out (1 float, device) gets the

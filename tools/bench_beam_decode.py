@@ -12,7 +12,13 @@ one CTA each).  Two utterances of the timed W = 100 configuration on the model o
 `oracle/beam_oracle.py` in the same run.  The card name and power limit are read in the same run.  Needs a GPU;
 prints one JSON line.
 
-    python tools/bench_beam_decode.py [--batch 32] [--frames 500] [--iters 10] [--reps 5]
+With --lm, the same probabilities are also decoded with a language model (`ds2_beam_decode_lm`, row N6, alpha = 0.8,
+beta = 1.0): a seeded synthetic ARPA 3-gram at the scale of LibriSpeech's pruned 3-gram (200 000 words, 1.5 M 2-grams,
+1.5 M 3-grams; written to a temporary directory).  The row then adds the host parse + trie time, the device build
+time, the table bytes, the decode times with the model, and two utterances of the W = 100 model-output decode checked
+against `oracle/lm_oracle.py`.
+
+    python tools/bench_beam_decode.py [--batch 32] [--frames 500] [--iters 10] [--reps 5] [--lm]
 """
 import argparse
 import ctypes as C
@@ -20,6 +26,8 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
+import time
 
 import numpy as np
 import torch
@@ -31,6 +39,7 @@ if ROOT not in sys.path:
 import deepspeech_pytorch_b200 as ds  # noqa: E402
 from deepspeech_pytorch_b200._lib import check, ptr  # noqa: E402
 from oracle import beam_oracle as BO  # noqa: E402
+from oracle import lm_oracle as LO  # noqa: E402
 
 
 def card_info():
@@ -72,14 +81,19 @@ def peaked_probs(B, T, C, seed=0):
     return torch.from_numpy((e / e.sum(-1, keepdims=True)).astype(np.float32))
 
 
-class Call:
-    """prepared buffers for back-to-back `ds2_beam_decode` launches"""
+LM_ALPHA, LM_BETA = 0.8, 1.0
 
-    def __init__(self, probs, W):
+
+class Call:
+    """prepared buffers for back-to-back `ds2_beam_decode` (or, with `lm`, `ds2_beam_decode_lm`) launches"""
+
+    def __init__(self, probs, W, lm=None):
         self.probs = probs.contiguous()
         B, T, Cn = self.probs.shape
-        self.shape, self.W = (B, T, Cn), W
-        self.nws = ds.get_lib().ds2_beam_decode_workspace_bytes(B, T, Cn, W)
+        self.shape, self.W, self.lm = (B, T, Cn), W, lm
+        lib = ds.get_lib()
+        self.nws = (lib.ds2_beam_decode_workspace_bytes if lm is None else lib.ds2_beam_decode_lm_workspace_bytes)(
+            B, T, Cn, W)
         dev = self.probs.device
         self.ws = torch.empty(self.nws, dtype=torch.uint8, device=dev)
         self.labels = torch.empty(B, W, T, dtype=torch.int32, device=dev)
@@ -90,6 +104,16 @@ class Call:
 
     def __call__(self):
         B, T, Cn = self.shape
+        if self.lm is not None:
+            lm = self.lm
+            check(ds.get_lib().ds2_beam_decode_lm(B, T, Cn, ptr(self.probs), None, 0, self.W, 40, 1.0,
+                                                  ptr(lm.device_tables(self.probs.device)), lm.order, LM_ALPHA,
+                                                  LM_BETA, lm.space, ptr(self.labels), ptr(self.timesteps),
+                                                  ptr(self.lengths), ptr(self.scores), ptr(self.n_beams),
+                                                  ptr(self.ws), self.nws,
+                                                  C.c_void_p(torch.cuda.current_stream().cuda_stream)),
+                  "ds2_beam_decode_lm")
+            return
         check(ds.get_lib().ds2_beam_decode(B, T, Cn, ptr(self.probs), None, 0, self.W, 40, 1.0, ptr(self.labels),
                                            ptr(self.timesteps), ptr(self.lengths), ptr(self.scores),
                                            ptr(self.n_beams), ptr(self.ws), self.nws,
@@ -102,6 +126,7 @@ def main():
     ap.add_argument("--frames", type=int, default=500)
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--lm", action="store_true", help="also decode with a LibriSpeech-pruned-3-gram-sized ARPA model")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_beam_decode: needs a CUDA device")
@@ -128,6 +153,30 @@ def main():
     inputs = {"peaked": peaked_probs(B, Tp, Cn).to(dev), "model": model_probs}
 
     calls = {(k, W): Call(p, W) for k, p in inputs.items() for W in (10, 100)}
+    lm_row = {}
+    if args.lm:
+        tmp = tempfile.mkdtemp(prefix="ds2_bench_lm_")
+        path = os.path.join(tmp, "synthetic_3gram.arpa.gz")
+        LO.synthetic_arpa(path, 200000, 3, [1500000, 1500000], seed=7, alphabet="ABCDEFGHIJKLMNOPQRSTUVWXYZ'",
+                          max_len=10, gz=True)
+        from deepspeech_pytorch_b200.lm import LanguageModel
+        t0 = time.perf_counter()
+        lm = LanguageModel(path, ds.LABELS, 0)
+        lm_row["lm_host_parse_and_trie_s"] = round(time.perf_counter() - t0, 2)
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        a.record()
+        lm.device_tables(dev)
+        b.record()
+        b.synchronize()
+        lm_row["lm_device_build_ms"] = round(a.elapsed_time(b), 2)
+        lm_row["lm_device_build_wall_ms"] = round(1e3 * (time.perf_counter() - t0), 1)
+        lm_row["lm_table_bytes"] = lm.table_bytes
+        lm_row["lm_ngrams"] = [len(x) for x in lm.model.logp]
+        lm_row["lm_trie_nodes"] = len(lm.trie.mask)
+        lm_row["lm_alpha_beta"] = [LM_ALPHA, LM_BETA]
+        calls.update({("lm_" + k, W): Call(p, W, lm) for k, p in inputs.items() for W in (10, 100)})
     for c in calls.values():
         c()
     forward()
@@ -162,6 +211,25 @@ def main():
     row["decode_model_W100_over_forward"] = round(med[("model", 100)] / med["forward"], 3)
     row["oracle_check_W100_model_2utts"] = "equal" if ok else "MISMATCH"
     row["oracle_margin"] = float(f"{ref['margin']:.3g}")
+    if args.lm:
+        row.update(lm_row)
+        row["decode_lm_model_W100_over_forward"] = round(med[("lm_model", 100)] / med["forward"], 3)
+        c = calls[("lm_model", 100)]
+        c()
+        torch.cuda.synchronize()
+        ref = LO.beam_decode_lm(model_probs[:2].cpu(), None, ds.LABELS, LO.read_arpa(path), LM_ALPHA, LM_BETA,
+                                blank=0, beam_width=100, cutoff_top_n=40, cutoff_prob=1.0)
+        lm_ok = (c.n_beams[:2].cpu().numpy().tolist() == ref["n_beams"].tolist()
+                 and np.array_equal(c.lengths[:2].cpu().numpy(), ref["lengths"])
+                 and np.array_equal(c.labels[:2].cpu().numpy(), ref["labels"])
+                 and np.array_equal(c.timesteps[:2].cpu().numpy(), ref["timesteps"]))
+        s, r = c.scores[:2].cpu().numpy(), ref["scores"]
+        f = np.isfinite(r)
+        lm_ok = lm_ok and bool(np.all(np.abs(s[f] - r[f]) <= 1e-10 * np.maximum(1.0, np.abs(r[f]))))
+        row["lm_oracle_check_W100_model_2utts"] = "equal" if lm_ok else "MISMATCH"
+        row["lm_oracle_margin"] = float(f"{ref['margin']:.3g}")
+        row["lm_top_beam_utt0"] = ''.join(ds.LABELS[int(x)] for x in c.labels[0, 0, :int(c.lengths[0, 0])])[:80]
+        ok = ok and lm_ok
     print(json.dumps(row))
     if not ok:
         raise SystemExit("bench_beam_decode: GPU result differs from the oracle")
