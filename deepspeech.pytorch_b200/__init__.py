@@ -3,8 +3,8 @@
 registers the package under that importable name)."""
 from . import _lib
 from ._lib import Ds2Error, get_lib
-from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, LMConfig, OptimConfig,
-                      SGDConfig, SpectConfig, UniDirectionalConfig)
+from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, InferenceConfig, LMConfig,
+                      ModelConfig, OptimConfig, SGDConfig, SpectConfig, TranscribeConfig, UniDirectionalConfig)
 from .enums import DecoderType, RNNType, SpectrogramWindow
 from .labels import LABELS
 
@@ -24,3 +24,4 @@ def get_precision() -> str:
 from . import ops  # noqa: E402
 from .decoder import BeamCTCDecoder, GreedyDecoder, load_decoder  # noqa: E402
 from .model import DeepSpeech  # noqa: E402
+from .inference import (ChunkSpectrogramParser, decode_results, load_audio, run_transcribe)  # noqa: E402

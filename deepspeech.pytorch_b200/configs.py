@@ -81,6 +81,29 @@ class LMConfig:
     lm_workers: int = 4         # ctcdecode's CPU worker count; ignored by the GPU decoder
 
 
+@dataclass
+class ModelConfig:
+    """inference_config.py:19-23"""
+    precision: int = 32         # 16: the recurrent stack's GEMMs and sweeps on fp16 operands (`set_precision('fp16')`)
+    cuda: bool = True
+    model_path: str = ''
+
+
+@dataclass
+class InferenceConfig:
+    """inference_config.py:26-29"""
+    lm: LMConfig = field(default_factory=LMConfig)
+    model: ModelConfig = field(default_factory=ModelConfig)
+
+
+@dataclass
+class TranscribeConfig(InferenceConfig):
+    """inference_config.py:32-36 (the settings of `run_transcribe` and `decode_results`)"""
+    audio_path: str = ''        # WAV file to transcribe
+    offsets: bool = False       # also return the frame offsets of the characters
+    chunk_size_seconds: float = -1   # <= 0: the whole file in one forward
+
+
 def cfg_type(cfg):
     """OmegaConf.get_type(cfg) when omegaconf wraps the config, else type(cfg) (model.py:152,274,282)."""
     try:

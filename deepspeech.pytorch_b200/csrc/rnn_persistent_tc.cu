@@ -74,6 +74,8 @@ struct PersistParams {
   float* xbuf;          // split-K bwd, exchange through L2: [CTA][source rank][step parity] partial dh_rec tiles
   unsigned int* xcnt;   //   ... [CTA] number of partial tiles received (monotonic, zeroed by the host)
   int* err;             // set to 1 if a barrier wait timed out
+  const float* h0;      // resident / split-K fwd with an initial state (ST): (D,B,H) or null (zeros)
+  const float* c0;      //   ... LSTM cell state, (D,B,H) or null
 };
 
 __device__ __forceinline__ void red_release(unsigned int* p, unsigned int v) {
@@ -149,10 +151,14 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 // fp16 copy of h_{t-1} (B x H, 64 KB) is streamed by TMA, and the MMAs are kind::f16 (K=16, half the
 // instruction count).  fp16 has the same 10-bit mantissa as TF32 and |h| < 1, |w| << 65504, so this
 // is the same arithmetic class as the TF32 path (fp32 accumulation either way).
-template <int RNN, bool RES>
+// ST (resident only): initial state p.h0 / p.c0.  Step 0 then runs the MMAs too, on fp16(h0) from the extra time step
+// of h16 (f16_weight_maps), the carried cst starts from c0 (LSTM) / h0 (GRU), and the reverse direction writes
+// fp16(h0) instead of 0 into the h16 rows of its padded steps: row len[b] is the operand of utterance b's first step.
+template <int RNN, bool RES, bool ST = false>
 __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const __grid_constant__ PersistParams p) {
   using namespace rp;
   using namespace tc;
+  static_assert(RES || !ST, "the streaming variant reads h_{t-1} from hseq and cannot carry an initial state");
   constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned, still __shared__
@@ -185,7 +191,15 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
     mbar_init(accum_bar, 1);
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < UT * NBp; i += THREADS) cst[i] = 0.f;
+  for (int i = threadIdx.x; i < UT * NBp; i += THREADS) {
+    float v = 0.f;
+    if constexpr (ST) {
+      const float* s0 = RNN == DS2_RNN_LSTM ? p.c0 : p.h0;
+      const int b = i % NBp;
+      if (RNN != DS2_RNN_TANH && s0 && b < B) v = s0[((size_t)d * B + b) * H + u0 + i / NBp];
+    }
+    cst[i] = v;
+  }
   for (int i = threadIdx.x; i < NB; i += THREADS) lens_s[i] = i < B ? p.len[i] : 0;
   __syncthreads();
   const uint32_t tx_bytes = (uint32_t)(G * UT * 128 + B * 128);
@@ -197,9 +211,10 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
         mbar_arrive_expect_tx(&empty[0], (uint32_t)(NKR * G * UT * 128));
         for (int c = 0; c < NKR; ++c) tma_load_3d(smem + c * A_BYTES, &p.tmW[d], &empty[0], c * 64, u0, 0);
         uint8_t* hbuf = smem + NKR * A_BYTES;
-        for (int step = 1; step < T; ++step) {
+        for (int step = ST ? 0 : 1; step < T; ++step) {
           const int t = d == 0 ? step : T - 1 - step;
           const int tp = d == 0 ? t - 1 : t + 1;
+          const int row = (ST ? tp + 1 : tp) * B;         // ST: the maps start at time step -1
           // the previous step's MMAs have finished reading hbuf: this CTA's epilogue (which waited for them)
           // arrived at the barrier we are about to pass
           grid_wait_counter(ctr, (unsigned int)p.NT * (unsigned int)step, p.err);
@@ -210,10 +225,10 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
             const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
             if (p.box3) {
               mbar_arrive_expect_tx(fb, (uint32_t)(4 * B_BYTES));
-              tma_load_3d(hbuf + c0 * B_BYTES, &p.tmV3[d], fb, 0, tp * B, c0);
+              tma_load_3d(hbuf + c0 * B_BYTES, &p.tmV3[d], fb, 0, row, c0);
             } else {
               mbar_arrive_expect_tx(fb, (uint32_t)((c1 - c0) * B * 128));
-              for (int c = c0; c < c1; ++c) tma_load_2d(hbuf + c * B_BYTES, &p.tmV[d], fb, c * 64, tp * B);
+              for (int c = c0; c < c1; ++c) tma_load_2d(hbuf + c * B_BYTES, &p.tmV[d], fb, c * 64, row);
             }
           }
           trace_stamp(p.trace, p.T, step, 1);
@@ -254,7 +269,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
           const uint64_t a_step = (uint64_t)(A_BYTES >> 4), b_step = (uint64_t)(B_BYTES >> 4);
           mbar_wait(&empty[0], 0);                 // weights resident
           uint32_t ph = 0;
-          for (int step = 1; step < T; ++step) {
+          for (int step = ST ? 0 : 1; step < T; ++step) {
             for (int g = 0; g < NG; ++g) {
               mbar_wait(full + g, ph);
               if (g == 0 && lane == 0) trace_stamp(p.trace, p.T, step, 2);
@@ -317,7 +332,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
           gx[j] = (has_row && b < B) ? p.gates[(((size_t)t * B + b) * D + d) * GH + (size_t)gsel * H + u] : 0.f;
         }
         float a16[16];
-        if (step > 0 && q < G) {
+        if ((ST || step > 0) && q < G) {
           if (cb == 0) { mbar_wait(accum_bar, acc_phase); if (e == 0) trace_stamp(p.trace, p.T, step, 5); }
           float acc[32];
           tmem_ld32(acc_img, acc_pitch(NB), ((uint32_t)(q * 32) << 16) + (uint32_t)cb, acc);
@@ -360,7 +375,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
           if (b < B) ex[(q * UT + ul) * NBp + b] = v[j];
         }
       }
-      if (step > 0) acc_phase ^= 1;
+      if (ST || step > 0) acc_phase ^= 1;
       if (e == 0) trace_stamp(p.trace, p.T, step, 6);
       named_bar_sync(1, 128);
       if (e == 0) trace_stamp(p.trace, p.T, step, 7);
@@ -420,6 +435,12 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
         }
 #pragma unroll
         for (int j = 0; j < NDF; ++j) o[5][j] = hval[j];
+        if constexpr (ST) {
+          if (!valid && d == 1) {
+#pragma unroll
+            for (int j = 0; j < NDF; ++j) hval[j] = p.h0 ? p.h0[((size_t)B + b) * H + u0 + uq + j] : 0.f;
+          }
+        }
         if (RES) {
           const __half2 lo = __floats2half2_rn(hval[0], hval[1]), hi = __floats2half2_rn(hval[2], hval[3]);
           uint2 pk;
@@ -530,7 +551,7 @@ static PersistParams sweep_params(const SeqArgs& a, int units, const char* trace
   PersistParams p{};
   p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / units; p.G = a.G;
   p.training = a.training;
-  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy;
+  p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy; p.h0 = a.h0; p.c0 = a.c0;
   for (int d = 0; d < a.D; ++d) { p.b_ih[d] = a.b_ih[d]; p.b_hh[d] = a.b_hh[d]; }
   p.trace = trace_ptr_from_env(trace_env);
   p.defer = sweep_defer_default();
@@ -646,16 +667,16 @@ static size_t fwd_smem_bytes(int NB) {
 }
 
 static size_t splitk_res_ws_bytes(int G, int T, int B, int H, int D);
+static size_t res_ws_bytes(int G, int T, int B, int H, int D);
 
 size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
   const int G = rnn == DS2_RNN_LSTM ? 4 : (rnn == DS2_RNN_GRU ? 3 : 1);
-  const size_t fwd = 4096 + align_up((size_t)D * G * H * H * 2, 256) + align_up((size_t)D * T * B * H * 2, 256);
+  const size_t fwd = res_ws_bytes(G, T, B, H, D);
   const size_t bwd = splitk_res_ws_bytes(G, T, B, H, D);
   return (fwd > bwd ? fwd : bwd) + 256;
 }
 
 static bool fwd_eligible(const SeqArgs& a) {
-  if (a.h0 || a.c0) return false;                 // initial states -> generic step kernels
   if (a.H % 32 != 0 || a.B > 256 || a.T < 2) return false;
   return vec_ok(a.gates, a.hseq, a.aux);
 }
@@ -672,35 +693,46 @@ static size_t res_smem_bytes(int NB, int H) {
          (32 + STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
-// workspace of the resident forward: [4 KB control][W16: D*G*H*H halfs][h16: D*T*B*H halfs]
+// workspace of the resident forward: [4 KB control][W16: D*G*H*H halfs][h16: (D*T + 2)*B*H halfs].  h16 is the
+// (D,T,B,H) sequence with one extra time step before it and one after it: the operands fp16(h0[0]) of the forward
+// direction's step t = 0 ("t = -1") and fp16(h0[1]) of the reverse direction's step t = T-1 ("t = T").
 static size_t res_ws_bytes(int G, int T, int B, int H, int D) {
-  return 4096 + align_up((size_t)D * G * H * H * 2, 256) + align_up((size_t)D * T * B * H * 2, 256);
+  return 4096 + align_up((size_t)D * G * H * H * 2, 256) + align_up(((size_t)D * T + 2) * B * H * 2, 256);
 }
 
 // Resident forward variants: the fp16 copy of W_hh (in the workspace) and the tensor maps of it and of the fp16 h
 // sequence.  `chunks`: 64-wide K chunks a CTA streams per step; a multiple of 4 takes one 3-D box per group of 4.
 // A box of W_hh holds 16 units; its rows are [gate][unit], or with `unit_major` [unit][4 gate rows] (a (k, gate, unit)
 // map, the GRU's fourth row of a unit is zero fill).
+// `state` (the kernels' ST): the h sequence maps start one time step earlier, so that row (tp + 1) * B of direction
+// d's map is time step tp, tp = -1 .. T; the extra steps are filled with fp16(h0) (zeros where h0 is null).
 static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chunks, cudaStream_t st,
-                           bool unit_major = false) {
+                           bool unit_major = false, bool state = false) {
   using namespace rp;
   const int G = a.G;
+  const size_t BH = (size_t)a.B * a.H;
   __half* w16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096);
-  p.h16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096 + align_up((size_t)a.D * G * a.H * a.H * 2, 256));
+  p.h16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096 + align_up((size_t)a.D * G * a.H * a.H * 2, 256)) + BH;
   const size_t wn = (size_t)G * a.H * a.H;
   p.box3 = chunks % 4 == 0;
+  const int rows = (a.T + (state ? 2 : 0)) * a.B;
   for (int d = 0; d < a.D; ++d) {
     DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
     int rc = unit_major
                  ? make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, G, a.H, (size_t)a.H * a.H, (size_t)a.H, 64, 4, UT)
                  : make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
     if (rc) return rc;
-    rc = make_tmap_f16(&p.tmV[d], p.h16 + (size_t)d * a.T * a.B * a.H, 2, a.H, a.T * a.B, 1, (size_t)a.H, 0, 64, a.B, 1);
+    __half* hbase = p.h16 + (size_t)d * a.T * BH - (state ? BH : 0);
+    rc = make_tmap_f16(&p.tmV[d], hbase, 2, a.H, rows, 1, (size_t)a.H, 0, 64, a.B, 1);
     if (rc) return rc;
     if (p.box3) {   // rows b >= B of a box belong to the next time step (or are zero-filled): those N columns are discarded
-      rc = make_tmap_f16(&p.tmV3[d], p.h16 + (size_t)d * a.T * a.B * a.H, 3, 64, a.T * a.B, a.H / 64, (size_t)a.H, 64, 64,
-                         p.NB, 4);
+      rc = make_tmap_f16(&p.tmV3[d], hbase, 3, 64, rows, a.H / 64, (size_t)a.H, 64, 64, p.NB, 4);
       if (rc) return rc;
+    }
+    if (state) {   // forward: the step before t = 0; reverse: the step after t = T - 1
+      __half* slot = d == 0 ? p.h16 - BH : p.h16 + (size_t)a.D * a.T * BH;
+      if (a.h0) DS2_LAUNCH(f32_to_f16_kernel, 132, 256, 0, st, BH, a.h0 + (size_t)d * BH, slot);
+      else DS2_CHECK_CUDA(cudaMemsetAsync(slot, 0, BH * sizeof(__half), st));
     }
   }
   return DS2_OK;
@@ -716,13 +748,15 @@ static int launch_fwd_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cuda
   if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   const size_t smem = one_cta_per_sm(res_smem_bytes(p.NB, a.H));
   if (smem > 227 * 1024) return 1;
-  const SweepKernel kern = rnn_fwd_persist_kernel<RNN, true>;
+  const bool state = a.h0 || a.c0;
+  const SweepKernel kern = state ? rnn_fwd_persist_kernel<RNN, true, true> : rnn_fwd_persist_kernel<RNN, true>;
   static DeviceOnce attr_once;
   int fit = 0;
-  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
+  if (int rc = opt_in_smem(attr_once, {rnn_fwd_persist_kernel<RNN, true>, rnn_fwd_persist_kernel<RNN, true, true>}))
+    return rc;
   if (int rc = coop_fit(kern, smem, &fit)) return rc;
   return launch_sweep(kern, 0, p.NT, smem, fit, true, 4096, nullptr, nullptr, p, st,
-                      [&] { return f16_weight_maps(a, p, ws, a.H / 64, st); });
+                      [&] { return f16_weight_maps(a, p, ws, a.H / 64, st, false, state); });
 }
 
 template <int RNN>
@@ -741,6 +775,9 @@ static int launch_fwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t 
     int rc = launch_fwd_resident<RNN>(a, ws, ws_bytes, st);
     if (rc != 1) return rc;
   }
+  // The streaming variant reads h_{t-1} from the fp32 output hseq, which must stay 0 at padded steps and has no step
+  // before the first: it cannot carry an initial state.
+  if (a.h0 || a.c0) return 1;
   PersistParams p = sweep_params(a, UT, "DS2_TRACE_FWD", ws);
   if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   if (ws_bytes < 4096) return 1;
@@ -1612,8 +1649,10 @@ __device__ __forceinline__ void quad_transpose(float (&v)[16]) {
   }
 }
 
-template <int RNN, int NKR_T = 0>
-__global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __grid_constant__ PersistParams p) {
+// ST: initial state p.h0 / p.c0, as in rnn_fwd_persist_kernel (step 0 runs the MMAs on fp16(h0), cs starts from
+// c0 / h0, the reverse direction's padded steps write fp16(h0) into h16).  The body is shared by the two kernels below.
+template <int RNN, int NKR_T, bool ST>
+__device__ __forceinline__ void fwd_splitk_sweep(const PersistParams& p) {
   using namespace rp;
   using namespace tc;
   constexpr int G = RNN == DS2_RNN_LSTM ? 4 : 3;
@@ -1663,9 +1702,10 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
         tma_load_3d(smem + c * AW + 64 * 128, &p.tmW[d], wbar, (kc0 + c) * 64, 0, U0 + (rank ^ 1) * UT);
       }
       uint8_t* hbuf = smem + NKR * AW;
-      for (int step = 1; step < T; ++step) {
+      for (int step = ST ? 0 : 1; step < T; ++step) {
         const int t = d == 0 ? step : T - 1 - step;
         const int tp = d == 0 ? t - 1 : t + 1;
+        const int row = (ST ? tp + 1 : tp) * B;           // ST: the maps start at time step -1
         // every CTA has finished the previous step, this one included: its MMAs no longer read hbuf
         grid_wait_counter(ctr, n_arrive * (unsigned int)step, p.err);
         fence_proxy_async_global();
@@ -1675,10 +1715,10 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
           const int c0 = grp_begin(g), c1 = min(NKR, grp_begin(g + 1));
           if (p.box3) {
             mbar_arrive_expect_tx(fb, (uint32_t)(4 * B_BYTES));
-            tma_load_3d(hbuf + c0 * B_BYTES, &p.tmV3[d], fb, 0, tp * B, kc0 + c0);
+            tma_load_3d(hbuf + c0 * B_BYTES, &p.tmV3[d], fb, 0, row, kc0 + c0);
           } else {
             mbar_arrive_expect_tx(fb, (uint32_t)((c1 - c0) * B * 128));
-            for (int c = c0; c < c1; ++c) tma_load_2d(hbuf + c * B_BYTES, &p.tmV[d], fb, (kc0 + c) * 64, tp * B);
+            for (int c = c0; c < c1; ++c) tma_load_2d(hbuf + c * B_BYTES, &p.tmV[d], fb, (kc0 + c) * 64, row);
           }
         }
         trace_stamp(p.trace, p.T, step, 1);
@@ -1706,7 +1746,14 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
 #pragma unroll
       for (int c = 0; c < NCH; ++c)
 #pragma unroll
-        for (int k = 0; k < 4; ++k) cs[c][k] = 0.f;
+        for (int k = 0; k < 4; ++k) {
+          cs[c][k] = 0.f;
+          if constexpr (ST) {
+            const float* s0 = RNN == DS2_RNN_LSTM ? p.c0 : p.h0;
+            const int b = 32 * c + fwd_cell_col(tid, k);
+            if (s0 && b < B) cs[c][k] = s0[((size_t)d * B + b) * H + u0 + fwd_cell_unit(tid, k)];
+          }
+        }
       const uint32_t dst_part = mapa_u32(smem_u32(part + tid), (uint32_t)(rank ^ 1));
       const uint32_t dst_bar = mapa_u32(smem_u32(part_bar), (uint32_t)(rank ^ 1));
       const uint32_t part_tx = (uint32_t)(64 * NB * 4);
@@ -1732,9 +1779,9 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
           }
         };
         if (NCH == 1) load_gx(0);
-        // s[c][4 g + k]: recurrent sum of gate g of cell k (zero at the first step: h_{-1} = 0)
+        // s[c][4 g + k]: recurrent sum of gate g of cell k (without ST zero at the first step: h_{-1} = 0)
         float s[NCH][16];
-        if (step > 0) {
+        if (ST || step > 0) {
           if (tid == 0) mbar_arrive_expect_tx(part_bar, part_tx);   // arm this step's phase (the peer may already have sent)
           WgAcc<2, NCH> acc;                             // live from the first MMA of the step to the partial sums only
           if constexpr (NKR_T > 0) {
@@ -1898,7 +1945,14 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
             if (q < G || q >= 4) fwd_units4(o[q], sv[c][q]);
           const int b = 32 * c + bs;
           if (b < B) {                                   // fp16 h_t: the MMA operand of the next step
-            const __half2 lo = __floats2half2_rn(sv[c][5][0], sv[c][5][1]), hi = __floats2half2_rn(sv[c][5][2], sv[c][5][3]);
+            float h4[4] = {sv[c][5][0], sv[c][5][1], sv[c][5][2], sv[c][5][3]};
+            if constexpr (ST) {
+              if (d == 1 && t >= p.len[b]) {
+#pragma unroll
+                for (int j = 0; j < 4; ++j) h4[j] = p.h0 ? p.h0[((size_t)B + b) * H + us + j] : 0.f;
+              }
+            }
+            const __half2 lo = __floats2half2_rn(h4[0], h4[1]), hi = __floats2half2_rn(h4[2], h4[3]);
             uint2 pk;
             pk.x = *reinterpret_cast<const unsigned int*>(&lo);
             pk.y = *reinterpret_cast<const unsigned int*>(&hi);
@@ -1951,6 +2005,24 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __
   cluster_sync_all();                                     // nobody exits while the peer may still write into its tile
 }
 
+template <int RNN, int NKR_T = 0>
+__global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_kernel(const __grid_constant__ PersistParams p) {
+  fwd_splitk_sweep<RNN, NKR_T, false>(p);
+}
+// With an initial state: compile-time chunk counts only, and only those whose ST body compiles without local memory
+// (ptxas: H / 128 = 1, 5, 8, 9, i.e. H = 128, 640, 1024, 1152).  The runtime-count body and the counts 2-4, 6, 7, 10
+// spill 8-596 bytes at the 168-register cap; a state at those H takes the 16-unit kernel where it fits.
+constexpr int FWD_SPLITK_MAX_NKR = 10;   // shared memory holds at most 10 chunks (H = 1280)
+template <int RNN, int NKR_T>
+__global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_splitk_state_kernel(const __grid_constant__ PersistParams p) {
+  static_assert(NKR_T == 1 || NKR_T == 5 || NKR_T == 8 || NKR_T == 9, "an ST chunk count that compiles without spills");
+  fwd_splitk_sweep<RNN, NKR_T, true>(p);
+}
+template <int RNN>
+static const SweepKernel fwd_splitk_state_kernels[FWD_SPLITK_MAX_NKR] = {
+    rnn_fwd_splitk_state_kernel<RNN, 1>, nullptr, nullptr, nullptr, rnn_fwd_splitk_state_kernel<RNN, 5>, nullptr,
+    nullptr, rnn_fwd_splitk_state_kernel<RNN, 8>, rnn_fwd_splitk_state_kernel<RNN, 9>, nullptr};
+
 static size_t fwd_splitk_smem_bytes(int NB, int H, bool defer) {
   return 1024 + (size_t)(H / 128) * (128 * 128 + (size_t)NB * 128) + (size_t)64 * NB * sizeof(float) +
          (defer && NB == 32 ? 6 * 128 * 16 : 0) + 10 * sizeof(uint64_t) + 64;
@@ -1967,13 +2039,20 @@ static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   if (p.NB > 64) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
   const size_t smem = one_cta_per_sm(fwd_splitk_smem_bytes(p.NB, a.H, p.defer));
   if (smem > 227 * 1024) return 1;
-  // H = 1024: unrolled issue loop
-  const SweepKernel kern = a.H == 1024 ? rnn_fwd_splitk_kernel<RNN, 8> : rnn_fwd_splitk_kernel<RNN, 0>;
+  // H = 1024: unrolled issue loop; with an initial state, see rnn_fwd_splitk_state_kernel
+  const bool state = a.h0 || a.c0;
+  const int nkr = a.H / 128;
+  if (state && (nkr > FWD_SPLITK_MAX_NKR || !fwd_splitk_state_kernels<RNN>[nkr - 1])) return 1;
+  const SweepKernel kern = state ? fwd_splitk_state_kernels<RNN>[nkr - 1]
+                                 : (a.H == 1024 ? rnn_fwd_splitk_kernel<RNN, 8> : rnn_fwd_splitk_kernel<RNN, 0>);
   static DeviceOnce attr_once;
-  if (int rc = opt_in_smem(attr_once, {rnn_fwd_splitk_kernel<RNN, 8>, rnn_fwd_splitk_kernel<RNN, 0>})) return rc;
+  const SweepKernel* sk = fwd_splitk_state_kernels<RNN>;
+  if (int rc = opt_in_smem(attr_once, {rnn_fwd_splitk_kernel<RNN, 8>, rnn_fwd_splitk_kernel<RNN, 0>, sk[0], sk[4], sk[7],
+                                       sk[8]}))
+    return rc;
   const int fit = cluster_fit(kern, 2, a.D * p.NT * 2, smem, st);
   return launch_sweep(kern, 2, p.NT * 2, smem, fit, true, 4096, "split-K forward sweep", "the 16-unit kernel", p, st,
-                      [&] { return f16_weight_maps(a, p, ws, a.H / 128, st, true); });
+                      [&] { return f16_weight_maps(a, p, ws, a.H / 128, st, true, state); });
 }
 
 static size_t splitk_smem_bytes(int NB, int CL) {
