@@ -3,8 +3,9 @@
 registers the package under that importable name)."""
 from . import _lib
 from ._lib import Ds2Error, get_lib
-from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, InferenceConfig, LMConfig,
-                      ModelConfig, OptimConfig, SGDConfig, SpectConfig, TranscribeConfig, UniDirectionalConfig)
+from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, EvalConfig, InferenceConfig,
+                      LMConfig, ModelConfig, OptimConfig, OptimizerConfig, SGDConfig, SpectConfig, TranscribeConfig,
+                      UniDirectionalConfig)
 from .enums import DecoderType, RNNType, SpectrogramWindow
 from .labels import LABELS
 
@@ -25,3 +26,6 @@ from . import ops  # noqa: E402
 from .decoder import BeamCTCDecoder, GreedyDecoder, load_decoder  # noqa: E402
 from .model import DeepSpeech  # noqa: E402
 from .inference import (ChunkSpectrogramParser, decode_results, load_audio, run_transcribe)  # noqa: E402
+from .evaluation import (AudioDataLoader, SpectrogramDataset, error_counts, evaluate, load_model,  # noqa: E402
+                         run_evaluation)
+from .lm_search import LMParamSearch, search_lm_params  # noqa: E402

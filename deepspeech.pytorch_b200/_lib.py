@@ -55,6 +55,11 @@ PROTOTYPES = {
     "ds2_beam_decode_lm_workspace_bytes": (sz, [i32] * 4),
     "ds2_beam_decode_lm": (i32, [i32, i32, i32, vp, vp, i32, i32, i32, f32, vp, i32, C.c_double, C.c_double, i32]
                            + [vp] * 6 + [sz, vp]),
+    "ds2_beam_decode_lm_grid_workspace_bytes": (sz, [i32] * 5),
+    "ds2_beam_decode_lm_grid": (i32, [i32, i32, i32, vp, vp, i32, i32, i32, f32, vp, i32, i32, vp, i32]
+                                + [vp] * 3 + [sz, vp]),
+    "ds2_error_counts_workspace_bytes": (sz, [i32, i32, i64, i32]),
+    "ds2_error_counts": (i32, [i32, i32, i32, vp, vp, vp, i64, vp, i32, i32, i32] + [vp] * 3 + [sz, vp]),
     "ds2_spectrogram_workspace_bytes": (sz, [i32]),
     "ds2_spectrogram_batch": (i32, [i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, vp, i32, vp, sz, vp]),
     "ds2_spec_augment_workspace_bytes": (sz, [i32]),

@@ -104,6 +104,40 @@ class TranscribeConfig(InferenceConfig):
     chunk_size_seconds: float = -1   # <= 0: the whole file in one forward
 
 
+@dataclass
+class EvalConfig(InferenceConfig):
+    """inference_config.py:39-45 (the settings of `evaluate`); `verbose` and `save_output` are unused there too"""
+    test_path: str = ''         # JSON manifest or directory of .wav files with transcripts under /txt/
+    verbose: bool = True
+    save_output: str = ''
+    batch_size: int = 20
+    num_workers: int = 4
+
+
+@dataclass
+class OptimizerConfig:
+    """search_lm_params.py:15-31 (the settings of `search_lm_params`) plus `seed` and `output_path`.  `n_jobs` and
+    the decoding use of `num_workers` have no effect on the GPU search; `num_workers` still sets the loader's file
+    readers."""
+    model_path: str = ''
+    test_path: str = ''
+    is_character_based: bool = True   # pick the best pair by CER (True) or WER (False)
+    lm_path: str = ''
+    beam_width: int = 10
+    alpha_from: float = 0.0
+    alpha_to: float = 3.0
+    beta_from: float = 0.0
+    beta_to: float = 1.0
+    n_trials: int = 500
+    n_jobs: int = 2
+    precision: int = 16
+    batch_size: int = 1
+    num_workers: int = 1
+    spect_cfg: SpectConfig = field(default_factory=SpectConfig)
+    seed: int = 0               # seed of the trial draws (numpy.random.default_rng)
+    output_path: str = ''       # where to write [[alpha, beta, wer, cer], ...] (select_lm_params.py's input)
+
+
 def cfg_type(cfg):
     """OmegaConf.get_type(cfg) when omegaconf wraps the config, else type(cfg) (model.py:152,274,282)."""
     try:

@@ -175,13 +175,18 @@ __device__ __forceinline__ long long hash_slot(unsigned long long k, long long H
   return (long long)(k & (unsigned long long)(HC - 1));
 }
 
-template <bool LM>
-__global__ void __launch_bounds__(BEAM_THREADS)
-beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t* __restrict__ out_len, int blank,
-                   int W, int top_n, float cutoff_prob, int32_t* __restrict__ labels, int32_t* __restrict__ timesteps,
-                   int32_t* __restrict__ lengths, double* __restrict__ scores, int32_t* __restrict__ n_beams,
-                   BeamPool pool, BeamLm lmp) {
-  const int u = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+// One beam search: utterance u, in pool slot `slot`, written to output row `out`.  TOP = false writes every beam
+// (rule 6) at out = u; TOP = true writes only the best beam: labels row `out` of (rows, T) and lengths[out] (the grid
+// entry, where timesteps, scores and n_beams are NULL).  Both kernels below run this body.
+template <bool LM, bool TOP>
+__device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T, int C,
+                                                 const float* __restrict__ probs, const int32_t* __restrict__ out_len,
+                                                 int blank, int W, int top_n, float cutoff_prob,
+                                                 int32_t* __restrict__ labels, int32_t* __restrict__ timesteps,
+                                                 int32_t* __restrict__ lengths, double* __restrict__ scores,
+                                                 int32_t* __restrict__ n_beams, const BeamPool& pool,
+                                                 const BeamLm& lmp) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* key = reinterpret_cast<unsigned long long*>(smem_raw);
   double* lb = reinterpret_cast<double*>(key + (size_t)W * C);
@@ -219,13 +224,13 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
   __shared__ int n_list, nK, n_valid, n_sel, need, passes, done, pre_e, pool_next;
 
   const long long NP = pool.NP, HC = pool.HC;
-  int* P_par = pool.parent + (size_t)u * NP;
-  int* P_lab = pool.label + (size_t)u * NP;
-  int* P_ts = pool.ts + (size_t)u * NP;
-  int* P_depth = pool.depth + (size_t)u * NP;
-  double* P_best = pool.best + (size_t)u * NP;
-  unsigned long long* hk = pool.hkey + (size_t)u * HC;
-  int* hv = pool.hval + (size_t)u * HC;
+  int* P_par = pool.parent + (size_t)slot * NP;
+  int* P_lab = pool.label + (size_t)slot * NP;
+  int* P_ts = pool.ts + (size_t)slot * NP;
+  int* P_depth = pool.depth + (size_t)slot * NP;
+  double* P_best = pool.best + (size_t)slot * NP;
+  unsigned long long* hk = pool.hkey + (size_t)slot * HC;
+  int* hv = pool.hval + (size_t)slot * HC;
 
   for (long long i = tid; i < HC; i += BEAM_THREADS) hk[i] = 0ull;
   const int Tu = out_len ? min(max(out_len[u], 0), T) : T;
@@ -500,7 +505,7 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
         node2[tid] = found;
         is_new = found < 0;
         if constexpr (LM) {                                 // a returning prefix (rule 2) keeps its lm value;
-          lmv_new = is_new ? 0.0 : pool.lm[(size_t)u * NP + found];   // a new one is looked up below
+          lmv_new = is_new ? 0.0 : pool.lm[(size_t)slot * NP + found];   // a new one is looked up below
         }
       }
     }
@@ -530,7 +535,7 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
           hs = (hs + 1) & (HC - 1);
         }
         node2[tid] = id;
-        if constexpr (LM) pool.lm[(size_t)u * NP + id] = lmv_new;
+        if constexpr (LM) pool.lm[(size_t)slot * NP + id] = lmv_new;
       }
       lb[tid] = b2[tid]; lnb[tid] = nb2[tid]; sc[tid] = lse(b2[tid], nb2[tid]);
       lab[tid] = lab2[tid]; node[tid] = node2[tid]; pnode[tid] = pnode2[tid];
@@ -577,7 +582,25 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
   }
 
   // ---- output (rule 6): zero the rows, then walk each beam's parent chain
-  const size_t row0 = (size_t)u * W * T;
+  if constexpr (TOP) {
+    int32_t* L = labels + (size_t)out * T;
+    for (int x = tid; x < T; x += BEAM_THREADS) L[x] = 0;
+    __syncthreads();
+    const int n = n_list;
+    if (n == 0) {
+      if (tid == 0) lengths[out] = 0;
+    } else if (tid < n && (LM ? rnk[tid] : tid) == 0) {
+      int nd = node[tid];
+      const int len = P_depth[nd];
+      lengths[out] = len;
+      for (int pos = len - 1; pos >= 0; --pos) {
+        L[pos] = P_lab[nd];
+        nd = P_par[nd];
+      }
+    }
+    return;
+  }
+  const size_t row0 = (size_t)out * W * T;
   for (size_t x = tid; x < (size_t)W * T; x += BEAM_THREADS) {
     labels[row0 + x] = 0;
     timesteps[row0 + x] = 0;
@@ -585,7 +608,7 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
   __syncthreads();
   if (tid < W) {
     const int r = LM && tid < n_list ? rnk[tid] : tid;
-    const size_t o = (size_t)u * W + r;
+    const size_t o = (size_t)out * W + r;
     if (tid < n_list) {
       int nd = node[tid];
       const int len = P_depth[nd];
@@ -603,7 +626,39 @@ beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t*
       scores[o] = CUDART_INF;
     }
   }
-  if (tid == 0) n_beams[u] = n_list;
+  if (tid == 0) n_beams[out] = n_list;
+}
+
+// ds2_beam_decode / ds2_beam_decode_lm: one CTA per utterance, pool slot = utterance
+template <bool LM>
+__global__ void __launch_bounds__(BEAM_THREADS)
+beam_decode_kernel(int T, int C, const float* __restrict__ probs, const int32_t* __restrict__ out_len, int blank,
+                   int W, int top_n, float cutoff_prob, int32_t* __restrict__ labels, int32_t* __restrict__ timesteps,
+                   int32_t* __restrict__ lengths, double* __restrict__ scores, int32_t* __restrict__ n_beams,
+                   BeamPool pool, BeamLm lmp) {
+  const int u = blockIdx.x;
+  beam_search_item<LM, false>(u, u, u, T, C, probs, out_len, blank, W, top_n, cutoff_prob, labels, timesteps,
+                              lengths, scores, n_beams, pool, lmp);
+}
+
+// ds2_beam_decode_lm_grid: item i = u * K + k is utterance u with pair k (utterance-major, so the caller's length
+// order is the start order).  CTA b runs items b, b + gridDim.x, ... in its own pool slot b; each item starts from a
+// cleared hash and node 0, so which slot runs an item does not change its result.
+__global__ void __launch_bounds__(BEAM_THREADS)
+beam_decode_grid_kernel(int B, int K, int T, int C, const float* __restrict__ probs,
+                        const int32_t* __restrict__ out_len, int blank, int W, int top_n, float cutoff_prob,
+                        const double* __restrict__ pairs, int32_t* __restrict__ labels,
+                        int32_t* __restrict__ lengths, BeamPool pool, BeamLm lmp) {
+  const int n_items = B * K;
+  for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+    const int u = it / K, k = it - u * K;
+    BeamLm L = lmp;
+    L.alpha = pairs[2 * k];
+    L.beta = pairs[2 * k + 1];
+    beam_search_item<true, true>(u, blockIdx.x, k * B + u, T, C, probs, out_len, blank, W, top_n, cutoff_prob,
+                                 labels, nullptr, lengths, nullptr, nullptr, pool, L);
+    __syncthreads();   // the next item's set-up overwrites the list this one's output read
+  }
 }
 
 size_t beam_workspace_bytes(int B, int T, int C, int beam_width, bool lm) {
@@ -616,11 +671,9 @@ size_t beam_workspace_bytes(int B, int T, int C, int beam_width, bool lm) {
          (lm ? align_up(n * 8, 256) : 0);
 }
 
-template <bool LM>
-int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
-                       int beam_width, int cutoff_top_n, float cutoff_prob, BeamLm lm, int32_t* labels,
-                       int32_t* timesteps, int32_t* lengths, double* scores, int32_t* n_beams, void* workspace,
-                       size_t workspace_bytes, void* stream) {
+// the checks every beam entry makes (DS2_REQUIRE returns from the caller's frame through this function's result)
+int beam_check_args(const char* fn, int B, int T, int C, int blank, int beam_width, int cutoff_top_n,
+                    float cutoff_prob) {
   DS2_REQUIRE(B > 0 && T > 0, "%s: bad shape B=%d T=%d", fn, B, T);
   DS2_REQUIRE(C >= 2 && C <= BEAM_MAX_C, "%s: C=%d outside [2, %d]", fn, C, BEAM_MAX_C);
   DS2_REQUIRE(blank >= 0 && blank < C, "%s: blank=%d outside [0, C=%d)", fn, blank, C);
@@ -629,14 +682,23 @@ int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, 
   DS2_REQUIRE(cutoff_top_n >= 1, "%s: cutoff_top_n=%d < 1", fn, cutoff_top_n);
   DS2_REQUIRE(cutoff_prob > 0.f && cutoff_prob <= 1.f, "%s: cutoff_prob=%g outside (0, 1]", fn, (double)cutoff_prob);
   DS2_REQUIRE((long long)T * beam_width < (1ll << 31) - 1, "%s: T*beam_width too large for the node pool", fn);
-  DS2_REQUIRE(probs && labels && timesteps && lengths && scores && n_beams, "%s: null pointer", fn);
-  const size_t need = beam_workspace_bytes(B, T, C, beam_width, LM);
-  DS2_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes,
-              need);
+  return DS2_OK;
+}
+
+int lm_check_args(const char* fn, int C, int blank, const void* lm, int lm_order, int space) {
+  DS2_REQUIRE(lm, "%s: null language model", fn);
+  DS2_REQUIRE(lm_order >= 1 && lm_order <= LM_MAX_ORDER, "%s: order=%d outside [1, %d]", fn, lm_order,
+              LM_MAX_ORDER);
+  DS2_REQUIRE(space >= 0 && space < C && space != blank && C <= BEAM_MAX_C,
+              "%s: space=%d outside [0, C=%d) or equal to blank=%d", fn, space, C, blank);
+  return DS2_OK;
+}
+
+// the pools of `slots` CTAs, carved from the arena in the order beam_workspace_bytes counts them
+BeamPool take_pool(Arena& ar, int slots, int T, int W, bool lm) {
   long long NP, HC;
-  pool_sizes(T, beam_width, &NP, &HC);
-  const size_t n = (size_t)B * NP, h = (size_t)B * HC;
-  Arena ar(workspace, workspace_bytes);
+  pool_sizes(T, W, &NP, &HC);
+  const size_t n = (size_t)slots * NP, h = (size_t)slots * HC;
   BeamPool pool;
   pool.parent = ar.take<int>(n);
   pool.label = ar.take<int>(n);
@@ -645,9 +707,25 @@ int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, 
   pool.best = ar.take<double>(n);
   pool.hkey = ar.take<unsigned long long>(h);
   pool.hval = ar.take<int>(h);
-  pool.lm = LM ? ar.take<double>(n) : nullptr;
+  pool.lm = lm ? ar.take<double>(n) : nullptr;
   pool.NP = NP;
   pool.HC = HC;
+  return pool;
+}
+
+template <bool LM>
+int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
+                       int beam_width, int cutoff_top_n, float cutoff_prob, BeamLm lm, int32_t* labels,
+                       int32_t* timesteps, int32_t* lengths, double* scores, int32_t* n_beams, void* workspace,
+                       size_t workspace_bytes, void* stream) {
+  const int rc = beam_check_args(fn, B, T, C, blank, beam_width, cutoff_top_n, cutoff_prob);
+  if (rc != DS2_OK) return rc;
+  DS2_REQUIRE(probs && labels && timesteps && lengths && scores && n_beams, "%s: null pointer", fn);
+  const size_t need = beam_workspace_bytes(B, T, C, beam_width, LM);
+  DS2_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes,
+              need);
+  Arena ar(workspace, workspace_bytes);
+  BeamPool pool = take_pool(ar, B, T, beam_width, LM);
   static DeviceOnce attr_once;
   if (attr_once.first()) {
     DS2_CHECK_CUDA(cudaFuncSetAttribute(beam_decode_kernel<LM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -659,6 +737,31 @@ int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, 
   DS2_LAUNCH(beam_decode_kernel<LM>, B, BEAM_THREADS, dyn_smem_bytes(beam_width, C, LM), st, T, C, probs, out_len,
              blank, beam_width, cutoff_top_n, cutoff_prob, labels, timesteps, lengths, scores, n_beams, pool, lm);
   return DS2_OK;
+}
+
+// CTAs of the grid kernel: as many as can be resident on the current device (occupancy x SMs), at most `items`;
+// 0 if the device cannot be queried
+long long grid_slots(long long items, int W, int C) {
+  static DeviceOnce attr_once;
+  if (attr_once.first()) {
+    if (cudaFuncSetAttribute(beam_decode_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)dyn_smem_bytes(BEAM_MAX_W, BEAM_MAX_C, true)) != cudaSuccess)
+      return 0;
+    attr_once.done();
+  }
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, beam_decode_grid_kernel, BEAM_THREADS,
+                                                    dyn_smem_bytes(W, C, true)) != cudaSuccess || per_sm < 1)
+    return 0;
+  const long long resident = (long long)per_sm * device_sm_count();
+  return resident < items ? resident : items;
+}
+
+size_t grid_workspace_bytes(int B, int T, int C, int W, int K) {
+  if (B <= 0 || T <= 0 || W <= 0 || C <= 0 || K <= 0) return 0;
+  const long long slots = grid_slots((long long)B * K, W, C);
+  if (slots <= 0) return 0;
+  return align_up((size_t)K * 2 * sizeof(double), 256) + beam_workspace_bytes((int)slots, T, C, W, true);
 }
 
 }  // namespace
@@ -687,11 +790,8 @@ int ds2_beam_decode_lm(int B, int T, int C, const float* probs, const int32_t* o
                        int cutoff_top_n, float cutoff_prob, const void* lm, int lm_order, double alpha, double beta,
                        int space, int32_t* labels, int32_t* timesteps, int32_t* lengths, double* scores,
                        int32_t* n_beams, void* workspace, size_t workspace_bytes, void* stream) {
-  DS2_REQUIRE(lm, "ds2_beam_decode_lm: null language model");
-  DS2_REQUIRE(lm_order >= 1 && lm_order <= LM_MAX_ORDER, "ds2_beam_decode_lm: order=%d outside [1, %d]", lm_order,
-              LM_MAX_ORDER);
-  DS2_REQUIRE(space >= 0 && space < C && space != blank && C <= BEAM_MAX_C,
-              "ds2_beam_decode_lm: space=%d outside [0, C=%d) or equal to blank=%d", space, C, blank);
+  const int rc = lm_check_args("ds2_beam_decode_lm", C, blank, lm, lm_order, space);
+  if (rc != DS2_OK) return rc;
   DS2_REQUIRE(std::isfinite(alpha) && std::isfinite(beta), "ds2_beam_decode_lm: alpha=%g, beta=%g not finite", alpha,
               beta);
   BeamLm L;
@@ -703,6 +803,48 @@ int ds2_beam_decode_lm(int B, int T, int C, const float* probs, const int32_t* o
   return beam_decode_launch<true>("ds2_beam_decode_lm", B, T, C, probs, out_len, blank, beam_width, cutoff_top_n,
                                   cutoff_prob, L, labels, timesteps, lengths, scores, n_beams, workspace,
                                   workspace_bytes, stream);
+}
+
+size_t ds2_beam_decode_lm_grid_workspace_bytes(int B, int T, int C, int beam_width, int K) {
+  return grid_workspace_bytes(B, T, C, beam_width, K);
+}
+
+int ds2_beam_decode_lm_grid(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
+                            int beam_width, int cutoff_top_n, float cutoff_prob, const void* lm, int lm_order, int K,
+                            const double* pairs, int space, int32_t* labels, int32_t* lengths, void* workspace,
+                            size_t workspace_bytes, void* stream) {
+  const char* fn = "ds2_beam_decode_lm_grid";
+  int rc = lm_check_args(fn, C, blank, lm, lm_order, space);
+  if (rc != DS2_OK) return rc;
+  rc = beam_check_args(fn, B, T, C, blank, beam_width, cutoff_top_n, cutoff_prob);
+  if (rc != DS2_OK) return rc;
+  DS2_REQUIRE(K >= 1, "%s: K=%d pairs, need at least 1", fn, K);
+  DS2_REQUIRE((long long)B * K < (1ll << 31) - 1, "%s: B*K too large", fn);
+  DS2_REQUIRE(probs && labels && lengths && pairs, "%s: null pointer", fn);
+  for (int k = 0; k < K; ++k)       // on the host: the kernel never sees a NaN or an infinity
+    DS2_REQUIRE(std::isfinite(pairs[2 * k]) && std::isfinite(pairs[2 * k + 1]),
+                "%s: pair %d: alpha=%g, beta=%g not finite", fn, k, pairs[2 * k], pairs[2 * k + 1]);
+  const long long slots = grid_slots((long long)B * K, beam_width, C);
+  DS2_REQUIRE(slots > 0, "%s: occupancy query failed", fn);
+  const size_t need = align_up((size_t)K * 2 * sizeof(double), 256) +
+                      beam_workspace_bytes((int)slots, T, C, beam_width, true);
+  DS2_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes,
+              need);
+  Arena ar(workspace, workspace_bytes);
+  double* pairs_d = ar.take<double>((size_t)K * 2);
+  BeamPool pool = take_pool(ar, (int)slots, T, beam_width, true);
+  BeamLm L;
+  L.tables = lm;
+  L.order = lm_order;
+  L.space = space;
+  L.alpha = 0.0;
+  L.beta = 0.0;
+  cudaStream_t st = as_stream(stream);
+  DS2_CHECK_CUDA(cudaMemcpyAsync(pairs_d, pairs, (size_t)K * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  DS2_PROF("beam_decode_lm_grid", st);
+  DS2_LAUNCH(beam_decode_grid_kernel, (int)slots, BEAM_THREADS, dyn_smem_bytes(beam_width, C, true), st, B, K, T, C,
+             probs, out_len, blank, beam_width, cutoff_top_n, cutoff_prob, pairs_d, labels, lengths, pool, L);
+  return DS2_OK;
 }
 
 }  // extern "C"

@@ -133,6 +133,68 @@ class BeamCTCDecoder:
                                              ptr(n_beams), ptr(ws), nws, stream), "ds2_beam_decode_lm")
         return labels.cpu(), scores.cpu(), timesteps.cpu(), lengths.cpu(), n_beams.cpu()
 
+    def decode_best(self, probs, sizes=None):
+        """beam 0 of `decode_beams` left on the device: probs (B,T,C) CUDA -> labels (B,T) int32, lengths (B) int32"""
+        if self.lm is not None:
+            labels, lengths = self.decode_best_grid(probs, sizes, [(self.alpha, self.beta)])
+            return labels[0], lengths[0]
+        import ctypes as C
+        probs = probs.to(torch.float32).contiguous()
+        B, T, Cn = probs.shape
+        dev, W = probs.device, self.beam_width
+        lib = get_lib()
+        with torch.cuda.device(dev):
+            Wa = max(W, 1)
+            nws = lib.ds2_beam_decode_workspace_bytes(B, T, Cn, W)
+            ws = torch.empty(max(nws, 1), dtype=torch.uint8, device=dev)
+            labels = torch.empty(B, Wa, T, dtype=torch.int32, device=dev)
+            timesteps = torch.empty_like(labels)
+            lengths = torch.empty(B, Wa, dtype=torch.int32, device=dev)
+            scores = torch.empty(B, Wa, dtype=torch.float64, device=dev)
+            n_beams = torch.empty(B, dtype=torch.int32, device=dev)
+            sz = None if sizes is None else torch.as_tensor(sizes).to(device=dev, dtype=torch.int32).contiguous()
+            check(lib.ds2_beam_decode(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
+                                      self.cutoff_prob, ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores),
+                                      ptr(n_beams), ptr(ws), nws, C.c_void_p(torch.cuda.current_stream().cuda_stream)),
+                  "ds2_beam_decode")
+        return labels[:, 0].contiguous(), lengths[:, 0].contiguous()
+
+    def decode_best_grid(self, probs, sizes, pairs):
+        """`ds2_beam_decode_lm_grid`: the best beam for each of K (alpha, beta) pairs in one launch.  probs (B,T,C)
+        CUDA, sizes (B) or None, pairs K x (alpha, beta) -> labels (K,B,T) int32, lengths (K,B) int32 on the device;
+        (k, b) is beam 0 of `decode_beams` after `reset_params(*pairs[k])`.  Pass the utterances longest first: the
+        items start in utterance order."""
+        import ctypes as C
+        import numpy as np
+        if self.lm is None:
+            raise _lib.Ds2Error("BeamCTCDecoder.decode_best_grid: needs a language model (lm_path)")
+        pr = np.ascontiguousarray(np.asarray(pairs, dtype=np.float64).reshape(-1, 2))
+        if pr.shape[0] < 1:
+            raise _lib.Ds2Error("BeamCTCDecoder.decode_best_grid: K = 0 (alpha, beta) pairs")
+        if not np.all(np.isfinite(pr)):
+            raise _lib.Ds2Error(f"BeamCTCDecoder.decode_best_grid: alpha and beta must be finite, got "
+                                f"{pr[~np.all(np.isfinite(pr), axis=1)].tolist()}")
+        if not probs.is_cuda:
+            raise _lib.Ds2Error("BeamCTCDecoder.decode_best_grid: probs must be a CUDA tensor")
+        probs = probs.to(torch.float32).contiguous()
+        B, T, Cn = probs.shape
+        K, dev, W = pr.shape[0], probs.device, self.beam_width
+        lib = get_lib()
+        with torch.cuda.device(dev):
+            lm = self.lm.device_tables(dev)
+            nws = lib.ds2_beam_decode_lm_grid_workspace_bytes(B, T, Cn, W, K)
+            ws = torch.empty(max(nws, 1), dtype=torch.uint8, device=dev)
+            labels = torch.empty(K, B, T, dtype=torch.int32, device=dev)
+            lengths = torch.empty(K, B, dtype=torch.int32, device=dev)
+            sz = None if sizes is None else torch.as_tensor(sizes).to(device=dev, dtype=torch.int32).contiguous()
+            check(lib.ds2_beam_decode_lm_grid(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
+                                              self.cutoff_prob, ptr(lm), self.lm.order, K,
+                                              pr.ctypes.data_as(C.c_void_p), self.lm.space, ptr(labels),
+                                              ptr(lengths), ptr(ws), nws,
+                                              C.c_void_p(torch.cuda.current_stream().cuda_stream)),
+                  "ds2_beam_decode_lm_grid")
+        return labels, lengths
+
     def convert_to_strings(self, out, seq_len):
         """decoder.py:79-91: [[str]] over utterances and beams, '' where the length is 0"""
         results = []

@@ -233,6 +233,42 @@ int ds2_beam_decode_lm(int B, int T, int C, const float* probs, const int32_t* o
                        double* scores, int32_t* n_beams,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- many (alpha, beta) pairs per launch (row N6), for search_lm_params.py:100-118, which reruns
+ * validation.py:run_evaluation with ds2_beam_decode_lm once per pair: the arguments of ds2_beam_decode_lm with K >= 1
+ * pairs instead of one.
+ *   pairs (K,2) fp64 (alpha_k, beta_k) on the HOST, each finite (checked here, then copied into the workspace)
+ *   labels (K,B,T) int32: the best beam of (pair k, utterance b), zero after its length; lengths (K,B) int32.
+ *   Each (k, b) is bit-identical to beam 0 of ds2_beam_decode_lm with (alpha_k, beta_k).
+ *   Items are (utterance, pair), utterance-major: pass the utterances sorted by length, longest first, so the
+ *   longest items start first.  One launch of as many CTAs as can be resident on the current device (occupancy x
+ *   SMs, at most B*K); each CTA runs its items one after another in its own node pool and hash.
+ *   Workspace: the pairs plus ds2_beam_decode_lm's workspace for that many CTAs (not for B*K utterances); it
+ *   depends on the current device.  Deterministic; one launch (after a K x 16 B host-to-device copy).           */
+size_t ds2_beam_decode_lm_grid_workspace_bytes(int B, int T, int C, int beam_width, int K);
+int ds2_beam_decode_lm_grid(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
+                            int beam_width, int cutoff_top_n, float cutoff_prob,
+                            const void* lm, int lm_order, int K, const double* pairs, int space,
+                            int32_t* labels, int32_t* lengths,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- WER / CER edit counts (validation.py:48-126, the Lev.distance calls of WordErrorRate / CharErrorRate) ----
+ * Rows are hypotheses: labels (R,T) int32 with lengths (R) int32 (clamped to [0, T]), R = K x B, row k*B + b
+ * scored against reference b.  References: targets flat int64 (n_targets) with target_sizes (B) int32, all on the
+ * device, as the collate produces them; max_target_size >= every target size.  Blank labels are dropped from the
+ * references (GreedyDecoder.convert_to_strings); a word is a maximal run of labels other than `space` (pass
+ * space = C when the labels have no space).  Per row:
+ *   [0] char_edits  Levenshtein distance with the spaces removed from both sides   [1] ref_chars  (non-space)
+ *   [2] word_edits  Levenshtein distance between the word sequences                [3] ref_words
+ * row_counts (R,4) int64 is written when non-NULL; pair_counts (K,4) int64, when non-NULL, is ADDED to (the
+ * caller zeroes it once; batches accumulate).  Bit-parallel (Myers / Hyyroe) in 64-bit words, one warp per row;
+ * no length limit.  Deterministic (integer sums).  Workspace: ds2_error_counts_workspace_bytes.  A reference
+ * longer than max_target_size is not scored: its rows get -1 in row_counts and add nothing to pair_counts.       */
+size_t ds2_error_counts_workspace_bytes(int K, int B, int64_t n_targets, int max_target_size);
+int ds2_error_counts(int K, int B, int T, const int32_t* labels, const int32_t* lengths, const int64_t* targets,
+                     int64_t n_targets, const int32_t* target_sizes, int max_target_size, int blank, int space,
+                     int64_t* row_counts, int64_t* pair_counts, void* workspace, size_t workspace_bytes,
+                     void* stream);
+
 /* ---- optimizer on flat fp32 buffers (row N1): clip_grad_norm_(max_norm) + AdamW / SGD-Nesterov,
  * model.py:273-297, configs/librispeech.yaml:12.  grad_scale multiplies g first (1/world for DDP
  * mean).  norm_ws: >= ds2_optim_workspace_bytes(); grad_norm_out (1 float, device) gets the
