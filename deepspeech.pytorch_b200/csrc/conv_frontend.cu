@@ -531,7 +531,7 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
   DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D1 * Tp, W.sums, g1, be1, rm1, rv1, training, momentum,
              eps, stats);
   DS2_LAUNCH(bn_act_kernel, 132 * 8, 256, 0, st, B, D1, Tp, z1, stats, g1, be1, out_len, a1);
-  if (tensor_core_mode() && !getenv("DS2_NO_CONV_TC") && !getenv("DS2_NO_CONV_TC_FWD")) {
+  if (tensor_core_mode()) {
     // conv2 on wgmma: channels-last copy of a1, packed taps, implicit GEMM with the kw taps folded into N
     rc = nchw_to_cl(B, D1, Tp, a1, W.cl, st);
     if (rc) return rc;
@@ -586,7 +586,7 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
   bool forked = false;
   {
     int wrc = 1;
-    if (tensor_core_mode() && !getenv("DS2_NO_CONV_TC") && !getenv("DS2_NO_CONV_TC_WGRAD")) {
+    if (tensor_core_mode()) {
       cudaStream_t wst = st;
       if (side && Tp % 4 == 0) {
         int frc = side_fork(st, side);
@@ -608,7 +608,7 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
   // even rows y=2j (41 rows), odd rows y=2j+1 (40 rows) of d(a1) (B,32,81,T')
   const size_t ob = (size_t)CO * D1 * Tp, oc = (size_t)D1 * Tp;
   int rc;
-  if (tensor_core_mode() && !getenv("DS2_NO_CONV_TC") && !getenv("DS2_NO_CONV_TC_DGRAD")) {
+  if (tensor_core_mode()) {
     // data gradient on wgmma: rows y=2i use taps kh=2m (d = i+5-m), rows y=2i+1 taps kh=2m+1
     rc = nchw_to_cl(B, D2, Tp, W.du2, W.cl, st);
     if (rc) return rc;
@@ -642,7 +642,7 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
   {
     // conv1 weight gradient on wgmma (reuses the conv2 weight gradient's staging buffer, which is free by now)
     int wrc = 1;
-    if (tensor_core_mode() && !getenv("DS2_NO_CONV_TC") && !getenv("DS2_NO_CONV1_TC_WGRAD")) {
+    if (tensor_core_mode()) {
       wrc = conv1_wgrad_tc(W.da1, x, W.shifted, W.wg_part, B, T, Tp, dw1, st);
       if (wrc < 0) return wrc;
     }

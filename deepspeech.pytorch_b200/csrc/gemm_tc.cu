@@ -9,7 +9,6 @@
 // Operands that are not K-major in memory (transA / !transB) are first transposed into the workspace.
 // Shapes the kernel does not take (tiny or unaligned) return 1 and the caller uses the FFMA GEMM.
 #include <stdio.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -23,8 +22,8 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 static EncodeTiledFn g_encode = nullptr;
 // TFLOAT32 makes the TMA unit round fp32 -> tf32 (nearest) while copying into shared memory: measured
 // bit-identical error statistics to cuBLAS TF32; plain FLOAT32 would let the MMA truncate (2.6x the
-// rms error and a -7e-4 relative bias on same-sign data).  DS2_TMAP_TF32=0 selects truncation.
-static CUtensorMapDataType g_tmap_dtype = CU_TENSOR_MAP_DATA_TYPE_TFLOAT32;
+// rms error and a -7e-4 relative bias on same-sign data).
+static constexpr CUtensorMapDataType g_tmap_dtype = CU_TENSOR_MAP_DATA_TYPE_TFLOAT32;
 
 static int load_encode() {
   if (g_encode) return DS2_OK;
@@ -35,8 +34,6 @@ static int load_encode() {
     set_error("cuTensorMapEncodeTiled not available from the driver");
     return DS2_ERR_CUDA;
   }
-  const char* e = getenv("DS2_TMAP_TF32");
-  if (e && e[0] == '0') g_tmap_dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   return DS2_OK;
 }
@@ -165,8 +162,6 @@ struct Cfg {
 static_assert(Cfg<256>::SMEM_BYTES <= 227 * 1024 && Cfg<128>::SMEM_BYTES <= 227 * 1024, "shared memory");
 }  // namespace gtc
 
-// gridDim.z > 1: split-K, every CTA adds its partial tile into C with vector atomics (C holds beta * C_old,
-// prepared by the host).
 // F16 (precision-16 mode): fp16 operands, the same 128-byte rows hold 64 halfs, wgmma k16 instead of tf32 k8;
 // accumulation and C stay fp32.  `alpha_dev` (optional) multiplies alpha by a device-resident factor (the inverse of
 // the power-of-two scale of a scaled fp16 operand).
@@ -188,9 +183,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint64_t* empty = full + STAGES;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
-  const int nk_all = (K + BK - 1) / BK, per = (nk_all + (int)gridDim.z - 1) / (int)gridDim.z;
-  const int kb0 = (int)blockIdx.z * per, kb1 = min(nk_all, kb0 + per), nk = max(0, kb1 - kb0);
-  const bool split = gridDim.z > 1;
+  const int nk = (K + BK - 1) / BK;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
@@ -205,13 +198,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     setmaxnreg_dec<PRODUCER_REGS>();
     if (warp == 0 && lane == 0) {
       for (int it = 0; it < nk; ++it) {
-        const int kb = kb0 + it, s = it % STAGES;
+        const int s = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         mbar_wait(&empty[s], ph ^ 1);
         mbar_arrive_expect_tx(&full[s], STAGE_BYTES);
         uint8_t* sa = smem + s * STAGE_BYTES;
-        tma_load_2d(sa, &tmA, &full[s], kb * BK, m0);
-        tma_load_2d(sa + A_BYTES, &tmB, &full[s], kb * BK, n0);
+        tma_load_2d(sa, &tmA, &full[s], it * BK, m0);
+        tma_load_2d(sa + A_BYTES, &tmB, &full[s], it * BK, n0);
       }
     }
   } else {
@@ -236,44 +229,34 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if (it > 0 && leader) mbar_arrive(&empty[(it - 1) % STAGES]);
     }
     wg_wait<0>();
-    if (nk > 0 && leader) mbar_arrive(&empty[(nk - 1) % STAGES]);
-    if (nk > 0) {
-      // fragment: rows 16 w + l/4 (+8), column pairs 8 i + 2 (l%4)
-      const int w = warp % 4;
-      const bool vec_ok = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(C) & 7) == 0);
+    if (leader) mbar_arrive(&empty[(nk - 1) % STAGES]);
+    // fragment: rows 16 w + l/4 (+8), column pairs 8 i + 2 (l%4)
+    const int w = warp % 4;
+    const bool vec_ok = ((ldc & 1) == 0) && ((reinterpret_cast<uintptr_t>(C) & 7) == 0);
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int row = m0 + 64 * wg + 16 * w + (lane >> 2) + 8 * hh;
-        if (row >= M) continue;
-        float* crow = C + (size_t)row * ldc;
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = m0 + 64 * wg + 16 * w + (lane >> 2) + 8 * hh;
+      if (row >= M) continue;
+      float* crow = C + (size_t)row * ldc;
 #pragma unroll
-        for (int i = 0; i < BN / 8; ++i) {
-          const int col = n0 + 8 * i + 2 * (lane & 3);
-          float2 o = make_float2(alpha * acc[4 * i + 2 * hh], alpha * acc[4 * i + 2 * hh + 1]);
-          if (vec_ok && col + 1 < N) {
-            float2* cp2 = reinterpret_cast<float2*>(crow + col);
-            if (split) {
-              atomicAdd(cp2, o);
-            } else {
-              if (beta != 0.f) {
-                const float2 old = *cp2;
-                o.x = fmaf(beta, old.x, o.x);
-                o.y = fmaf(beta, old.y, o.y);
-              }
-              *cp2 = o;
-            }
-          } else {
+      for (int i = 0; i < BN / 8; ++i) {
+        const int col = n0 + 8 * i + 2 * (lane & 3);
+        float2 o = make_float2(alpha * acc[4 * i + 2 * hh], alpha * acc[4 * i + 2 * hh + 1]);
+        if (vec_ok && col + 1 < N) {
+          float2* cp2 = reinterpret_cast<float2*>(crow + col);
+          if (beta != 0.f) {
+            const float2 old = *cp2;
+            o.x = fmaf(beta, old.x, o.x);
+            o.y = fmaf(beta, old.y, o.y);
+          }
+          *cp2 = o;
+        } else {
 #pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              if (col + j >= N) break;
-              float v = j ? o.y : o.x;
-              if (split) {
-                atomicAdd(crow + col + j, v);
-              } else {
-                if (beta != 0.f) v = fmaf(beta, crow[col + j], v);
-                crow[col + j] = v;
-              }
-            }
+          for (int j = 0; j < 2; ++j) {
+            if (col + j >= N) break;
+            float v = j ? o.y : o.x;
+            if (beta != 0.f) v = fmaf(beta, crow[col + j], v);
+            crow[col + j] = v;
           }
         }
       }
@@ -313,21 +296,12 @@ size_t gemm_tc_workspace_bytes(int transA, int transB, int M, int N, int K) {
 
 static bool tc_eligible(int M, int N, int K) { return K >= 32 && M >= 32 && N >= 16 && (long long)M * N * K >= (1 << 18); }
 
-// K-way split (DS2_GEMM_CFG / DS2_GEMM16_CFG = 2, 3: 2 or 4 parts, added into C with float atomics).  Never chosen
-// by itself: the order of the atomic adds varies from run to run, and the training step must be bit-repeatable.
-static int choose_splits(const char* env, float beta) {
-  const char* e = getenv(env);
-  const int forced = e ? atoi(e) : 0;
-  if (forced >= 2 && forced <= 3 && (beta == 0.f || beta == 1.f)) return 1 << (forced - 1);
-  return 1;
-}
-
 // columns of the output tile: 256 wherever N needs more than one 128-column tile
 static int tile_n(int N) { return N > 128 ? 256 : 128; }
 
 template <bool F16, int BN>
 static int launch_gemm_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, float alpha, float beta,
-                          float* C, int ldc, int splits, cudaStream_t st, const float* alpha_dev) {
+                          float* C, int ldc, cudaStream_t st, const float* alpha_dev) {
   auto kern = gemm_tc_kernel<F16, BN>;
   constexpr int smem = gtc::Cfg<BN>::SMEM_BYTES;
   static DeviceOnce attr_once;
@@ -335,18 +309,16 @@ static int launch_gemm_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, int M,
     DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_once.done();
   }
-  if (splits > 1 && beta == 0.f)
-    DS2_CHECK_CUDA(cudaMemset2DAsync(C, (size_t)ldc * sizeof(float), 0, (size_t)N * sizeof(float), (size_t)M, st));
-  dim3 grid(cdiv(N, BN), cdiv(M, gtc::BM), splits);
+  dim3 grid(cdiv(N, BN), cdiv(M, gtc::BM));
   DS2_LAUNCH(kern, grid, gtc::THREADS, smem, st, tmA, tmB, M, N, K, alpha, beta, C, ldc, alpha_dev);
   return DS2_OK;
 }
 
 template <bool F16>
 static int launch_gemm_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, int M, int N, int K, float alpha, float beta,
-                          float* C, int ldc, int splits, cudaStream_t st, const float* alpha_dev = nullptr) {
-  if (tile_n(N) == 256) return launch_gemm_tc<F16, 256>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st, alpha_dev);
-  return launch_gemm_tc<F16, 128>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st, alpha_dev);
+                          float* C, int ldc, cudaStream_t st, const float* alpha_dev = nullptr) {
+  if (tile_n(N) == 256) return launch_gemm_tc<F16, 256>(tmA, tmB, M, N, K, alpha, beta, C, ldc, st, alpha_dev);
+  return launch_gemm_tc<F16, 128>(tmA, tmB, M, N, K, alpha, beta, C, ldc, st, alpha_dev);
 }
 
 // TF32 wgmma reads both operands K-major: an operand stored the other way round (transA / !transB) is first
@@ -377,13 +349,12 @@ int gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const floa
   }
   if ((ldak & 3) || (ldbk & 3) || (reinterpret_cast<uintptr_t>(Ak) & 15) || (reinterpret_cast<uintptr_t>(Bk) & 15))
     return 1;
-  const int splits = choose_splits("DS2_GEMM_CFG", beta);
   CUtensorMap tmA, tmB;
   int rc = make_tmap_2d(&tmA, Ak, M, K, ldak, gtc::BM, gtc::BK);
   if (rc) return rc;
   rc = make_tmap_2d(&tmB, Bk, N, K, ldbk, tile_n(N), gtc::BK);
   if (rc) return rc;
-  return launch_gemm_tc<false>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st);
+  return launch_gemm_tc<false>(tmA, tmB, M, N, K, alpha, beta, C, ldc, st);
 }
 
 // C[M,N] (fp32) = alpha * [*alpha_dev] * A[M,K] . B[N,K]^T + beta * C with fp16 K-major operands (precision-16 mode).
@@ -392,13 +363,12 @@ int gemm_tc_f16(int M, int N, int K, float alpha, const void* A16, int lda, cons
                 float* C, int ldc, const float* alpha_dev, cudaStream_t st) {
   if (!tc_eligible(M, N, K) || M < 128) return 1;
   if ((lda & 7) || (ldb & 7) || (reinterpret_cast<uintptr_t>(A16) & 15) || (reinterpret_cast<uintptr_t>(B16) & 15)) return 1;
-  const int splits = choose_splits("DS2_GEMM16_CFG", beta);
   CUtensorMap tmA, tmB;
   int rc = make_tmap_f16(&tmA, A16, 2, K, M, 1, (size_t)lda, 0, 64, gtc::BM, 1);
   if (rc) return rc;
   rc = make_tmap_f16(&tmB, B16, 2, K, N, 1, (size_t)ldb, 0, 64, tile_n(N), 1);
   if (rc) return rc;
-  return launch_gemm_tc<true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, splits, st, alpha_dev);
+  return launch_gemm_tc<true>(tmA, tmB, M, N, K, alpha, beta, C, ldc, st, alpha_dev);
 }
 
 }  // namespace ds2

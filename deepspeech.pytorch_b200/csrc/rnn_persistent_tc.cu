@@ -20,7 +20,6 @@
 // K = G*H; the partial sums travel through distributed shared memory or, with XG, through L2).
 #include <cooperative_groups.h>
 #include <cuda_fp16.h>
-#include <dlfcn.h>
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -517,26 +516,9 @@ static bool vec_ok(const void* a, const void* b = nullptr, const void* c = nullp
   return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c) |
            reinterpret_cast<uintptr_t>(d)) & 15) == 0;
 }
-// Nsight Compute cannot replay a cooperative launch of a kernel with a cluster dimension (it aborts the target).
-// Under the profiler's injection — or with DS2_SPLITK_NONCOOP=1 — the cluster sweeps are launched without the
-// cooperative attribute; co-residency is still verified with cudaOccupancyMaxActiveClusters, and a lone kernel of
-// <= 148 one-per-SM CTAs on an otherwise idle stream becomes resident as a whole either way.
-static bool noncoop_cluster_launch() {
-  const char* e = getenv("DS2_SPLITK_NONCOOP");
-  if (e) return atoi(e) != 0;
-  static const bool under_ncu = [] {
-    if (getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR") || getenv("NV_NSIGHT_INJECTION_TRANSPORT_TYPE") ||
-        getenv("NV_TPS_LAUNCH_TOKEN"))
-      return true;
-    const char* inj = getenv("CUDA_INJECTION64_PATH");
-    if (inj && (strstr(inj, "nsight-compute") || strstr(inj, "cuda-injection"))) return true;
-    void* h = dlopen("libcuda-injection.so", RTLD_NOLOAD | RTLD_LAZY);   // already mapped by the profiler?
-    if (h) { dlclose(h); return true; }
-    return false;
-  }();
-  return under_ncu;
-}
 
+// The switches that force a variant the library picks by itself for other shapes (DESIGN §6.1): unset gives `dflt`,
+// a value its integer, so that `=0` turns a switch off.
 static int env_flag(const char* name, int dflt) {
   const char* e = getenv(name);
   return e ? atoi(e) : dflt;
@@ -575,8 +557,7 @@ static int opt_in_smem(DeviceOnce& once, std::initializer_list<SweepKernel> kern
 }
 
 // Launch configuration of a sweep for cudaLaunchKernelEx: cooperative (the grid barrier needs every CTA resident),
-// in clusters of `cluster` CTAs when cluster > 1.  Cluster launches drop the cooperative attribute under
-// noncoop_cluster_launch().
+// in clusters of `cluster` CTAs when cluster > 1.
 struct SweepConfig {
   cudaLaunchAttribute attrs[2];
   cudaLaunchConfig_t cfg{};
@@ -590,7 +571,7 @@ struct SweepConfig {
     attrs[1].id = cudaLaunchAttributeCooperative;
     attrs[1].val.cooperative = 1;
     cfg.attrs = cluster > 1 ? attrs : attrs + 1;
-    cfg.numAttrs = cluster > 1 && !noncoop_cluster_launch() ? 2 : 1;
+    cfg.numAttrs = cluster > 1 ? 2 : 1;
   }
   SweepConfig(const SweepConfig&) = delete;   // cfg.attrs points into the object
 };
@@ -766,7 +747,7 @@ template <int RNN>
 static int launch_fwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
   using namespace rp;
   const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
-  if (!getenv("DS2_NO_RESIDENT")) {
+  if (!env_flag("DS2_NO_RESIDENT", 0)) {
     if (RNN != DS2_RNN_TANH && env_flag("DS2_FWD_SPLITK", 1)) {   // 2-CTA clusters, half the MMA chain per step
       constexpr int R = RNN == DS2_RNN_TANH ? DS2_RNN_LSTM : RNN;
       int rc = launch_fwd_splitk<R>(a, ws, ws_bytes, st);
@@ -2210,7 +2191,7 @@ static int launch_bwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaSt
   using namespace rp;
   const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
   const int GH = G * a.H;
-  if (!getenv("DS2_NO_RESIDENT")) {
+  if (!env_flag("DS2_NO_RESIDENT", 0)) {
     int rc = launch_bwd_splitk_resident<RNN, CL>(a, ws, ws_bytes, st);
     if (rc != 1) return rc;
   }
@@ -2280,7 +2261,7 @@ int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaS
   if (a.H % 32 != 0 || a.B > 256 || a.T < 2) return 1;
   {
     int rc = 1;
-    if (!getenv("DS2_NO_SPLITK")) {
+    if (!env_flag("DS2_NO_SPLITK", 0)) {
       // 8-CTA clusters (128 units, K/8 per CTA) halve the MMA chain of a step; 4-CTA clusters take the shapes
       // they do not (H % 128, K/8 not a multiple of 64, or 8-CTA clusters that do not fit the GPCs)
       if (env_flag("DS2_SPLITK_CL", 8) == 8) {

@@ -324,11 +324,9 @@ def test_tf32_sweep_variants_agree_with_the_fp32_path(rnn, B, monkeypatch):
             assert rel_l2(a, b) < 1e-2, env
 
 
-@pytest.mark.parametrize("cfg", ["1", "2", "3"])
-def test_gemm_tile_configurations_vs_fp64(cfg, monkeypatch):
-    """128x128 tiles with K in one pass, in 2 and in 4 split-K parts; operands stored K-major and transposed (the
-    latter go through a transpose into the workspace); TF32 error level."""
-    monkeypatch.setenv("DS2_GEMM_CFG", cfg)
+def test_gemm_tile_configurations_vs_fp64():
+    """128- and 256-column tiles; operands stored K-major and transposed (the latter go through a transpose into the
+    workspace); TF32 error level."""
     ds.set_precision("tf32")
     g = torch.Generator(device="cuda").manual_seed(3)
     for tA, tB, M, N, K in [(0, 1, 600, 520, 300), (1, 0, 512, 320, 2000), (0, 0, 640, 1312, 512),
@@ -337,13 +335,12 @@ def test_gemm_tile_configurations_vs_fp64(cfg, monkeypatch):
         b = torch.randn((N, K) if tB else (K, N), generator=g, device="cuda")
         ref = (a.t() if tA else a).double() @ (b.t() if tB else b).double()
         c = ds.ops.gemm(a, b, bool(tA), bool(tB))
-        assert rel_l2(c, ref) < 1e-3, (cfg, tA, tB, M, N, K)
+        assert rel_l2(c, ref) < 1e-3, (tA, tB, M, N, K)
 
 
-def test_gemm_split_k_accumulates_into_c(monkeypatch):
-    """weight-gradient shape class: 2-way split-K with vector atomics (opt-in: never chosen by the library itself, whose
-    training step is bit-repeatable), beta = 0 and beta = 1"""
-    monkeypatch.setenv("DS2_GEMM_CFG", "2")
+def test_gemm_weight_gradient_shape_accumulates_into_c():
+    """weight-gradient shape class (both operands transposed into the workspace): beta = 0, and alpha = 0.5 with
+    beta = 1 adding into C"""
     ds.set_precision("tf32")
     g = torch.Generator(device="cuda").manual_seed(5)
     M, N, K = 4096, 1024, 2304
@@ -432,12 +429,10 @@ def test_deferred_weight_gradient_gemms_give_the_same_gradients():
     assert rel(out[True][0], out[True][1]) > 1e-2
 
 
-@pytest.mark.parametrize("cfg", ["1", "2", "3"])
-def test_gemm_f16_tile_configurations_vs_fp64(cfg, monkeypatch):
-    """the precision-16 mode's GEMM (fp16 K-major operands, fp32 accumulation) with K in one pass, in 2 and in 4
-    split-K parts, a K tail (K % 64 != 0) and alpha / beta"""
+def test_gemm_f16_tile_configurations_vs_fp64():
+    """the precision-16 mode's GEMM (fp16 K-major operands, fp32 accumulation): 128- and 256-column tiles, a K tail
+    (K % 64 != 0) and alpha / beta"""
     import ctypes as C
-    monkeypatch.setenv("DS2_GEMM16_CFG", cfg)
     lib = ds.get_lib()
     g = torch.Generator(device="cuda").manual_seed(7)
     for M, N, K, alpha, beta in [(640, 520, 1000, 1.0, 0.0), (4096, 1024, 4104, 0.5, 1.0), (300, 96, 72, 1.0, 0.0)]:
@@ -449,7 +444,7 @@ def test_gemm_f16_tile_configurations_vs_fp64(cfg, monkeypatch):
                               C.c_void_p(out.data_ptr()), N, C.c_void_p(torch.cuda.current_stream().cuda_stream))
         assert rc == 0, lib.ds2_last_error()
         ref = alpha * (a.double() @ b.double().t()) + beta * c0.double()
-        assert rel_l2(out, ref) < 1e-5, (cfg, M, N, K)
+        assert rel_l2(out, ref) < 1e-5, (M, N, K)
 
 
 @pytest.mark.parametrize("T,B", [(301, 5), (1000, 3), (301, 4), (640, 6)])
