@@ -526,19 +526,25 @@ static int env_flag(const char* name, int dflt) {
 // DS2_SWEEP_DEFER=0: store everything before the barrier arrival (see PersistParams::defer)
 static int sweep_defer_default() { return env_flag("DS2_SWEEP_DEFER", 1); }
 
-// The fields every sweep fills the same way.  `units`: hidden units per CTA, or per cluster (group of CTAs) of the
-// split-K variants.  The 4 KB control block at the start of the workspace holds err (offset 0) and the per-direction
-// step counters (offset 128).
+// The 4 KB control block at the start of every sweep workspace, zeroed before each sweep: err (offset 0), the
+// per-direction step counters and the per-CTA tile counters xcnt of the 4-CTA L2 exchange (at most XCNT_MAX CTAs).
+constexpr size_t CTL_BAR = 128, CTL_XCNT = 1024, CTL_BYTES = 4096;
+constexpr int XCNT_MAX = (int)(CTL_BYTES - CTL_XCNT) / 4;
+
+static int sweep_nb(int B) { return (B + 31) / 32 * 32; }   // batch columns of the MMAs
+
+// The fields every sweep fills the same way.  `units`: hidden units per CTA, or per group of CTAs of the split-K
+// variants.
 static PersistParams sweep_params(const SeqArgs& a, int units, const char* trace_env, void* ws) {
   PersistParams p{};
-  p.T = a.T; p.B = a.B; p.NB = (a.B + 31) / 32 * 32; p.H = a.H; p.D = a.D; p.NT = a.H / units; p.G = a.G;
+  p.T = a.T; p.B = a.B; p.NB = sweep_nb(a.B); p.H = a.H; p.D = a.D; p.NT = a.H / units; p.G = a.G;
   p.training = a.training;
   p.len = a.len; p.gates = a.gates; p.hseq = a.hseq; p.aux = a.aux; p.dy = a.dy; p.h0 = a.h0; p.c0 = a.c0;
   for (int d = 0; d < a.D; ++d) { p.b_ih[d] = a.b_ih[d]; p.b_hh[d] = a.b_hh[d]; }
   p.trace = trace_ptr_from_env(trace_env);
   p.defer = sweep_defer_default();
   p.err = static_cast<int*>(ws);
-  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + 128);
+  p.bar = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + CTL_BAR);
   return p;
 }
 
@@ -576,90 +582,11 @@ struct SweepConfig {
   SweepConfig(const SweepConfig&) = delete;   // cfg.attrs points into the object
 };
 
-// CTAs of `kern` that can be co-resident as plain CTAs (one per SM at most, see one_cta_per_sm)
-static int coop_fit(SweepKernel kern, size_t smem, int* fit) {
-  int per_sm = 0;
-  DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, rp::THREADS, smem));
-  *fit = per_sm * device_sm_count();
-  return DS2_OK;
-}
-
-// CTAs of `kern` that can be co-resident in whole clusters of `cluster` CTAs (a cluster cannot span two GPCs), or -1
-// when the device rejects the configuration
-static int cluster_fit(SweepKernel kern, int cluster, int grid, size_t smem, cudaStream_t st) {
-  SweepConfig c(cluster, grid, smem, st);
-  int max_clusters = 0;
-  if (cudaOccupancyMaxActiveClusters(&max_clusters, kern, &c.cfg) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return -1;
-  }
-  return max_clusters * cluster;
-}
-
-// The launch policy of every sweep.  `fit` CTAs can be co-resident, and the grid barrier needs every CTA of a launch
-// resident: both directions (p.D * per_dir CTAs) go in one launch when they fit; otherwise, if `per_dir_ok`, one
-// launch per direction; otherwise the shape is declined (return 1).  Then `prepare()` (operand copies, tensor maps),
-// the zeroed control block (its first `ctl_bytes` bytes of workspace), the launches and sweep_check_kernel.
-// cluster == 0: cudaLaunchCooperativeKernel, and a refused launch is an error.  cluster >= 1: cudaLaunchKernelEx in
-// clusters of that size (1: no cluster dimension); a refused first launch declines, with a warning on stderr
-// unless `fallback` is null, and a refused second launch is an error.
-template <typename Prepare>
-static int launch_sweep(SweepKernel kern, int cluster, int per_dir, size_t smem, int fit, bool per_dir_ok,
-                        size_t ctl_bytes, const char* what, const char* fallback, PersistParams& p, cudaStream_t st,
-                        Prepare&& prepare) {
-  int grid = p.D * per_dir, launches = 1;
-  if (fit < grid) {
-    if (!per_dir_ok || fit < per_dir) return 1;
-    grid = per_dir;
-    launches = p.D;
-  }
-  if (int rc = prepare()) return rc;
-  DS2_CHECK_CUDA(cudaMemsetAsync(p.err, 0, ctl_bytes, st));
-  SweepConfig c(cluster, grid, smem, st);
-  for (int li = 0; li < launches; ++li) {
-    p.d0 = li;
-    if (cluster == 0) {
-      void* args[] = {&p};
-      DS2_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)kern, dim3(grid), dim3(rp::THREADS), args, smem, st));
-    } else {
-      const cudaError_t le = cudaLaunchKernelEx(&c.cfg, kern, p);
-      if (le != cudaSuccess) {
-        (void)cudaGetLastError();
-        if (li == 0) {
-          if (fallback)
-            fprintf(stderr, "ds2_b200: WARNING %s launch failed (%s); using %s\n", what, cudaGetErrorString(le), fallback);
-          return 1;
-        }
-        set_error("%s: second launch failed: %s", what, cudaGetErrorString(le));
-        return DS2_ERR_CUDA;
-      }
-    }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-  }
-  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
-  return DS2_OK;
-}
-
 static size_t fwd_smem_bytes(int NB) {
   using namespace rp;
   size_t NBp = NB + 1;
   return 1024 + (size_t)STAGES * (A_BYTES + (size_t)NB * 128) + (5 * UT * NBp + NB + 4) * sizeof(float) +
          (2 * STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
-}
-
-static size_t splitk_res_ws_bytes(int G, int T, int B, int H, int D);
-static size_t res_ws_bytes(int G, int T, int B, int H, int D);
-
-size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
-  const int G = rnn == DS2_RNN_LSTM ? 4 : (rnn == DS2_RNN_GRU ? 3 : 1);
-  const size_t fwd = res_ws_bytes(G, T, B, H, D);
-  const size_t bwd = splitk_res_ws_bytes(G, T, B, H, D);
-  return (fwd > bwd ? fwd : bwd) + 256;
-}
-
-static bool fwd_eligible(const SeqArgs& a) {
-  if (a.H % 32 != 0 || a.B > 256 || a.T < 2) return false;
-  return vec_ok(a.gates, a.hseq, a.aux);
 }
 
 __global__ void f32_to_f16_kernel(size_t n, const float* __restrict__ in, __half* __restrict__ out) {
@@ -674,11 +601,25 @@ static size_t res_smem_bytes(int NB, int H) {
          (32 + STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
-// workspace of the resident forward: [4 KB control][W16: D*G*H*H halfs][h16: (D*T + 2)*B*H halfs].  h16 is the
+// The next `bytes` (256-aligned) of a workspace layout at offset `off`, or null when the base is null (sizing only)
+template <typename T>
+static T* carve(void* base, size_t& off, size_t bytes) {
+  T* at = base ? reinterpret_cast<T*>(static_cast<char*>(base) + off) : nullptr;
+  off += align_up(bytes, 256);
+  return at;
+}
+
+// Workspace of the resident forward: [4 KB control][W16: D*G*H*H halfs][h16: (D*T + 2)*B*H halfs].  h16 is the
 // (D,T,B,H) sequence with one extra time step before it and one after it: the operands fp16(h0[0]) of the forward
 // direction's step t = 0 ("t = -1") and fp16(h0[1]) of the reverse direction's step t = T-1 ("t = T").
-static size_t res_ws_bytes(int G, int T, int B, int H, int D) {
-  return 4096 + align_up((size_t)D * G * H * H * 2, 256) + align_up(((size_t)D * T + 2) * B * H * 2, 256);
+// Returns the bytes; with a base, also the addresses (h16: of time step 0, after the extra step).
+struct ResFwdWs { __half* w16; __half* h16; };
+static size_t res_fwd_carve(int G, int T, int B, int H, int D, void* base, ResFwdWs& w) {
+  size_t off = CTL_BYTES;
+  w.w16 = carve<__half>(base, off, (size_t)D * G * H * H * 2);
+  w.h16 = carve<__half>(base, off, ((size_t)D * T + 2) * B * H * 2);
+  if (base) w.h16 += (size_t)B * H;
+  return off;
 }
 
 // Resident forward variants: the fp16 copy of W_hh (in the workspace) and the tensor maps of it and of the fp16 h
@@ -692,16 +633,17 @@ static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chu
   using namespace rp;
   const int G = a.G;
   const size_t BH = (size_t)a.B * a.H;
-  __half* w16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096);
-  p.h16 = reinterpret_cast<__half*>(static_cast<char*>(ws) + 4096 + align_up((size_t)a.D * G * a.H * a.H * 2, 256)) + BH;
+  ResFwdWs w;
+  res_fwd_carve(G, a.T, a.B, a.H, a.D, ws, w);
+  p.h16 = w.h16;
   const size_t wn = (size_t)G * a.H * a.H;
   p.box3 = chunks % 4 == 0;
   const int rows = (a.T + (state ? 2 : 0)) * a.B;
   for (int d = 0; d < a.D; ++d) {
-    DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w16 + (size_t)d * wn);
+    DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w.w16 + (size_t)d * wn);
     int rc = unit_major
-                 ? make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, G, a.H, (size_t)a.H * a.H, (size_t)a.H, 64, 4, UT)
-                 : make_tmap_f16(&p.tmW[d], w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
+                 ? make_tmap_f16(&p.tmW[d], w.w16 + (size_t)d * wn, 3, a.H, G, a.H, (size_t)a.H * a.H, (size_t)a.H, 64, 4, UT)
+                 : make_tmap_f16(&p.tmW[d], w.w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
     if (rc) return rc;
     __half* hbase = p.h16 + (size_t)d * a.T * BH - (state ? BH : 0);
     rc = make_tmap_f16(&p.tmV[d], hbase, 2, a.H, rows, 1, (size_t)a.H, 0, 64, a.B, 1);
@@ -717,74 +659,6 @@ static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chu
     }
   }
   return DS2_OK;
-}
-
-template <int RNN>
-static int launch_fwd_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
-  const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
-  if (a.H % 64 != 0 || a.H / 64 > 32) return 1;
-  if (!vec_ok(a.gates, a.hseq, a.aux)) return 1;
-  if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
-  PersistParams p = sweep_params(a, rp::UT, "DS2_TRACE_FWD", ws);
-  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  const size_t smem = one_cta_per_sm(res_smem_bytes(p.NB, a.H));
-  if (smem > 227 * 1024) return 1;
-  const bool state = a.h0 || a.c0;
-  const SweepKernel kern = state ? rnn_fwd_persist_kernel<RNN, true, true> : rnn_fwd_persist_kernel<RNN, true>;
-  static DeviceOnce attr_once;
-  int fit = 0;
-  if (int rc = opt_in_smem(attr_once, {rnn_fwd_persist_kernel<RNN, true>, rnn_fwd_persist_kernel<RNN, true, true>}))
-    return rc;
-  if (int rc = coop_fit(kern, smem, &fit)) return rc;
-  return launch_sweep(kern, 0, p.NT, smem, fit, true, 4096, nullptr, nullptr, p, st,
-                      [&] { return f16_weight_maps(a, p, ws, a.H / 64, st, false, state); });
-}
-
-template <int RNN>
-static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st);
-
-template <int RNN>
-static int launch_fwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
-  using namespace rp;
-  const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
-  if (!env_flag("DS2_NO_RESIDENT", 0)) {
-    if (RNN != DS2_RNN_TANH && env_flag("DS2_FWD_SPLITK", 1)) {   // 2-CTA clusters, half the MMA chain per step
-      constexpr int R = RNN == DS2_RNN_TANH ? DS2_RNN_LSTM : RNN;
-      int rc = launch_fwd_splitk<R>(a, ws, ws_bytes, st);
-      if (rc != 1) return rc;
-    }
-    int rc = launch_fwd_resident<RNN>(a, ws, ws_bytes, st);
-    if (rc != 1) return rc;
-  }
-  // The streaming variant reads h_{t-1} from the fp32 output hseq, which must stay 0 at padded steps and has no step
-  // before the first: it cannot carry an initial state.
-  if (a.h0 || a.c0) return 1;
-  PersistParams p = sweep_params(a, UT, "DS2_TRACE_FWD", ws);
-  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  if (ws_bytes < 4096) return 1;
-  const size_t smem = one_cta_per_sm(fwd_smem_bytes(p.NB));
-  if (smem > 227 * 1024) return 1;
-  const SweepKernel kern = rnn_fwd_persist_kernel<RNN, false>;
-  static DeviceOnce attr_once;
-  int fit = 0;
-  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
-  if (int rc = coop_fit(kern, smem, &fit)) return rc;
-  return launch_sweep(kern, 0, p.NT, smem, fit, true, 4096, nullptr, nullptr, p, st, [&] {
-    for (int d = 0; d < a.D; ++d) {
-      int rc = make_tmap_3d(&p.tmW[d], a.w_hh[d], a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, BK, UT, G);
-      if (rc) return rc;
-      rc = make_tmap_2d(&p.tmV[d], a.hseq + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
-      if (rc) return rc;
-    }
-    return 0;
-  });
-}
-
-int rnn_sweep_fwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (!fwd_eligible(a)) return 1;
-  if (rnn == DS2_RNN_LSTM) return launch_fwd<DS2_RNN_LSTM>(a, ws, ws_bytes, st);
-  if (rnn == DS2_RNN_GRU) return launch_fwd<DS2_RNN_GRU>(a, ws, ws_bytes, st);
-  return launch_fwd<DS2_RNN_TANH>(a, ws, ws_bytes, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2009,33 +1883,6 @@ static size_t fwd_splitk_smem_bytes(int NB, int H, bool defer) {
          (defer && NB == 32 ? 6 * 128 * 16 : 0) + 10 * sizeof(uint64_t) + 64;
 }
 
-// returns 1 when the shape / device does not take this variant (the caller then uses the 16-unit resident kernel)
-template <int RNN>
-static int launch_fwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : 3;
-  if (a.H % 128 != 0 || a.H / 128 > 32) return 1;
-  if (!vec_ok(a.gates, a.hseq, a.aux) || !a.aux) return 1;
-  if (ws_bytes < res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
-  PersistParams p = sweep_params(a, 32, "DS2_TRACE_FWD", ws);
-  if (p.NB > 64) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  const size_t smem = one_cta_per_sm(fwd_splitk_smem_bytes(p.NB, a.H, p.defer));
-  if (smem > 227 * 1024) return 1;
-  // H = 1024: unrolled issue loop; with an initial state, see rnn_fwd_splitk_state_kernel
-  const bool state = a.h0 || a.c0;
-  const int nkr = a.H / 128;
-  if (state && (nkr > FWD_SPLITK_MAX_NKR || !fwd_splitk_state_kernels<RNN>[nkr - 1])) return 1;
-  const SweepKernel kern = state ? fwd_splitk_state_kernels<RNN>[nkr - 1]
-                                 : (a.H == 1024 ? rnn_fwd_splitk_kernel<RNN, 8> : rnn_fwd_splitk_kernel<RNN, 0>);
-  static DeviceOnce attr_once;
-  const SweepKernel* sk = fwd_splitk_state_kernels<RNN>;
-  if (int rc = opt_in_smem(attr_once, {rnn_fwd_splitk_kernel<RNN, 8>, rnn_fwd_splitk_kernel<RNN, 0>, sk[0], sk[4], sk[7],
-                                       sk[8]}))
-    return rc;
-  const int fit = cluster_fit(kern, 2, a.D * p.NT * 2, smem, st);
-  return launch_sweep(kern, 2, p.NT * 2, smem, fit, true, 4096, "split-K forward sweep", "the 16-unit kernel", p, st,
-                      [&] { return f16_weight_maps(a, p, ws, a.H / 128, st, true, state); });
-}
-
 static size_t splitk_smem_bytes(int NB, int CL) {
   using namespace rp;
   size_t NBp = NB + 1;
@@ -2069,218 +1916,368 @@ static size_t splitk_res_smem_bytes(int NB, int Kc, int CL) {
   return 1024 + (size_t)(Kc / 64) * ((size_t)UT * CL * 128 + (size_t)NB * 128) +
          ((size_t)CL * xt_slice(UT, NB) + UT * NBp + NB + 16) * sizeof(float) + (32 + STAGES + 3) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
-// workspace of the resident backward: [4 KB control][gmax D*(T+1) uints][dymax: T uints][W^T fp16: D*H*GH]
-// [dg16: T*B*D*GH][xbuf: D*H/16 CTAs x 4 sources x 2 parities partial tiles, the 4-CTA L2 exchange]
-// The control block holds err (offset 0), the step counters (128) and the L2 exchange's xcnt (1024: <= 768 CTAs).
-constexpr size_t XCNT_OFFSET = 1024;
-constexpr int XCNT_MAX = (4096 - (int)XCNT_OFFSET) / 4;
-static size_t splitk_xbuf_bytes(int B, int H, int D) {
-  return (size_t)D * (H / 16) * 4 * 2 * xt_slice(rp::UT, (B + 31) / 32 * 32) * sizeof(float);
-}
-static size_t splitk_res_ws_bytes(int G, int T, int B, int H, int D) {
+
+// Workspace of the resident backward: [4 KB control][gmax: D*(T+1) uints][dymax: T uints][W^T fp16: D*H*GH]
+// [dg16: T*B*D*GH][xbuf: D*H/16 CTAs x 4 sources x 2 parities partial tiles, the 4-CTA L2 exchange].
+// Returns the bytes; with a base, also the addresses.
+struct ResBwdWs { unsigned int* gmax; unsigned int* dymax; __half* wT16; __half* dg16; float* xbuf; };
+static size_t res_bwd_carve(int G, int T, int B, int H, int D, void* base, ResBwdWs& w) {
   const size_t GH = (size_t)G * H;
-  return 4096 + align_up((size_t)D * (T + 1) * 4, 256) + align_up((size_t)T * 4, 256) +
-         align_up((size_t)D * H * GH * 2, 256) + align_up((size_t)T * B * D * GH * 2, 256) +
-         align_up(splitk_xbuf_bytes(B, H, D), 256);
+  size_t off = CTL_BYTES;
+  w.gmax = carve<unsigned int>(base, off, (size_t)D * (T + 1) * 4);
+  w.dymax = carve<unsigned int>(base, off, (size_t)T * 4);
+  w.wT16 = carve<__half>(base, off, (size_t)D * H * GH * 2);
+  w.dg16 = carve<__half>(base, off, (size_t)T * B * D * GH * 2);
+  w.xbuf = carve<float>(base, off, (size_t)D * (H / 16) * 4 * 2 * xt_slice(rp::UT, sweep_nb(B)) * sizeof(float));
+  return off;
 }
 
+size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
+  const int G = rnn == DS2_RNN_LSTM ? 4 : (rnn == DS2_RNN_GRU ? 3 : 1);
+  ResFwdWs fw;
+  ResBwdWs bw;
+  const size_t fwd = res_fwd_carve(G, T, B, H, D, nullptr, fw), bwd = res_bwd_carve(G, T, B, H, D, nullptr, bw);
+  return (fwd > bwd ? fwd : bwd) + 256;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Selection and launch.  choose_fwd / choose_bwd pick a sweep variant without side effects (they call nothing but the
+// shared-memory opt-ins and the occupancy queries); launch_sweep then prepares that variant's operands and launches it.
+
+// The operand preparation a sweep variant needs before its launch
+enum class Prep {
+  FWD_F32,   // maps over the fp32 W_hh and hseq: the 16-unit streaming forward
+  FWD_F16,   // fp16 W_hh in the workspace (f16_weight_maps): the resident and the split-K forward
+  BWD_F32,   // the fp32 W_hh^T (materialize_w_hh) and bwd_f32_maps: the 16-unit and the split-K streaming backward
+  BWD_F16,   // fp16 W_hh^T, max |dY[t]| and the resident backward's workspace: the resident split-K backward
+};
+
+// A sweep variant as the selection returns it
+struct SweepChoice {
+  SweepKernel kern;
+  int cluster;                      // 0: cooperative launch; 1, 2, 4, 8: cudaLaunchKernelEx in clusters of that size
+  int group;                        // CTAs that share one slice of hidden units: 1, 2, 4 or 8 (not always a cluster)
+  int per_dir;                      // CTAs per direction
+  size_t smem;
+  Prep prep;
+  int rank;                         // place in the order of preference: a refused launch resumes the selection after it
+  const char* what = nullptr;       // the variant, in the messages of a refused launch ...
+  const char* fallback = nullptr;   // ... and what runs instead, when a refusal deserves a warning
+  int launches = 0;                 // 1: both directions in one launch; D: one launch per direction
+};
+
+// CTAs of `c` that can be co-resident in a grid of `grid`: one per SM at most (see one_cta_per_sm), in whole clusters
+// (a cluster cannot span two GPCs).  -1 when the device rejects the clusters or a CTA would need more than the 227 KB of
+// shared memory it can have.  The occupancy queries depend on the opt-in: call opt_in_smem first.
+static int co_resident(const SweepChoice& c, int grid, cudaStream_t st, int* fit) {
+  *fit = -1;
+  if (c.smem > 227 * 1024) return DS2_OK;
+  if (c.cluster <= 1) {
+    int per_sm = 0;
+    DS2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, c.kern, rp::THREADS, c.smem));
+    *fit = per_sm * device_sm_count();
+    return DS2_OK;
+  }
+  SweepConfig cfg(c.cluster, grid, c.smem, st);
+  int max_clusters = 0;
+  if (cudaOccupancyMaxActiveClusters(&max_clusters, c.kern, &cfg.cfg) == cudaSuccess) *fit = max_clusters * c.cluster;
+  else (void)cudaGetLastError();
+  return DS2_OK;
+}
+
+// The grid barrier needs every CTA of a launch resident: c->launches = 1 when both directions' CTAs can be, D when
+// only one direction's can and `per_dir_ok`, otherwise 0 (the variant does not fit)
+static int place(SweepChoice* c, int D, bool per_dir_ok, cudaStream_t st) {
+  int fit = 0;
+  if (int rc = co_resident(*c, D * c->per_dir, st, &fit)) return rc;
+  c->launches = fit >= D * c->per_dir ? 1 : (per_dir_ok && fit >= c->per_dir ? D : 0);
+  return DS2_OK;
+}
+
+// Forward: the 2-CTA split-K kernel (half the MMA chain per step), the 16-unit resident kernel, the 16-unit streaming
+// kernel (DESIGN §5.1), from rank `from` on.  Returns 0 with *c, 1 when no variant takes the shape, or an error.
+template <int RNN>
+static int choose_fwd(const SeqArgs& a, size_t ws_bytes, int from, cudaStream_t st, SweepChoice* c) {
+  constexpr int R = RNN == DS2_RNN_TANH ? DS2_RNN_LSTM : RNN;   // the split-K kernels exist for LSTM and GRU
+  const int H = a.H, NB = sweep_nb(a.B);
+  // NB: columns of the MMA warpgroup's accumulator (WgAcc), 64 for the variants with MMA M = 128
+  if (H % 32 != 0 || NB > 128 || a.T < 2 || !vec_ok(a.gates, a.hseq, a.aux)) return 1;
+  const bool state = a.h0 || a.c0;
+  ResFwdWs w;
+  const bool resident = !env_flag("DS2_NO_RESIDENT", 0) && ws_bytes >= res_fwd_carve(a.G, a.T, a.B, H, a.D, nullptr, w);
+  if (from <= 0 && resident && RNN != DS2_RNN_TANH && env_flag("DS2_FWD_SPLITK", 1) && H % 128 == 0 && H / 128 <= 32 &&
+      NB <= 64 && a.aux) {
+    // with an initial state only the chunk counts of fwd_splitk_state_kernels; H = 1024: unrolled issue loop
+    const SweepKernel* sk = fwd_splitk_state_kernels<R>;
+    const int nkr = H / 128;
+    const SweepKernel kern = state ? (nkr <= FWD_SPLITK_MAX_NKR ? sk[nkr - 1] : nullptr)
+                                   : (H == 1024 ? rnn_fwd_splitk_kernel<R, 8> : rnn_fwd_splitk_kernel<R, 0>);
+    static DeviceOnce once;
+    if (kern) {
+      if (int rc = opt_in_smem(once, {rnn_fwd_splitk_kernel<R, 8>, rnn_fwd_splitk_kernel<R, 0>, sk[0], sk[4], sk[7], sk[8]}))
+        return rc;
+      *c = {kern, 2, 2, H / 16, one_cta_per_sm(fwd_splitk_smem_bytes(NB, H, sweep_defer_default())), Prep::FWD_F16, 0,
+            "split-K forward sweep", "the 16-unit kernel"};
+      if (int rc = place(c, a.D, true, st)) return rc;
+      if (c->launches) return DS2_OK;
+    }
+  }
+  if (from <= 1 && resident && H % 64 == 0 && H / 64 <= 32) {
+    static DeviceOnce once;
+    if (int rc = opt_in_smem(once, {rnn_fwd_persist_kernel<RNN, true>, rnn_fwd_persist_kernel<RNN, true, true>})) return rc;
+    *c = {state ? rnn_fwd_persist_kernel<RNN, true, true> : rnn_fwd_persist_kernel<RNN, true>, 0, 1, H / 16,
+          one_cta_per_sm(res_smem_bytes(NB, H)), Prep::FWD_F16, 1};
+    if (int rc = place(c, a.D, true, st)) return rc;
+    if (c->launches) return DS2_OK;
+  }
+  // The streaming variant reads h_{t-1} from the fp32 output hseq, which must stay 0 at padded steps and has no step
+  // before the first: it cannot carry an initial state.
+  if (!state && ws_bytes >= CTL_BYTES) {
+    static DeviceOnce once;
+    if (int rc = opt_in_smem(once, {rnn_fwd_persist_kernel<RNN, false>})) return rc;
+    *c = {rnn_fwd_persist_kernel<RNN, false>, 0, 1, H / 16, one_cta_per_sm(fwd_smem_bytes(NB)), Prep::FWD_F32, 2};
+    if (int rc = place(c, a.D, true, st)) return rc;
+    if (c->launches) return DS2_OK;
+  }
+  return 1;
+}
+
+// The split-K backward over groups of CL CTAs, resident (`res`) or streaming: *c with c->launches = 0 when the shape or
+// the device does not take it.  8-CTA groups run only with both directions in one launch: they are only worth it when
+// the directions run concurrently.
 template <int RNN, int CL>
-static int launch_bwd_splitk_resident(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+static int choose_bwd_splitk(const SeqArgs& a, size_t ws_bytes, bool res, cudaStream_t st, SweepChoice* c) {
   using namespace rp;
-  const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
-  const int GH = G * a.H;
-  constexpr int UM = UT * CL;
-  if (a.H % UM != 0 || GH % CL != 0 || (GH / CL) % 64 != 0 || (GH / CL) / 64 > 120) return 1;   // <= 32 group barriers
-  if (CL == 8 && ((a.B + 7) / 8 * 8) % 16 != 0) return 1;                                       // M = 128: N % 16 == 0
-  if (!vec_ok(a.gates, a.hseq, a.aux, a.dy)) return 1;
-  if (ws_bytes < splitk_res_ws_bytes(G, a.T, a.B, a.H, a.D)) return 1;
-  PersistParams p = sweep_params(a, UM, "DS2_TRACE_BWD", ws);
-  if (p.NB > (CL == 8 ? 64 : 128)) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
+  const int GH = a.G * a.H, Kc = GH / CL, NB = sweep_nb(a.B);   // Kc: the K of one CTA
+  if (a.H % (UT * CL) != 0 || GH % CL != 0 || NB > (CL == 8 ? 64 : 128)) return DS2_OK;
+  if (CL == 8 && ((a.B + 7) / 8 * 8) % 16 != 0) return DS2_OK;   // M = 128: N % 16 == 0
+  if (!vec_ok(a.gates, a.hseq, a.aux, a.dy)) return DS2_OK;
+  if (!res) {
+    if (Kc % BK != 0 || ws_bytes < CTL_BYTES) return DS2_OK;
+    static DeviceOnce once;
+    if (int rc = opt_in_smem(once, {rnn_bwd_splitk_kernel<RNN, false, CL>})) return rc;
+    *c = {rnn_bwd_splitk_kernel<RNN, false, CL>, CL, CL, a.H / 16, one_cta_per_sm(splitk_smem_bytes(NB, CL)),
+          Prep::BWD_F32, 0, "split-K backward sweep"};
+    return place(c, a.D, CL != 8, st);
+  }
+  // <= 32 group barriers
+  ResBwdWs w;
+  if (Kc % 64 != 0 || Kc / 64 > 120 || ws_bytes < res_bwd_carve(a.G, a.T, a.B, a.H, a.D, nullptr, w)) return DS2_OK;
+  // DS2_SPLITK_XCHG=cluster|global: force the partial-tile exchange through distributed shared memory or through L2
+  const char* xe = getenv("DS2_SPLITK_XCHG");
+  const bool force_cluster = xe && !strcmp(xe, "cluster"), force_global = xe && !strcmp(xe, "global");
+  if (force_global && CL != 4) return DS2_OK;
+  // H = 1024 (the BASELINE shapes): compile-time chunk count -> unrolled issue loop
+  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  constexpr int NKU = (G * 1024 / CL) / 64;   // chunks per CTA at H = 1024: 16 / 12 / 4 (CL 4), 8 / 6 / 2 (CL 8)
+  const bool unrolled = a.H == 1024;
+  constexpr bool XG = CL == 4;                // only the 4-CTA variant has the L2 exchange
+  static DeviceOnce once;
+  int rc = opt_in_smem(once, {rnn_bwd_splitk_kernel<RNN, true, CL, NKU>, rnn_bwd_splitk_kernel<RNN, true, CL, 0>,
+                              rnn_bwd_splitk_kernel<RNN, true, CL, NKU, XG>, rnn_bwd_splitk_kernel<RNN, true, CL, 0, XG>});
+  if (rc) return rc;
+  *c = {unrolled ? rnn_bwd_splitk_kernel<RNN, true, CL, NKU> : rnn_bwd_splitk_kernel<RNN, true, CL, 0>, CL, CL, a.H / 16,
+        one_cta_per_sm(splitk_res_smem_bytes(NB, Kc, CL)), Prep::BWD_F16, 0, "resident split-K backward sweep",
+        CL == 8 ? nullptr : "a slower variant"};
+  // From what the device reports: (1) every cluster of the grid co-resident: cluster exchange, one launch.
+  // (2) Otherwise the plain cooperative grid co-resident (a cluster cannot span two GPCs, so clusters of 4 can fail
+  // where single CTAs fit: 32 clusters of 4 on a 132-SM H100): L2 exchange, one launch.  (3) Otherwise one launch
+  // per direction with the cluster exchange.
+  const int grid = a.D * c->per_dir;
+  int fit = 0;
+  if ((rc = co_resident(*c, grid, st, &fit))) return rc;
+  if (fit < 0) return DS2_OK;
+  if (XG && (force_global || (fit < grid && !force_cluster))) {
+    SweepChoice xg = *c;
+    xg.kern = unrolled ? rnn_bwd_splitk_kernel<RNN, true, CL, NKU, XG> : rnn_bwd_splitk_kernel<RNN, true, CL, 0, XG>;
+    xg.cluster = 1;
+    if ((rc = co_resident(xg, grid, st, &fit))) return rc;
+    if (grid <= XCNT_MAX && (fit >= grid || force_global)) *c = xg;
+    else if (force_global) return DS2_OK;
+  }
+  return place(c, a.D, CL != 8, st);
+}
+
+// Backward: the 8-CTA resident and streaming split-K kernels (DS2_SPLITK_CL=8, the default), the 4-CTA resident and
+// streaming ones, the 16-unit kernel on W_hh^T (DESIGN §5.1), from rank `from` on.  Returns 0 with *c, 1 when no
+// variant takes the shape, or an error.
+template <int RNN>
+static int choose_bwd(const SeqArgs& a, size_t ws_bytes, int from, cudaStream_t st, SweepChoice* c) {
+  if (a.H % 32 != 0 || sweep_nb(a.B) > 128 || a.T < 2) return 1;
+  const bool splitk = !env_flag("DS2_NO_SPLITK", 0), resident = !env_flag("DS2_NO_RESIDENT", 0);
+  const bool cl8 = env_flag("DS2_SPLITK_CL", 8) == 8;
+  for (int rank = from; rank < 5; ++rank) {
+    int rc = DS2_OK;
+    c->launches = 0;
+    switch (rank) {
+      case 0: if (splitk && cl8 && resident) rc = choose_bwd_splitk<RNN, 8>(a, ws_bytes, true, st, c); break;
+      case 1: if (splitk && cl8) rc = choose_bwd_splitk<RNN, 8>(a, ws_bytes, false, st, c); break;
+      case 2: if (splitk && resident) rc = choose_bwd_splitk<RNN, 4>(a, ws_bytes, true, st, c); break;
+      case 3: if (splitk) rc = choose_bwd_splitk<RNN, 4>(a, ws_bytes, false, st, c); break;
+      default:
+        if (ws_bytes >= CTL_BYTES) {
+          static DeviceOnce once;
+          if ((rc = opt_in_smem(once, {rnn_bwd_persist_kernel<RNN>}))) return rc;
+          *c = {rnn_bwd_persist_kernel<RNN>, 0, 1, a.H / 16, one_cta_per_sm(fwd_smem_bytes(sweep_nb(a.B))), Prep::BWD_F32, 0};
+          rc = place(c, a.D, true, st);
+        }
+    }
+    if (rc) return rc;
+    if (c->launches) {
+      c->rank = rank;
+      return DS2_OK;
+    }
+  }
+  return 1;
+}
+
+// Maps of the streaming backward kernels: the fp32 W_hh^T (H, G*H) in boxes of `rows` unit rows, the gate gradients
+// (rows (t,b), full row width D*G*H: the direction offset is a coordinate) and, for the GRU, the n-gate part of dGh in
+// the aux buffer
+static int bwd_f32_maps(const SeqArgs& a, PersistParams& p, int rows) {
+  using namespace rp;
+  const int GH = a.G * a.H;
+  for (int d = 0; d < a.D; ++d) {
+    int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, rows, BK);
+    if (rc) return rc;
+    rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
+    if (rc) return rc;
+    if (a.G == 3) {
+      rc = make_tmap_2d(&p.tmV2[d], a.aux + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
+      if (rc) return rc;
+    }
+  }
+  return DS2_OK;
+}
+
+// The resident split-K backward: its workspace, the bias-gradient and fp16 gate-gradient outputs, the fp16 W_hh^T
+// (the forward pass's copy when there is one, else converted from the fp32 transposes), the maps over it and over the
+// fp16 gate gradients, and max |dY[t]| per time step (the step-0 scale, and part of every later step's scale: spiky
+// upstream gradients).  *ctl_bytes: the control block and gmax, which are zeroed.
+static int prepare_res_bwd(const SweepChoice& c, const SeqArgs& a, void* ws, PersistParams& p, cudaStream_t st,
+                           size_t* ctl_bytes) {
+  using namespace rp;
+  const int GH = a.G * a.H, CL = c.group;
+  ResBwdWs w;
+  res_bwd_carve(a.G, a.T, a.B, a.H, a.D, ws, w);
+  p.gmax = w.gmax; p.dymax = w.dymax; p.dg16 = w.dg16; p.xbuf = w.xbuf;
+  p.xcnt = reinterpret_cast<unsigned int*>(static_cast<char*>(ws) + CTL_XCNT);
+  *ctl_bytes = reinterpret_cast<char*>(w.dymax) - static_cast<char*>(ws);
   for (int d = 0; d < a.D; ++d) { p.dbias[d] = a.dbias[d]; p.dbias_hn[d] = a.dbias_hn[d]; }
-  if (a.f16_dg && a.f16_dgT && a.f16_scale && (RNN != DS2_RNN_GRU || a.f16_auxT)) {
+  if (a.f16_dg && a.f16_dgT && a.f16_scale && (a.G != 3 || a.f16_auxT)) {
     p.dgn16 = static_cast<__half*>(a.f16_dg);
     p.dgn16T = static_cast<__half*>(a.f16_dgT);
     p.auxn16T = static_cast<__half*>(a.f16_auxT);
     p.nscale = a.f16_scale;
   }
-  char* base = static_cast<char*>(ws);
-  size_t off = 4096;
-  p.gmax = reinterpret_cast<unsigned int*>(base + off); off += align_up((size_t)a.D * (a.T + 1) * 4, 256);
-  p.dymax = reinterpret_cast<unsigned int*>(base + off); off += align_up((size_t)a.T * 4, 256);
-  __half* wT16 = reinterpret_cast<__half*>(base + off); off += align_up((size_t)a.D * a.H * GH * 2, 256);
-  p.dg16 = reinterpret_cast<__half*>(base + off); off += align_up((size_t)a.T * a.B * a.D * GH * 2, 256);
-  p.xbuf = reinterpret_cast<float*>(base + off);
-  p.xcnt = reinterpret_cast<unsigned int*>(base + XCNT_OFFSET);
-  const size_t smem = one_cta_per_sm(splitk_res_smem_bytes(p.NB, GH / CL, CL));
-  if (smem > 227 * 1024) return 1;
-  // DS2_SPLITK_XCHG=cluster|global: force the partial-tile exchange through distributed shared memory or through L2
-  const char* xe = getenv("DS2_SPLITK_XCHG");
-  const bool force_cluster = xe && !strcmp(xe, "cluster"), force_global = xe && !strcmp(xe, "global");
-  if (force_global && CL != 4) return 1;   // only the 4-CTA variant has the L2 exchange
-  // H = 1024 (the BASELINE shapes): compile-time chunk count -> unrolled issue loop
-  constexpr int NKU = (G * 1024 / CL) / 64;   // chunks per CTA at H = 1024: 16 / 12 / 4 (CL 4), 8 / 6 / 2 (CL 8)
-  SweepKernel kern = a.H == 1024 ? rnn_bwd_splitk_kernel<RNN, true, CL, NKU> : rnn_bwd_splitk_kernel<RNN, true, CL, 0>;
-  static DeviceOnce attr_once;
-  int rc;
-  if constexpr (CL == 4)
-    rc = opt_in_smem(attr_once, {rnn_bwd_splitk_kernel<RNN, true, CL, NKU>, rnn_bwd_splitk_kernel<RNN, true, CL, 0>,
-                                 rnn_bwd_splitk_kernel<RNN, true, CL, NKU, true>, rnn_bwd_splitk_kernel<RNN, true, CL, 0, true>});
-  else
-    rc = opt_in_smem(attr_once, {rnn_bwd_splitk_kernel<RNN, true, CL, NKU>, rnn_bwd_splitk_kernel<RNN, true, CL, 0>});
-  if (rc) return rc;
-  // Path, from what the device reports: (1) every cluster of the grid co-resident: cluster exchange, one launch.
-  // (2) Otherwise the plain cooperative grid co-resident (a cluster cannot span two GPCs, so clusters of 4 can fail
-  // where single CTAs fit: 32 clusters of 4 on a 132-SM H100): L2 exchange, one launch.  (3) Otherwise one launch
-  // per direction with the cluster exchange; never with 8-CTA clusters, which are only worth it when both
-  // directions run concurrently.
-  const int grid = a.D * p.NT * CL;
-  int cluster = CL;
-  int fit = cluster_fit(kern, CL, grid, smem, st);
-  if (fit < 0) return 1;
-  if (force_global || (fit < grid && !force_cluster)) {
-    if constexpr (CL == 4) {
-      const SweepKernel kern_xg =
-          a.H == 1024 ? rnn_bwd_splitk_kernel<RNN, true, CL, NKU, true> : rnn_bwd_splitk_kernel<RNN, true, CL, 0, true>;
-      int resident = 0;
-      if ((rc = coop_fit(kern_xg, smem, &resident))) return rc;
-      if (grid <= XCNT_MAX && (resident >= grid || force_global)) {
-        kern = kern_xg;
-        cluster = 1;
-        fit = resident;
-      }
-    }
-    if (force_global && cluster != 1) return 1;
-  }
-  // the control block and gmax are zeroed
-  rc = launch_sweep(kern, cluster, p.NT * CL, smem, fit, CL != 8, 4096 + align_up((size_t)a.D * (a.T + 1) * 4, 256),
-                    "resident split-K backward sweep", CL == 8 ? nullptr : "a slower variant", p, st, [&]() -> int {
-    const size_t wn = (size_t)a.H * GH;
-    const bool cached = a.w_hhT16[0] && (a.D == 1 || a.w_hhT16[1]);   // fp16 W_hh^T left by the forward pass
+  const size_t wn = (size_t)a.H * GH;
+  const bool cached = a.w_hhT16[0] && (a.D == 1 || a.w_hhT16[1]);   // fp16 W_hh^T left by the forward pass
+  if (!cached)
+    if (int rc = materialize_w_hh(a, st)) return rc;
+  p.box3 = ((GH / CL) / 64) % 4 == 0;
+  for (int d = 0; d < a.D; ++d) {
+    const __half* wsrc = static_cast<const __half*>(a.w_hhT16[d]);
     if (!cached) {
-      int mrc = materialize_w_hh(a, st);
-      if (mrc) return mrc;
+      DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w.wT16 + (size_t)d * wn);
+      wsrc = w.wT16 + (size_t)d * wn;
     }
-    for (int d = 0; d < a.D; ++d) {
-      const __half* wsrc = static_cast<const __half*>(a.w_hhT16[d]);
-      if (!cached) {
-        DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], wT16 + (size_t)d * wn);
-        wsrc = wT16 + (size_t)d * wn;
-      }
-      int trc = make_tmap_f16(&p.tmW[d], wsrc, 2, GH, a.H, 1, (size_t)GH, 0, 64, UM, 1);
-      if (trc) return trc;
-      trc = make_tmap_f16(&p.tmV[d], p.dg16, 2, a.D * GH, a.T * a.B, 1, (size_t)a.D * GH, 0, 64, a.B, 1);
-      if (trc) return trc;
-      p.box3 = ((GH / CL) / 64) % 4 == 0;
-      if (p.box3) {
-        trc = make_tmap_f16(&p.tmV3[d], p.dg16, 3, 64, a.T * a.B, a.D * GH / 64, (size_t)a.D * GH, 64, 64, p.NB, 4);
-        if (trc) return trc;
-      }
+    int rc = make_tmap_f16(&p.tmW[d], wsrc, 2, GH, a.H, 1, (size_t)GH, 0, 64, UT * CL, 1);
+    if (rc) return rc;
+    rc = make_tmap_f16(&p.tmV[d], p.dg16, 2, a.D * GH, a.T * a.B, 1, (size_t)a.D * GH, 0, 64, a.B, 1);
+    if (rc) return rc;
+    if (p.box3) {
+      rc = make_tmap_f16(&p.tmV3[d], p.dg16, 3, 64, a.T * a.B, a.D * GH / 64, (size_t)a.D * GH, 64, 64, p.NB, 4);
+      if (rc) return rc;
     }
-    // per-time-step max |dY[t]|: the step-0 scale, and part of every later step's scale (spiky upstream gradients)
-    DS2_LAUNCH(absmax_rows_kernel, a.T, 256, 0, st, (size_t)a.B * a.H, a.dy, p.dymax);
-    return DS2_OK;
-  });
-  if (rc != DS2_OK) return rc;
-  if (a.dbias_done && a.dbias[0]) *a.dbias_done = 1;
-  if (a.f16_done && p.dgn16) *a.f16_done = 1;
+  }
+  DS2_LAUNCH(absmax_rows_kernel, a.T, 256, 0, st, (size_t)a.B * a.H, a.dy, p.dymax);
   return DS2_OK;
 }
 
-template <int RNN, int CL>
-static int launch_bwd_splitk(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+// Prepares the operands of the chosen variant, zeroes the control block, launches the sweep (c.launches launches:
+// p.d0 is the first direction of each) and sweep_check_kernel.  cluster == 0: cudaLaunchCooperativeKernel, and a
+// refused launch is an error.  cluster >= 1: cudaLaunchKernelEx in clusters of that size (1: no cluster dimension); a
+// refused first launch returns 1, with a warning on stderr when c.fallback names what runs instead, and a refused
+// second launch is an error.
+static int launch_sweep(const SweepChoice& c, const SeqArgs& a, void* ws, cudaStream_t st) {
   using namespace rp;
-  const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
-  const int GH = G * a.H;
-  if (!env_flag("DS2_NO_RESIDENT", 0)) {
-    int rc = launch_bwd_splitk_resident<RNN, CL>(a, ws, ws_bytes, st);
-    if (rc != 1) return rc;
+  const bool fwd = c.prep == Prep::FWD_F32 || c.prep == Prep::FWD_F16;
+  PersistParams p = sweep_params(a, UT * c.group, fwd ? "DS2_TRACE_FWD" : "DS2_TRACE_BWD", ws);
+  size_t ctl_bytes = CTL_BYTES;
+  int rc = DS2_OK;
+  switch (c.prep) {
+    case Prep::FWD_F32:
+      for (int d = 0; d < a.D && !rc; ++d) {
+        rc = make_tmap_3d(&p.tmW[d], a.w_hh[d], a.H, a.H, a.G, (size_t)a.H, (size_t)a.H * a.H, BK, UT, a.G);
+        if (!rc) rc = make_tmap_2d(&p.tmV[d], a.hseq + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
+      }
+      break;
+    case Prep::FWD_F16:
+      rc = f16_weight_maps(a, p, ws, a.H / (64 * c.group), st, c.group == 2, a.h0 || a.c0);
+      break;
+    case Prep::BWD_F32:
+      rc = materialize_w_hh(a, st);
+      if (!rc) rc = bwd_f32_maps(a, p, UT * c.group);
+      break;
+    case Prep::BWD_F16:
+      rc = prepare_res_bwd(c, a, ws, p, st, &ctl_bytes);
+      break;
   }
-  constexpr int UM = UT * CL;
-  if (a.H % UM != 0 || (GH / CL) % BK != 0 || GH % CL != 0) return 1;
-  { int mrc = materialize_w_hh(a, st); if (mrc) return mrc; }   // this kernel streams the fp32 W_hh^T
-  if (CL == 8 && ((a.B + 7) / 8 * 8) % 16 != 0) return 1;
-  if (!vec_ok(a.gates, a.hseq, a.aux, a.dy)) return 1;
-  PersistParams p = sweep_params(a, UM, "DS2_TRACE_BWD", ws);
-  if (p.NB > (CL == 8 ? 64 : 128)) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  if (ws_bytes < 4096) return 1;
-  const size_t smem = one_cta_per_sm(splitk_smem_bytes(p.NB, CL));
-  if (smem > 227 * 1024) return 1;
-  const SweepKernel kern = rnn_bwd_splitk_kernel<RNN, false, CL>;
-  static DeviceOnce attr_once;
-  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
-  const int fit = cluster_fit(kern, CL, a.D * p.NT * CL, smem, st);
-  return launch_sweep(kern, CL, p.NT * CL, smem, fit, CL != 8, 4096, "split-K backward sweep", nullptr, p, st, [&] {
-    for (int d = 0; d < a.D; ++d) {
-      int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, UM, BK);   // W_hh^T (H, G*H): UM unit rows per box
-      if (rc) return rc;
-      rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
-      if (rc) return rc;
-      if (RNN == DS2_RNN_GRU) {
-        rc = make_tmap_2d(&p.tmV2[d], a.aux + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
-        if (rc) return rc;
+  if (rc) return rc;
+  DS2_CHECK_CUDA(cudaMemsetAsync(p.err, 0, ctl_bytes, st));
+  const int grid = c.launches == 1 ? a.D * c.per_dir : c.per_dir;
+  SweepConfig cfg(c.cluster, grid, c.smem, st);
+  for (int li = 0; li < c.launches; ++li) {
+    p.d0 = li;
+    if (c.cluster == 0) {
+      void* args[] = {&p};
+      DS2_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)c.kern, dim3(grid), dim3(THREADS), args, c.smem, st));
+    } else {
+      const cudaError_t le = cudaLaunchKernelEx(&cfg.cfg, c.kern, p);
+      if (le != cudaSuccess) {
+        (void)cudaGetLastError();
+        if (li == 0) {
+          if (c.fallback)
+            fprintf(stderr, "ds2_b200: WARNING %s launch failed (%s); using %s\n", c.what, cudaGetErrorString(le),
+                    c.fallback);
+          return 1;
+        }
+        set_error("%s: second launch failed: %s", c.what, cudaGetErrorString(le));
+        return DS2_ERR_CUDA;
       }
     }
-    return 0;
-  });
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+  }
+  DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
+  if (c.prep == Prep::BWD_F16) {
+    if (a.dbias_done && a.dbias[0]) *a.dbias_done = 1;
+    if (a.f16_done && p.dgn16) *a.f16_done = 1;
+  }
+  return DS2_OK;
 }
 
-template <int RNN>
-static int launch_bwd(const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
-  using namespace rp;
-  const int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
-  const int GH = G * a.H;
-  { int mrc = materialize_w_hh(a, st); if (mrc) return mrc; }   // fp32 W_hh^T through TMA
-  PersistParams p = sweep_params(a, UT, "DS2_TRACE_BWD", ws);
-  if (p.NB > 128) return 1;                       // columns of the MMA warpgroup's accumulator (WgAcc)
-  if (ws_bytes < 4096) return 1;
-  const size_t smem = one_cta_per_sm(fwd_smem_bytes(p.NB));
-  if (smem > 227 * 1024) return 1;
-  const SweepKernel kern = rnn_bwd_persist_kernel<RNN>;
-  static DeviceOnce attr_once;
-  int fit = 0;
-  if (int rc = opt_in_smem(attr_once, {kern})) return rc;
-  if (int rc = coop_fit(kern, smem, &fit)) return rc;
-  return launch_sweep(kern, 0, p.NT, smem, fit, true, 4096, nullptr, nullptr, p, st, [&] {
-    for (int d = 0; d < a.D; ++d) {
-      // a.w_hh[d] is the transposed recurrent matrix (H, G*H) here
-      int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, UT, BK);
-      if (rc) return rc;
-      // gate gradients: rows (t,b), full row width D*GH (the direction offset is a coordinate)
-      rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
-      if (rc) return rc;
-      if (RNN == DS2_RNN_GRU) {
-        rc = make_tmap_2d(&p.tmV2[d], a.aux + (size_t)d * a.T * a.B * a.H, a.T * a.B, a.H, a.H, a.B, BK);
-        if (rc) return rc;
-      }
-    }
-    return 0;
-  });
+// Launches the variant `choose` picks; when cudaLaunchKernelEx refuses it, the next one it picks after it
+using ChooseSweep = int (*)(const SeqArgs&, size_t, int, cudaStream_t, SweepChoice*);
+static int run_sweep(ChooseSweep choose, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+  SweepChoice c{};
+  for (int from = 0;; from = c.rank + 1) {
+    int rc = choose(a, ws_bytes, from, st, &c);
+    if (rc) return rc;
+    rc = launch_sweep(c, a, ws, st);
+    if (rc != 1) return rc;
+  }
+}
+
+int rnn_sweep_fwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+  return run_sweep(rnn == DS2_RNN_LSTM ? choose_fwd<DS2_RNN_LSTM> : rnn == DS2_RNN_GRU ? choose_fwd<DS2_RNN_GRU>
+                                                                                      : choose_fwd<DS2_RNN_TANH>,
+                   a, ws, ws_bytes, st);
 }
 
 int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
-  if (a.H % 32 != 0 || a.B > 256 || a.T < 2) return 1;
-  {
-    int rc = 1;
-    if (!env_flag("DS2_NO_SPLITK", 0)) {
-      // 8-CTA clusters (128 units, K/8 per CTA) halve the MMA chain of a step; 4-CTA clusters take the shapes
-      // they do not (H % 128, K/8 not a multiple of 64, or 8-CTA clusters that do not fit the GPCs)
-      if (env_flag("DS2_SPLITK_CL", 8) == 8) {
-        if (rnn == DS2_RNN_LSTM) rc = launch_bwd_splitk<DS2_RNN_LSTM, 8>(a, ws, ws_bytes, st);
-        else if (rnn == DS2_RNN_GRU) rc = launch_bwd_splitk<DS2_RNN_GRU, 8>(a, ws, ws_bytes, st);
-        else rc = launch_bwd_splitk<DS2_RNN_TANH, 8>(a, ws, ws_bytes, st);
-      }
-      if (rc == 1) {
-        if (rnn == DS2_RNN_LSTM) rc = launch_bwd_splitk<DS2_RNN_LSTM, 4>(a, ws, ws_bytes, st);
-        else if (rnn == DS2_RNN_GRU) rc = launch_bwd_splitk<DS2_RNN_GRU, 4>(a, ws, ws_bytes, st);
-        else rc = launch_bwd_splitk<DS2_RNN_TANH, 4>(a, ws, ws_bytes, st);
-      }
-    }
-    if (rc != 1) return rc;   // done or a hard error; 1 = not eligible -> 16-unit kernel below
-  }
-  if (rnn == DS2_RNN_LSTM) return launch_bwd<DS2_RNN_LSTM>(a, ws, ws_bytes, st);
-  if (rnn == DS2_RNN_GRU) return launch_bwd<DS2_RNN_GRU>(a, ws, ws_bytes, st);
-  return launch_bwd<DS2_RNN_TANH>(a, ws, ws_bytes, st);
+  return run_sweep(rnn == DS2_RNN_LSTM ? choose_bwd<DS2_RNN_LSTM> : rnn == DS2_RNN_GRU ? choose_bwd<DS2_RNN_GRU>
+                                                                                      : choose_bwd<DS2_RNN_TANH>,
+                   a, ws, ws_bytes, st);
 }
-
 
 }  // namespace ds2
