@@ -99,6 +99,14 @@ struct Arena {
   }
 };
 
+// The next `bytes` (256-aligned) of a workspace layout at offset `off`, or null when the base is null (sizing only)
+template <typename T>
+inline T* carve(void* base, size_t& off, size_t bytes) {
+  T* at = base ? reinterpret_cast<T*>(static_cast<char*>(base) + off) : nullptr;
+  off += align_up(bytes, 256);
+  return at;
+}
+
 #ifdef __CUDACC__
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 

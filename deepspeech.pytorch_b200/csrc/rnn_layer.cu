@@ -5,7 +5,10 @@
 //
 // This file holds the host orchestration and the generic FFMA step kernels (any H, any B): one
 // launch per time step covering both directions.  rnn_persistent_tc.cu provides the wgmma
-// persistent sweep that replaces the step launches when the shape is eligible.
+// persistent sweep that replaces the step launches when the shape is eligible.  The backward gives
+// every sweep the layer's W_hh and workspace for the fp32 W_hh^T (SeqArgs): a sweep that reads the
+// transpose makes it.  The tensor-core backward sweep reports whether it also accumulated the bias
+// gradients and wrote the fp16 gate-gradient copies (SweepBwdOut); the layer computes what it did not.
 //
 // reserve layout (floats):  gates (T,B,D,G*H) | hseq (D,T,B,H) | aux (D,T,B,H: LSTM cell states /
 //                           GRU W_hn h + b_hn; absent for tanh) | bn mean,invstd (2*In)
@@ -23,12 +26,10 @@ namespace ds2 {
 constexpr int UT = 8;   // hidden units per CTA
 constexpr int KC = 64;  // reduction chunk staged in shared memory
 
-__device__ __forceinline__ int gates_per(int rnn) { return rnn == DS2_RNN_LSTM ? 4 : (rnn == DS2_RNN_GRU ? 3 : 1); }
-
 // grid (ceil(H/UT), D), block (32, UT)
 template <int RNN>
 __global__ void __launch_bounds__(32 * UT) rnn_step_fwd_kernel(SeqArgs a, int step) {
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  constexpr int G = num_gates(RNN);
   __shared__ float hs[32][KC + 1];
   __shared__ float ws[G * UT][KC + 1];
   const int d = blockIdx.y, T = a.T, B = a.B, H = a.H, D = a.D;
@@ -108,10 +109,10 @@ __global__ void __launch_bounds__(32 * UT) rnn_step_fwd_kernel(SeqArgs a, int st
   }
 }
 
-// Backward step.  w_hh[d] here is the TRANSPOSED recurrent matrix (H, G*H).
+// Backward step on the transposed recurrent matrix w_hhT[d] (H, G*H).
 template <int RNN>
 __global__ void __launch_bounds__(32 * UT) rnn_step_bwd_kernel(SeqArgs a, int step) {
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  constexpr int G = num_gates(RNN);
   __shared__ float gs[32][KC + 1];
   __shared__ float ws[UT][KC + 1];
   const int d = blockIdx.y, T = a.T, B = a.B, H = a.H, D = a.D;
@@ -122,7 +123,7 @@ __global__ void __launch_bounds__(32 * UT) rnn_step_bwd_kernel(SeqArgs a, int st
   const int lane = threadIdx.x, uy = threadIdx.y, tid = uy * 32 + lane;
   const int u0 = blockIdx.x * UT, u = u0 + uy;
   const int GH = G * H;
-  const float* __restrict__ WT = a.w_hh[d];
+  const float* __restrict__ WT = a.w_hhT[d];
 
   for (int bt = 0; bt < (B + 31) / 32; ++bt) {
     const int b = bt * 32 + lane;
@@ -228,8 +229,6 @@ static int colsum(int rows, int F, const float* src, size_t ld, float* dst, cuda
   return DS2_OK;
 }
 
-static inline int num_gates(int rnn) { return rnn == DS2_RNN_LSTM ? 4 : (rnn == DS2_RNN_GRU ? 3 : 1); }
-
 struct Reserve {
   float *gates, *hseq, *aux, *bnstats;
   __half* wT16;   // (D, H, G*H) fp16 W_hh^T, written by a tensor-core-mode training forward for the backward sweep
@@ -263,26 +262,56 @@ static bool wT16_take(const void* reserve) {
   return g_wT16_valid.erase(reserve) > 0;
 }
 
-// lazily materialised fp32 W_hh^T of the backward pass (SeqArgs::fill_w_hh)
-struct FillWhh {
-  int GH, H, D, done;
-  const float* const* w_hh;
-  float* wT[2];
+// Workspace of one pass, each buffer 256-byte aligned, then what the sweep and the fp32 / TF32 GEMMs use (gws):
+//   fwd  xbn (TB,In) | sums (4*In doubles) | fp16: x16 (TB,In) | W_ih16 (D*G*H,In)
+//   bwd  xbn | xhat | dxbn (TB,In) | sums (2*In doubles) | W_hh^T (H,G*H) per direction | carry (D,B,H) |
+//        fp16: dG16 (TB,D*G*H) | dG16^T | x16^T (In,TB) | h16^T (D*H,TB) | GRU aux16^T (D*H,TB) | W_ih16^T (In,D*G*H) |
+//        scale (16 floats)
+// The BN buffers are there whether or not the layer has BatchNorm; the fp16 operand copies exactly when the pass runs
+// its GEMMs on them (f16).  Returns the bytes; with a base, also the addresses.
+struct LayerWs {
+  float *xbn, *xhat, *dxbn;
+  double* sums;
+  float* w_hhT[2];
+  float* carry;
+  bool f16;
+  __half *x16, *w16, *dG16, *dG16T, *x16T, *h16T, *aux16T, *w16T;
+  float* scale;
 };
-static int fill_w_hh_cb(void* ctx, void* stream) {
-  FillWhh* f = static_cast<FillWhh*>(ctx);
-  if (f->done) return DS2_OK;
-  for (int dir = 0; dir < f->D; ++dir) {
-    int rc = transpose(f->GH, f->H, f->w_hh[dir], f->wT[dir], static_cast<cudaStream_t>(stream));
-    if (rc) return rc;
+static size_t layer_ws_carve(const ds2_rnn_desc* d, bool bwd, void* base, LayerWs& w) {
+  const size_t D = d->bidirectional ? 2 : 1, TB = (size_t)d->T * d->B, In = d->In, H = d->H;
+  const size_t GH = num_gates(d->rnn_type) * H, DGH = D * GH;
+  w = LayerWs{};
+  size_t off = 0;
+  w.xbn = carve<float>(base, off, TB * In * 4);
+  if (bwd) {
+    w.xhat = carve<float>(base, off, TB * In * 4);
+    w.dxbn = carve<float>(base, off, TB * In * 4);
   }
-  f->done = 1;
-  return DS2_OK;
+  w.sums = carve<double>(base, off, (bwd ? 2 : 4) * In * 8);
+  if (bwd) {
+    for (size_t dir = 0; dir < D; ++dir) w.w_hhT[dir] = carve<float>(base, off, GH * H * 4);
+    w.carry = carve<float>(base, off, D * d->B * H * 4);
+  }
+  w.f16 = f16_gemm_mode() && d->B % 8 == 0 && In % 8 == 0 && H % 8 == 0 && (!bwd || TB >= 128);
+  if (w.f16 && !bwd) {
+    w.x16 = carve<__half>(base, off, TB * In * 2);
+    w.w16 = carve<__half>(base, off, DGH * In * 2);
+  } else if (w.f16) {
+    w.dG16 = carve<__half>(base, off, TB * DGH * 2);
+    w.dG16T = carve<__half>(base, off, TB * DGH * 2);
+    w.x16T = carve<__half>(base, off, TB * In * 2);
+    w.h16T = carve<__half>(base, off, D * H * TB * 2);
+    if (d->rnn_type == DS2_RNN_GRU) w.aux16T = carve<__half>(base, off, D * H * TB * 2);
+    w.w16T = carve<__half>(base, off, In * DGH * 2);
+    w.scale = carve<float>(base, off, 16 * 4);
+  }
+  return off;
 }
 
 // wgmma persistent sweeps (rnn_persistent_tc.cu).  Return 1 when the shape is not eligible.
 int rnn_sweep_fwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st);
-int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st);
+int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st, SweepBwdOut* out);
 size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D);
 
 static int sweep_fwd(int rnn, const SeqArgs& a, cudaStream_t st) {
@@ -294,7 +323,12 @@ static int sweep_fwd(int rnn, const SeqArgs& a, cudaStream_t st) {
   }
   return DS2_OK;
 }
+// The FFMA backward reads the fp32 W_hh^T: transposed here, again if a tensor-core preparation made it before declining
 static int sweep_bwd(int rnn, const SeqArgs& a, cudaStream_t st) {
+  for (int dir = 0; dir < a.D; ++dir) {
+    int rc = transpose(a.G * a.H, a.H, a.w_hh[dir], a.w_hhT[dir], st);
+    if (rc) return rc;
+  }
   dim3 grid(cdiv(a.H, UT), a.D), block(32, UT);
   for (int s = 0; s < a.T; ++s) {
     if (rnn == DS2_RNN_LSTM) DS2_LAUNCH(rnn_step_bwd_kernel<DS2_RNN_LSTM>, grid, block, 0, st, a, s);
@@ -316,21 +350,18 @@ size_t ds2_rnn_reserve_floats(const ds2_rnn_desc* d) {
 
 size_t ds2_rnn_workspace_bytes(const ds2_rnn_desc* d) {
   if (!d) return 0;
-  const size_t D = d->bidirectional ? 2 : 1, G = num_gates(d->rnn_type);
-  const size_t TB = (size_t)d->T * d->B, GH = G * d->H;
-  size_t n = 0;
-  n += 3 * align_up(TB * d->In * 4, 256);                 // xbn, xhat, dxbn
-  n += align_up(4 * (size_t)d->In * 8, 256);              // BN double sums
-  n += D * align_up(GH * d->H * 4, 256);                  // W_hh^T per direction
-  n += align_up(D * (size_t)d->B * d->H * 4, 256);        // carry
-  if (f16_gemm_mode()) {
-    // precision-16 operand copies: x16, W16 (fwd); dG16, dG16^T, x16^T, h16^T, aux16^T, W16^T, scale (bwd)
-    n += 2 * align_up(TB * d->In * 2, 256) + 2 * align_up(D * GH * d->In * 2, 256) + 2 * align_up(TB * D * GH * 2, 256) +
-         2 * align_up(D * d->H * TB * 2, 256) + 512;
-  }
-  n += rnn_sweep_tc_workspace_bytes(d->rnn_type, d->T, d->B, d->H, (int)D);
-  n += ds2_gemm_workspace_bytes(1, 0, (int)GH, d->In > d->H ? d->In : d->H, (int)TB);
-  return n + 4096;
+  const int D = d->bidirectional ? 2 : 1, TB = d->T * d->B, Kr = (d->T - 1) * d->B, In = d->In, H = d->H;
+  const int GH = num_gates(d->rnn_type) * H, rows_x = d->rnn_type == DS2_RNN_GRU ? 2 * H : GH;
+  // what each ds2_gemm of the layer needs (gemm_tc's operand transposes, gemm_simt's split-K slabs): the input
+  // projection, dW_ih, dW_hh (GRU: its r, z rows and its n rows apart) and dX
+  const size_t gemm[] = {ds2_gemm_workspace_bytes(0, 1, TB, GH, In), ds2_gemm_workspace_bytes(1, 0, GH, In, TB),
+                         ds2_gemm_workspace_bytes(1, 0, rows_x, H, Kr), ds2_gemm_workspace_bytes(1, 0, H, H, Kr),
+                         ds2_gemm_workspace_bytes(0, 0, TB, In, GH)};
+  size_t gemm_max = 0;
+  for (size_t g : gemm) gemm_max = g > gemm_max ? g : gemm_max;
+  LayerWs w;
+  const size_t fwd = layer_ws_carve(d, false, nullptr, w), bwd = layer_ws_carve(d, true, nullptr, w);
+  return (fwd > bwd ? fwd : bwd) + rnn_sweep_tc_workspace_bytes(d->rnn_type, d->T, d->B, H, D) + gemm_max + 4096;
 }
 
 static int check_desc(const ds2_rnn_desc* d) {
@@ -353,39 +384,32 @@ int ds2_rnn_layer_fwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
   const int D = d->bidirectional ? 2 : 1, G = num_gates(d->rnn_type), T = d->T, B = d->B, In = d->In, H = d->H;
   const int TB = T * B, GH = G * H;
   Reserve R = carve_reserve(d, reserve);
-  Arena ar(ws, ws_bytes);
+  LayerWs W;
+  const size_t used = layer_ws_carve(d, false, ws, W);
+  void* gws = static_cast<char*>(ws) + used;
+  const size_t gws_bytes = ws_bytes - used;
   const float* xin = x;
   if (bn_gamma) {
-    float* xbn = ar.take<float>((size_t)TB * In);
-    double* sums = ar.take<double>(4 * (size_t)In);
-    rc = bn_rows_fwd(TB, In, x, bn_gamma, bn_beta, bn_rmean, bn_rvar, d->training, d->bn_momentum, d->bn_eps, xbn,
-                     nullptr, R.bnstats, sums, st);
+    rc = bn_rows_fwd(TB, In, x, bn_gamma, bn_beta, bn_rmean, bn_rvar, d->training, d->bn_momentum, d->bn_eps, W.xbn,
+                     nullptr, R.bnstats, W.sums, st);
     if (rc) return rc;
-    xin = xbn;
+    xin = W.xbn;
   }
-  void* gws = ar.base + ar.off;
-  size_t gws_bytes = ar.cap - ar.off;
   // input projection for every time step and both directions: gates[:, d*GH:(d+1)*GH] = xin . W_ih[d]^T
   {
     DS2_PROF("rnn_fwd_proj_gemm", st);
     bool done = false;
-    if (f16_gemm_mode() && B % 8 == 0 && In % 8 == 0 && H % 8 == 0) {
+    if (W.f16) {
       // precision 16: fp16 copies of the layer input and of both directions' W_ih (stacked: one N = D*G*H GEMM)
-      __half* x16 = ar.take<__half>((size_t)TB * In);
-      __half* w16 = ar.take<__half>((size_t)D * GH * In);
-      if (x16 && w16) {
-        rc = f32_to_f16_rows(TB, In, xin, In, x16, In, nullptr, st);
+      rc = f32_to_f16_rows(TB, In, xin, In, W.x16, In, nullptr, st);
+      if (rc) return rc;
+      for (int dir = 0; dir < D; ++dir) {
+        rc = f32_to_f16_rows(GH, In, w_ih[dir], In, W.w16 + (size_t)dir * GH * In, In, nullptr, st);
         if (rc) return rc;
-        for (int dir = 0; dir < D; ++dir) {
-          rc = f32_to_f16_rows(GH, In, w_ih[dir], In, w16 + (size_t)dir * GH * In, In, nullptr, st);
-          if (rc) return rc;
-        }
-        rc = gemm_tc_f16(TB, D * GH, In, 1.f, x16, In, w16, In, 0.f, R.gates, D * GH, nullptr, st);
-        if (rc < 0) return rc;
-        done = rc == 0;
       }
-      gws = ar.base + ar.off;
-      gws_bytes = ar.cap - ar.off;
+      rc = gemm_tc_f16(TB, D * GH, In, 1.f, W.x16, In, W.w16, In, 0.f, R.gates, D * GH, nullptr, st);
+      if (rc < 0) return rc;
+      done = rc == 0;
     }
     for (int dir = 0; dir < D && !done; ++dir) {
       rc = ds2_gemm(0, 1, TB, GH, In, 1.f, xin, In, w_ih[dir], In, 0.f, R.gates + (size_t)dir * GH, D * GH, gws,
@@ -457,92 +481,54 @@ int ds2_rnn_layer_bwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
   const int D = d->bidirectional ? 2 : 1, G = num_gates(d->rnn_type), T = d->T, B = d->B, In = d->In, H = d->H;
   const int TB = T * B, GH = G * H;
   Reserve R = carve_reserve(d, reserve);
-  Arena ar(ws, ws_bytes);
-  float *xbn = nullptr, *xhat = nullptr, *dxbn = nullptr;
-  double* sums = nullptr;
-  if (bn_gamma) {
-    xbn = ar.take<float>((size_t)TB * In);
-    xhat = ar.take<float>((size_t)TB * In);
-    dxbn = ar.take<float>((size_t)TB * In);
-    sums = ar.take<double>(2 * (size_t)In);
-  }
-  float* wT[2] = {nullptr, nullptr};
-  for (int dir = 0; dir < D; ++dir) wT[dir] = ar.take<float>((size_t)GH * H);
-  float* carry = ar.take<float>((size_t)D * B * H);
-  void* gws = ar.base + ar.off;
-  size_t gws_bytes = ar.cap - ar.off;
+  LayerWs W;
+  const size_t used = layer_ws_carve(d, true, ws, W);
+  void* gws = static_cast<char*>(ws) + used;
+  const size_t gws_bytes = ws_bytes - used;
 
-  // W_hh^T: fp16 copy from the forward pass when there is one (the fp32 transposes are then made only if a path that
-  // streams fp32 weights is taken), otherwise transposed here
-  FillWhh fill{GH, H, D, 0, w_hh, {wT[0], wT[1]}};
+  // W_hh^T: the fp16 copy from the forward pass when there is one; the sweep that needs another form makes it
   const bool have_wT16 = tensor_core_mode() && wT16_take(reserve);
-  if (have_wT16) {
-    if (side) {   // written on the side stream by the forward pass
-      rc = side_wait_for_workspace(reserve, st);
-      if (rc) return rc;
-    }
-  } else {
-    rc = fill_w_hh_cb(&fill, st);
+  if (have_wT16 && side) {   // written on the side stream by the forward pass
+    rc = side_wait_for_workspace(reserve, st);
     if (rc) return rc;
   }
-  DS2_CHECK_CUDA(cudaMemsetAsync(carry, 0, sizeof(float) * (size_t)D * B * H, st));
+  DS2_CHECK_CUDA(cudaMemsetAsync(W.carry, 0, sizeof(float) * (size_t)D * B * H, st));
   SeqArgs a{};
   a.T = T; a.B = B; a.H = H; a.D = D; a.G = G; a.len = len;
   a.gates = R.gates; a.hseq = R.hseq; a.aux = R.aux;
-  for (int dir = 0; dir < D; ++dir) { a.w_hh[dir] = wT[dir]; a.b_ih[dir] = b_ih[dir]; a.b_hh[dir] = b_hh[dir]; }
-  a.dy = dy; a.carry = carry; a.training = 1;
-  a.fill_w_hh = fill_w_hh_cb; a.fill_w_hh_ctx = &fill;
+  for (int dir = 0; dir < D; ++dir) {
+    a.w_hh[dir] = w_hh[dir]; a.w_hhT[dir] = W.w_hhT[dir]; a.b_ih[dir] = b_ih[dir]; a.b_hh[dir] = b_hh[dir];
+  }
+  a.dy = dy; a.carry = W.carry; a.training = 1;
   if (have_wT16)
     for (int dir = 0; dir < D; ++dir) a.w_hhT16[dir] = R.wT16 + (size_t)dir * H * GH;
   // bias gradients are column sums of the gate gradients: the tensor-core sweep can accumulate them on the fly
-  int dbias_done = 0;
-  const bool gru_l = d->rnn_type == DS2_RNN_GRU;
+  const bool gru = d->rnn_type == DS2_RNN_GRU;
   for (int dir = 0; dir < D; ++dir) {
     a.dbias[dir] = db_ih[dir];
-    a.dbias_hn[dir] = gru_l ? db_hh[dir] + 2 * H : nullptr;
+    a.dbias_hn[dir] = gru ? db_hh[dir] + 2 * H : nullptr;
     DS2_CHECK_CUDA(cudaMemsetAsync(db_ih[dir], 0, sizeof(float) * GH, st));
-    if (gru_l) DS2_CHECK_CUDA(cudaMemsetAsync(db_hh[dir] + 2 * H, 0, sizeof(float) * H, st));
+    if (gru) DS2_CHECK_CUDA(cudaMemsetAsync(db_hh[dir] + 2 * H, 0, sizeof(float) * H, st));
   }
-  a.dbias_done = &dbias_done;
   // ---- precision 16: scaled fp16 copies of the gate gradients (row-major for dX, transposed for the weight
   // gradients), transposed fp16 copies of the layer input / the hidden sequence / W_ih; every GEMM K-major fp16.
-  // The split-K sweep writes the gate-gradient copies itself (scale from max|dY|); other sweeps leave f16_done = 0
-  // and the copies are converted from the fp32 gate gradients afterwards.
-  const bool gru = d->rnn_type == DS2_RNN_GRU;
-  __half *dG16 = nullptr, *dG16T = nullptr, *x16T = nullptr, *h16T = nullptr, *aux16T = nullptr, *w16T = nullptr;
-  float* scale = nullptr;
-  int f16_done = 0;
-  bool f16 = f16_gemm_mode() && B % 8 == 0 && In % 8 == 0 && H % 8 == 0 && TB >= 128;
+  // The split-K sweep writes the gate-gradient copies itself (scale from max|dY|); after other sweeps they are
+  // converted from the fp32 gate gradients.
+  const bool f16 = W.f16;
   if (f16) {
-    const size_t DGH = (size_t)D * GH;
-    dG16 = ar.take<__half>((size_t)TB * DGH);
-    dG16T = ar.take<__half>((size_t)TB * DGH);
-    x16T = ar.take<__half>((size_t)TB * In);
-    h16T = ar.take<__half>((size_t)D * H * TB);
-    aux16T = gru ? ar.take<__half>((size_t)D * H * TB) : nullptr;
-    w16T = ar.take<__half>((size_t)In * DGH);
-    scale = ar.take<float>(16);
-    f16 = dG16 && dG16T && x16T && h16T && w16T && scale && (!gru || aux16T);
-    gws = ar.base + ar.off;
-    gws_bytes = ar.cap - ar.off;
-  }
-  if (f16) {
-    rc = pow2_scale_for(TB, H, dy, (size_t)H, reinterpret_cast<unsigned int*>(scale + 8), scale, 5, st);
+    rc = pow2_scale_for(TB, H, dy, (size_t)H, reinterpret_cast<unsigned int*>(W.scale + 8), W.scale, 5, st);
     if (rc) return rc;
-    a.f16_dg = dG16; a.f16_dgT = dG16T; a.f16_auxT = aux16T; a.f16_scale = scale; a.f16_done = &f16_done;
+    a.f16_dg = W.dG16; a.f16_dgT = W.dG16T; a.f16_auxT = W.aux16T; a.f16_scale = W.scale;
   }
+  SweepBwdOut made{false, false};
   {
     DS2_PROF("rnn_bwd_sweep", st);
     rc = 1;
     if (tensor_core_mode()) {
-      rc = rnn_sweep_bwd_tc(d->rnn_type, a, gws, gws_bytes, st);
+      rc = rnn_sweep_bwd_tc(d->rnn_type, a, gws, gws_bytes, st, &made);
       if (rc == 1) note_fallback("backward sweep", d->rnn_type, T, B, H, D);
     }
-    if (rc == 1) {
-      rc = fill_w_hh_cb(&fill, st);
-      if (rc) return rc;
-      rc = sweep_bwd(d->rnn_type, a, st);
-    }
+    if (rc == 1) rc = sweep_bwd(d->rnn_type, a, st);
     if (rc) return rc;
   }
 
@@ -550,22 +536,22 @@ int ds2_rnn_layer_bwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
   const float* xin = x;
   if (bn_gamma) {
     // recompute xhat and xbn from the saved batch statistics
-    rc = bn_rows_reapply(TB, In, x, bn_gamma, bn_beta, R.bnstats, xbn, xhat, st);
+    rc = bn_rows_reapply(TB, In, x, bn_gamma, bn_beta, R.bnstats, W.xbn, W.xhat, st);
     if (rc) return rc;
-    xin = xbn;
+    xin = W.xbn;
   }
   DS2_PROF("rnn_bwd_gemms", st);
   if (f16) {
     const size_t DGH = (size_t)D * GH;
-    if (!f16_done) {
-      unsigned int* absmax_ws = reinterpret_cast<unsigned int*>(scale + 8);
-      rc = pow2_scale_for(TB, (int)DGH, R.gates, DGH, absmax_ws, scale, 10, st);
+    if (!made.f16) {
+      unsigned int* absmax_ws = reinterpret_cast<unsigned int*>(W.scale + 8);
+      rc = pow2_scale_for(TB, (int)DGH, R.gates, DGH, absmax_ws, W.scale, 10, st);
       if (rc) return rc;
-      rc = f32_to_f16_transpose(TB, (int)DGH, R.gates, DGH, dG16, DGH, dG16T, (size_t)TB, scale, st);
+      rc = f32_to_f16_transpose(TB, (int)DGH, R.gates, DGH, W.dG16, DGH, W.dG16T, (size_t)TB, W.scale, st);
       if (rc) return rc;
     }
     for (int dir = 0; dir < D; ++dir) {
-      rc = f32_to_f16_transpose(GH, In, w_ih[dir], (size_t)In, nullptr, 0, w16T + (size_t)dir * GH, DGH, nullptr, st);
+      rc = f32_to_f16_transpose(GH, In, w_ih[dir], (size_t)In, nullptr, 0, W.w16T + (size_t)dir * GH, DGH, nullptr, st);
       if (rc) return rc;
     }
   }
@@ -579,22 +565,36 @@ int ds2_rnn_layer_bwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
     gst = side;
   }
   if (f16) {
-    rc = f32_to_f16_transpose(TB, In, xin, (size_t)In, nullptr, 0, x16T, (size_t)TB, nullptr, gst);
+    rc = f32_to_f16_transpose(TB, In, xin, (size_t)In, nullptr, 0, W.x16T, (size_t)TB, nullptr, gst);
     if (rc) return rc;
     for (int dir = 0; dir < D; ++dir) {
-      rc = f32_to_f16_transpose(TB, H, R.hseq + (size_t)dir * TB * H, (size_t)H, nullptr, 0, h16T + (size_t)dir * H * TB,
+      rc = f32_to_f16_transpose(TB, H, R.hseq + (size_t)dir * TB * H, (size_t)H, nullptr, 0, W.h16T + (size_t)dir * H * TB,
                                 (size_t)TB, nullptr, gst);
       if (rc) return rc;
-      if (gru && !f16_done) {
+      if (gru && !made.f16) {
         rc = f32_to_f16_transpose(TB, H, R.aux + (size_t)dir * TB * H, (size_t)H, nullptr, 0,
-                                  aux16T + (size_t)dir * H * TB, (size_t)TB, scale, gst);
+                                  W.aux16T + (size_t)dir * H * TB, (size_t)TB, W.scale, gst);
         if (rc) return rc;
       }
     }
   }
+  // C (M,N) = A^T . B over K rows of (t,b): on the fp16 copies A16 (M,K) and B16 (N,K) (row stride TB) on gst when
+  // the pass has them and gemm_tc_f16 takes the shape, otherwise with ds2_gemm on the fp32 A (K,M) and B (K,N) on st
+  auto weight_grad = [&](int M, int N, int K, const __half* A16, const __half* B16, const float* A, int lda,
+                         const float* Bf, int ldb, float* C, int ldc) {
+    int r = 1;
+    if (f16) {
+      r = gemm_tc_f16(M, N, K, 1.f, A16, TB, B16, TB, 0.f, C, ldc, W.scale + 1, gst);
+      if (r < 0) return r;
+    }
+    return r == 1 ? ds2_gemm(1, 0, M, N, K, 1.f, A, lda, Bf, ldb, 0.f, C, ldc, gws, gws_bytes, stream) : r;
+  };
+  // element `off` of an fp16 copy; null when the pass has no fp16 copies
+  auto f16_at = [&](const __half* p, size_t off) { return f16 ? p + off : nullptr; };
   bool dx_done = false;
   if (f16 && dx) {   // dX = dG (TB x D*GH) . [W_ih fwd ; W_ih rev] : one K = D*G*H GEMM for both directions
-    rc = gemm_tc_f16(TB, In, D * GH, 1.f, dG16, D * GH, w16T, D * GH, 0.f, bn_gamma ? dxbn : dx, In, scale + 1, st);
+    rc = gemm_tc_f16(TB, In, D * GH, 1.f, W.dG16, D * GH, W.w16T, D * GH, 0.f, bn_gamma ? W.dxbn : dx, In, W.scale + 1,
+                     st);
     if (rc < 0) return rc;
     dx_done = rc == 0;
   }
@@ -604,42 +604,26 @@ int ds2_rnn_layer_bwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
     const float* aux_d = R.aux ? R.aux + (size_t)dir * TB * H : nullptr;   // GRU: dGh_n (TB,H)
     const float* hseq_d = R.hseq + (size_t)dir * TB * H;
     // dW_ih = dGx^T . xin
-    rc = 1;
-    if (f16) {
-      rc = gemm_tc_f16(GH, In, TB, 1.f, dG16T + (size_t)dir * GH * TB, TB, x16T, TB, 0.f, dw_ih[dir], In, scale + 1, gst);
-      if (rc < 0) return rc;
-    }
-    if (rc == 1) rc = ds2_gemm(1, 0, GH, In, TB, 1.f, dG, ldg, xin, In, 0.f, dw_ih[dir], In, gws, gws_bytes, stream);
+    rc = weight_grad(GH, In, TB, f16_at(W.dG16T, (size_t)dir * GH * TB), W.x16T, dG, ldg, xin, In, dw_ih[dir], In);
     if (rc) return rc;
-    if (!dbias_done) {
+    if (!made.dbias) {
       rc = colsum(TB, GH, dG, ldg, db_ih[dir], st);
       if (rc) return rc;
     }
-    // dW_hh = sum_t dGh[t]^T . h_prev[t]; h_prev[t] = hseq[t-1] (forward) / hseq[t+1] (reverse)
+    // dW_hh = sum_t dGh[t]^T . h_prev[t]; h_prev[t] = hseq[t-1] (forward) / hseq[t+1] (reverse).  In the transposed
+    // fp16 copies a shift by one time step is a shift by B columns.
     const int Kr = (T - 1) * B;
     const size_t a_off = dir == 0 ? (size_t)B : 0, h_off = dir == 0 ? 0 : (size_t)B;
     const int rows_x = gru ? 2 * H : GH;   // rows whose dGh == dGx
     if (Kr > 0) {
-      rc = 1;
-      if (f16) {   // in the transposed copies a shift by one time step is a shift by B columns
-        rc = gemm_tc_f16(rows_x, H, Kr, 1.f, dG16T + (size_t)dir * GH * TB + a_off, TB, h16T + (size_t)dir * H * TB + h_off,
-                         TB, 0.f, dw_hh[dir], H, scale + 1, gst);
-        if (rc < 0) return rc;
-      }
-      if (rc == 1)
-        rc = ds2_gemm(1, 0, rows_x, H, Kr, 1.f, dG + a_off * ldg, ldg, hseq_d + h_off * H, H, 0.f, dw_hh[dir], H, gws,
-                      gws_bytes, stream);
+      rc = weight_grad(rows_x, H, Kr, f16_at(W.dG16T, (size_t)dir * GH * TB + a_off),
+                       f16_at(W.h16T, (size_t)dir * H * TB + h_off), dG + a_off * ldg, ldg, hseq_d + h_off * H, H,
+                       dw_hh[dir], H);
       if (rc) return rc;
       if (gru) {
-        rc = 1;
-        if (f16) {
-          rc = gemm_tc_f16(H, H, Kr, 1.f, aux16T + (size_t)dir * H * TB + a_off, TB, h16T + (size_t)dir * H * TB + h_off,
-                           TB, 0.f, dw_hh[dir] + (size_t)2 * H * H, H, scale + 1, gst);
-          if (rc < 0) return rc;
-        }
-        if (rc == 1)
-          rc = ds2_gemm(1, 0, H, H, Kr, 1.f, aux_d + a_off * H, H, hseq_d + h_off * H, H, 0.f,
-                        dw_hh[dir] + (size_t)2 * H * H, H, gws, gws_bytes, stream);
+        rc = weight_grad(H, H, Kr, f16_at(W.aux16T, (size_t)dir * H * TB + a_off),
+                         f16_at(W.h16T, (size_t)dir * H * TB + h_off), aux_d + a_off * H, H,
+                         hseq_d + h_off * H, H, dw_hh[dir] + (size_t)2 * H * H, H);
         if (rc) return rc;
       }
     } else {
@@ -647,7 +631,7 @@ int ds2_rnn_layer_bwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
     }
     if (gru) {
       DS2_CHECK_CUDA(cudaMemcpyAsync(db_hh[dir], db_ih[dir], sizeof(float) * 2 * H, cudaMemcpyDeviceToDevice, st));
-      if (!dbias_done) {
+      if (!made.dbias) {
         rc = colsum(TB, H, aux_d, H, db_hh[dir] + 2 * H, st);
         if (rc) return rc;
       }
@@ -656,7 +640,7 @@ int ds2_rnn_layer_bwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
     }
     // dX (pre-BN-affine) += dGx . W_ih
     if (dx && !dx_done) {
-      rc = ds2_gemm(0, 0, TB, In, GH, 1.f, dG, ldg, w_ih[dir], In, dir == 0 ? 0.f : 1.f, bn_gamma ? dxbn : dx, In,
+      rc = ds2_gemm(0, 0, TB, In, GH, 1.f, dG, ldg, w_ih[dir], In, dir == 0 ? 0.f : 1.f, bn_gamma ? W.dxbn : dx, In,
                     gws, gws_bytes, stream);
       if (rc) return rc;
     }
@@ -667,7 +651,7 @@ int ds2_rnn_layer_bwd(const ds2_rnn_desc* d, const float* x, const int32_t* len,
   }
   if (bn_gamma) {
     DS2_REQUIRE(dx && dbn_gamma && dbn_beta, "rnn bwd: BN layer needs dx, dbn_gamma, dbn_beta");
-    rc = bn_rows_bwd(TB, In, xhat, bn_gamma, R.bnstats, dxbn, dx, dbn_gamma, dbn_beta, sums, st);
+    rc = bn_rows_bwd(TB, In, W.xhat, bn_gamma, R.bnstats, W.dxbn, dx, dbn_gamma, dbn_beta, W.sums, st);
     if (rc) return rc;
   }
   return DS2_OK;

@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_fwd_persist_kernel(const _
   using namespace rp;
   using namespace tc;
   static_assert(RES || !ST, "the streaming variant reads h_{t-1} from hseq and cannot carry an initial state");
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  constexpr int G = num_gates(RNN);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned, still __shared__
   const int NB = p.NB, B = p.B, T = p.T, H = p.H, D = p.D;
@@ -601,14 +601,6 @@ static size_t res_smem_bytes(int NB, int H) {
          (32 + STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
-// The next `bytes` (256-aligned) of a workspace layout at offset `off`, or null when the base is null (sizing only)
-template <typename T>
-static T* carve(void* base, size_t& off, size_t bytes) {
-  T* at = base ? reinterpret_cast<T*>(static_cast<char*>(base) + off) : nullptr;
-  off += align_up(bytes, 256);
-  return at;
-}
-
 // Workspace of the resident forward: [4 KB control][W16: D*G*H*H halfs][h16: (D*T + 2)*B*H halfs].  h16 is the
 // (D,T,B,H) sequence with one extra time step before it and one after it: the operands fp16(h0[0]) of the forward
 // direction's step t = 0 ("t = -1") and fp16(h0[1]) of the reverse direction's step t = T-1 ("t = T").
@@ -673,7 +665,7 @@ template <int RNN>
 __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_persist_kernel(const __grid_constant__ PersistParams p) {
   using namespace rp;
   using namespace tc;
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  constexpr int G = num_gates(RNN);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned, still __shared__
   const int NB = p.NB, B = p.B, T = p.T, H = p.H, D = p.D;
@@ -919,7 +911,7 @@ __global__ void __launch_bounds__(rp::THREADS, 1) rnn_bwd_splitk_kernel(const __
   using namespace rp;
   using namespace tc;
   static_assert(!XG || (RES && CL == 4), "the L2 exchange is built for the resident 4-CTA variant");
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  constexpr int G = num_gates(RNN);
   constexpr int UM = UT * CL;                  // units per cluster (all M rows valid): 64 or 128 = MMA M
   constexpr int A_BYTES = UM * 128;            // one K chunk of the weight tile (shadows rp::A_BYTES)
   extern __shared__ uint8_t smem_raw[];
@@ -1510,7 +1502,7 @@ template <int RNN, int NKR_T, bool ST>
 __device__ __forceinline__ void fwd_splitk_sweep(const PersistParams& p) {
   using namespace rp;
   using namespace tc;
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : 3;
+  constexpr int G = num_gates(RNN);
   constexpr int AW = 128 * 128;                          // bytes of one K chunk of the weight tile (128 rows)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned, still __shared__
@@ -1933,7 +1925,7 @@ static size_t res_bwd_carve(int G, int T, int B, int H, int D, void* base, ResBw
 }
 
 size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
-  const int G = rnn == DS2_RNN_LSTM ? 4 : (rnn == DS2_RNN_GRU ? 3 : 1);
+  const int G = num_gates(rnn);
   ResFwdWs fw;
   ResBwdWs bw;
   const size_t fwd = res_fwd_carve(G, T, B, H, D, nullptr, fw), bwd = res_bwd_carve(G, T, B, H, D, nullptr, bw);
@@ -1948,7 +1940,7 @@ size_t rnn_sweep_tc_workspace_bytes(int rnn, int T, int B, int H, int D) {
 enum class Prep {
   FWD_F32,   // maps over the fp32 W_hh and hseq: the 16-unit streaming forward
   FWD_F16,   // fp16 W_hh in the workspace (f16_weight_maps): the resident and the split-K forward
-  BWD_F32,   // the fp32 W_hh^T (materialize_w_hh) and bwd_f32_maps: the 16-unit and the split-K streaming backward
+  BWD_F32,   // the fp32 W_hh^T and its maps (bwd_f32_maps): the 16-unit and the split-K streaming backward
   BWD_F16,   // fp16 W_hh^T, max |dY[t]| and the resident backward's workspace: the resident split-K backward
 };
 
@@ -2068,7 +2060,7 @@ static int choose_bwd_splitk(const SeqArgs& a, size_t ws_bytes, bool res, cudaSt
   const bool force_cluster = xe && !strcmp(xe, "cluster"), force_global = xe && !strcmp(xe, "global");
   if (force_global && CL != 4) return DS2_OK;
   // H = 1024 (the BASELINE shapes): compile-time chunk count -> unrolled issue loop
-  constexpr int G = RNN == DS2_RNN_LSTM ? 4 : (RNN == DS2_RNN_GRU ? 3 : 1);
+  constexpr int G = num_gates(RNN);
   constexpr int NKU = (G * 1024 / CL) / 64;   // chunks per CTA at H = 1024: 16 / 12 / 4 (CL 4), 8 / 6 / 2 (CL 8)
   const bool unrolled = a.H == 1024;
   constexpr bool XG = CL == 4;                // only the 4-CTA variant has the L2 exchange
@@ -2131,14 +2123,16 @@ static int choose_bwd(const SeqArgs& a, size_t ws_bytes, int from, cudaStream_t 
   return 1;
 }
 
-// Maps of the streaming backward kernels: the fp32 W_hh^T (H, G*H) in boxes of `rows` unit rows, the gate gradients
-// (rows (t,b), full row width D*G*H: the direction offset is a coordinate) and, for the GRU, the n-gate part of dGh in
-// the aux buffer
-static int bwd_f32_maps(const SeqArgs& a, PersistParams& p, int rows) {
+// Operands of the streaming backward kernels: the fp32 W_hh^T (H, G*H), transposed here into w_hhT, and the maps over
+// it in boxes of `rows` unit rows, over the gate gradients (rows (t,b), full row width D*G*H: the direction offset is
+// a coordinate) and, for the GRU, over the n-gate part of dGh in the aux buffer
+static int bwd_f32_maps(const SeqArgs& a, PersistParams& p, int rows, cudaStream_t st) {
   using namespace rp;
   const int GH = a.G * a.H;
   for (int d = 0; d < a.D; ++d) {
-    int rc = make_tmap_2d(&p.tmW[d], a.w_hh[d], a.H, GH, GH, rows, BK);
+    int rc = transpose(GH, a.H, a.w_hh[d], a.w_hhT[d], st);
+    if (rc) return rc;
+    rc = make_tmap_2d(&p.tmW[d], a.w_hhT[d], a.H, GH, GH, rows, BK);
     if (rc) return rc;
     rc = make_tmap_2d(&p.tmV[d], a.gates, a.T * a.B, a.D * GH, a.D * GH, a.B, BK);
     if (rc) return rc;
@@ -2151,7 +2145,7 @@ static int bwd_f32_maps(const SeqArgs& a, PersistParams& p, int rows) {
 }
 
 // The resident split-K backward: its workspace, the bias-gradient and fp16 gate-gradient outputs, the fp16 W_hh^T
-// (the forward pass's copy when there is one, else converted from the fp32 transposes), the maps over it and over the
+// (the forward pass's copy when there is one, else converted from the fp32 transpose), the maps over it and over the
 // fp16 gate gradients, and max |dY[t]| per time step (the step-0 scale, and part of every later step's scale: spiky
 // upstream gradients).  *ctl_bytes: the control block and gmax, which are zeroed.
 static int prepare_res_bwd(const SweepChoice& c, const SeqArgs& a, void* ws, PersistParams& p, cudaStream_t st,
@@ -2172,13 +2166,12 @@ static int prepare_res_bwd(const SweepChoice& c, const SeqArgs& a, void* ws, Per
   }
   const size_t wn = (size_t)a.H * GH;
   const bool cached = a.w_hhT16[0] && (a.D == 1 || a.w_hhT16[1]);   // fp16 W_hh^T left by the forward pass
-  if (!cached)
-    if (int rc = materialize_w_hh(a, st)) return rc;
   p.box3 = ((GH / CL) / 64) % 4 == 0;
   for (int d = 0; d < a.D; ++d) {
     const __half* wsrc = static_cast<const __half*>(a.w_hhT16[d]);
     if (!cached) {
-      DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w.wT16 + (size_t)d * wn);
+      if (int rc = transpose(GH, a.H, a.w_hh[d], a.w_hhT[d], st)) return rc;
+      DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hhT[d], w.wT16 + (size_t)d * wn);
       wsrc = w.wT16 + (size_t)d * wn;
     }
     int rc = make_tmap_f16(&p.tmW[d], wsrc, 2, GH, a.H, 1, (size_t)GH, 0, 64, UT * CL, 1);
@@ -2198,8 +2191,8 @@ static int prepare_res_bwd(const SweepChoice& c, const SeqArgs& a, void* ws, Per
 // p.d0 is the first direction of each) and sweep_check_kernel.  cluster == 0: cudaLaunchCooperativeKernel, and a
 // refused launch is an error.  cluster >= 1: cudaLaunchKernelEx in clusters of that size (1: no cluster dimension); a
 // refused first launch returns 1, with a warning on stderr when c.fallback names what runs instead, and a refused
-// second launch is an error.
-static int launch_sweep(const SweepChoice& c, const SeqArgs& a, void* ws, cudaStream_t st) {
+// second launch is an error.  `out` (backward): what the sweep produced besides the gate gradients.
+static int launch_sweep(const SweepChoice& c, const SeqArgs& a, void* ws, cudaStream_t st, SweepBwdOut* out) {
   using namespace rp;
   const bool fwd = c.prep == Prep::FWD_F32 || c.prep == Prep::FWD_F16;
   PersistParams p = sweep_params(a, UT * c.group, fwd ? "DS2_TRACE_FWD" : "DS2_TRACE_BWD", ws);
@@ -2216,8 +2209,7 @@ static int launch_sweep(const SweepChoice& c, const SeqArgs& a, void* ws, cudaSt
       rc = f16_weight_maps(a, p, ws, a.H / (64 * c.group), st, c.group == 2, a.h0 || a.c0);
       break;
     case Prep::BWD_F32:
-      rc = materialize_w_hh(a, st);
-      if (!rc) rc = bwd_f32_maps(a, p, UT * c.group);
+      rc = bwd_f32_maps(a, p, UT * c.group, st);
       break;
     case Prep::BWD_F16:
       rc = prepare_res_bwd(c, a, ws, p, st, &ctl_bytes);
@@ -2249,21 +2241,19 @@ static int launch_sweep(const SweepChoice& c, const SeqArgs& a, void* ws, cudaSt
     g_launches.fetch_add(1, std::memory_order_relaxed);
   }
   DS2_LAUNCH(sweep_check_kernel, 1, 1, 0, st, p.err);
-  if (c.prep == Prep::BWD_F16) {
-    if (a.dbias_done && a.dbias[0]) *a.dbias_done = 1;
-    if (a.f16_done && p.dgn16) *a.f16_done = 1;
-  }
+  if (out && c.prep == Prep::BWD_F16) *out = {a.dbias[0] != nullptr, p.dgn16 != nullptr};
   return DS2_OK;
 }
 
 // Launches the variant `choose` picks; when cudaLaunchKernelEx refuses it, the next one it picks after it
 using ChooseSweep = int (*)(const SeqArgs&, size_t, int, cudaStream_t, SweepChoice*);
-static int run_sweep(ChooseSweep choose, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+static int run_sweep(ChooseSweep choose, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st,
+                     SweepBwdOut* out = nullptr) {
   SweepChoice c{};
   for (int from = 0;; from = c.rank + 1) {
     int rc = choose(a, ws_bytes, from, st, &c);
     if (rc) return rc;
-    rc = launch_sweep(c, a, ws, st);
+    rc = launch_sweep(c, a, ws, st, out);
     if (rc != 1) return rc;
   }
 }
@@ -2274,10 +2264,11 @@ int rnn_sweep_fwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaS
                    a, ws, ws_bytes, st);
 }
 
-int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st) {
+int rnn_sweep_bwd_tc(int rnn, const SeqArgs& a, void* ws, size_t ws_bytes, cudaStream_t st, SweepBwdOut* out) {
+  *out = {false, false};
   return run_sweep(rnn == DS2_RNN_LSTM ? choose_bwd<DS2_RNN_LSTM> : rnn == DS2_RNN_GRU ? choose_bwd<DS2_RNN_GRU>
                                                                                       : choose_bwd<DS2_RNN_TANH>,
-                   a, ws, ws_bytes, st);
+                   a, ws, ws_bytes, st, out);
 }
 
 }  // namespace ds2
