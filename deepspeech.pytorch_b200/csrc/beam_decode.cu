@@ -661,14 +661,29 @@ beam_decode_grid_kernel(int B, int K, int T, int C, const float* __restrict__ pr
   }
 }
 
-size_t beam_workspace_bytes(int B, int T, int C, int beam_width, bool lm) {
-  (void)C;
+// The pools of `slots` CTAs at offset `off` of a workspace, each array 256-byte aligned:
+//   parent | label | ts | depth (slots*NP ints) | best (slots*NP doubles) | hkey | hval (slots*HC) | LM: lm (slots*NP)
+// With a null base only `off` advances.
+BeamPool carve_pool(void* base, size_t& off, int slots, int T, int W, bool lm) {
+  BeamPool pool;
+  pool_sizes(T, W, &pool.NP, &pool.HC);
+  const size_t n = (size_t)slots * pool.NP, h = (size_t)slots * pool.HC;
+  pool.parent = carve<int>(base, off, n * 4);
+  pool.label = carve<int>(base, off, n * 4);
+  pool.ts = carve<int>(base, off, n * 4);
+  pool.depth = carve<int>(base, off, n * 4);
+  pool.best = carve<double>(base, off, n * 8);
+  pool.hkey = carve<unsigned long long>(base, off, h * 8);
+  pool.hval = carve<int>(base, off, h * 4);
+  pool.lm = lm ? carve<double>(base, off, n * 8) : nullptr;
+  return pool;
+}
+
+size_t beam_workspace_bytes(int B, int T, int beam_width, bool lm) {
   if (B <= 0 || T <= 0 || beam_width <= 0) return 0;
-  long long NP, HC;
-  pool_sizes(T, beam_width, &NP, &HC);
-  const size_t n = (size_t)B * NP, h = (size_t)B * HC;
-  return 4 * align_up(n * 4, 256) + align_up(n * 8, 256) + align_up(h * 8, 256) + align_up(h * 4, 256) +
-         (lm ? align_up(n * 8, 256) : 0);
+  size_t off = 0;
+  carve_pool(nullptr, off, B, T, beam_width, lm);
+  return off;
 }
 
 // the checks every beam entry makes (DS2_REQUIRE returns from the caller's frame through this function's result)
@@ -694,25 +709,6 @@ int lm_check_args(const char* fn, int C, int blank, const void* lm, int lm_order
   return DS2_OK;
 }
 
-// the pools of `slots` CTAs, carved from the arena in the order beam_workspace_bytes counts them
-BeamPool take_pool(Arena& ar, int slots, int T, int W, bool lm) {
-  long long NP, HC;
-  pool_sizes(T, W, &NP, &HC);
-  const size_t n = (size_t)slots * NP, h = (size_t)slots * HC;
-  BeamPool pool;
-  pool.parent = ar.take<int>(n);
-  pool.label = ar.take<int>(n);
-  pool.ts = ar.take<int>(n);
-  pool.depth = ar.take<int>(n);
-  pool.best = ar.take<double>(n);
-  pool.hkey = ar.take<unsigned long long>(h);
-  pool.hval = ar.take<int>(h);
-  pool.lm = lm ? ar.take<double>(n) : nullptr;
-  pool.NP = NP;
-  pool.HC = HC;
-  return pool;
-}
-
 template <bool LM>
 int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
                        int beam_width, int cutoff_top_n, float cutoff_prob, BeamLm lm, int32_t* labels,
@@ -721,11 +717,10 @@ int beam_decode_launch(const char* fn, int B, int T, int C, const float* probs, 
   const int rc = beam_check_args(fn, B, T, C, blank, beam_width, cutoff_top_n, cutoff_prob);
   if (rc != DS2_OK) return rc;
   DS2_REQUIRE(probs && labels && timesteps && lengths && scores && n_beams, "%s: null pointer", fn);
-  const size_t need = beam_workspace_bytes(B, T, C, beam_width, LM);
+  size_t need = 0;
+  const BeamPool pool = carve_pool(workspace, need, B, T, beam_width, LM);
   DS2_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes,
               need);
-  Arena ar(workspace, workspace_bytes);
-  BeamPool pool = take_pool(ar, B, T, beam_width, LM);
   static DeviceOnce attr_once;
   if (attr_once.first()) {
     DS2_CHECK_CUDA(cudaFuncSetAttribute(beam_decode_kernel<LM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -757,11 +752,14 @@ long long grid_slots(long long items, int W, int C) {
   return resident < items ? resident : items;
 }
 
-size_t grid_workspace_bytes(int B, int T, int C, int W, int K) {
-  if (B <= 0 || T <= 0 || W <= 0 || C <= 0 || K <= 0) return 0;
-  const long long slots = grid_slots((long long)B * K, W, C);
-  if (slots <= 0) return 0;
-  return align_up((size_t)K * 2 * sizeof(double), 256) + beam_workspace_bytes((int)slots, T, C, W, true);
+// Workspace of the grid decode (bytes; with a base, also the addresses): the K (alpha, beta) pairs, 256-byte aligned,
+// then the pools of `slots` CTAs
+struct GridWs { double* pairs; BeamPool pool; };
+size_t grid_ws_carve(int K, int slots, int T, int W, void* base, GridWs& w) {
+  size_t off = 0;
+  w.pairs = carve<double>(base, off, (size_t)K * 2 * sizeof(double));
+  w.pool = carve_pool(base, off, slots, T, W, true);
+  return off;
 }
 
 }  // namespace
@@ -771,11 +769,11 @@ extern "C" {
 using namespace ds2;
 
 size_t ds2_beam_decode_workspace_bytes(int B, int T, int C, int beam_width) {
-  return beam_workspace_bytes(B, T, C, beam_width, false);
+  return beam_workspace_bytes(B, T, beam_width, false);
 }
 
 size_t ds2_beam_decode_lm_workspace_bytes(int B, int T, int C, int beam_width) {
-  return beam_workspace_bytes(B, T, C, beam_width, true);
+  return beam_workspace_bytes(B, T, beam_width, true);
 }
 
 int ds2_beam_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank, int beam_width,
@@ -806,7 +804,11 @@ int ds2_beam_decode_lm(int B, int T, int C, const float* probs, const int32_t* o
 }
 
 size_t ds2_beam_decode_lm_grid_workspace_bytes(int B, int T, int C, int beam_width, int K) {
-  return grid_workspace_bytes(B, T, C, beam_width, K);
+  if (B <= 0 || T <= 0 || beam_width <= 0 || C <= 0 || K <= 0) return 0;
+  const long long slots = grid_slots((long long)B * K, beam_width, C);
+  if (slots <= 0) return 0;
+  GridWs w;
+  return grid_ws_carve(K, (int)slots, T, beam_width, nullptr, w);
 }
 
 int ds2_beam_decode_lm_grid(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
@@ -826,13 +828,10 @@ int ds2_beam_decode_lm_grid(int B, int T, int C, const float* probs, const int32
                 "%s: pair %d: alpha=%g, beta=%g not finite", fn, k, pairs[2 * k], pairs[2 * k + 1]);
   const long long slots = grid_slots((long long)B * K, beam_width, C);
   DS2_REQUIRE(slots > 0, "%s: occupancy query failed", fn);
-  const size_t need = align_up((size_t)K * 2 * sizeof(double), 256) +
-                      beam_workspace_bytes((int)slots, T, C, beam_width, true);
+  GridWs G;
+  const size_t need = grid_ws_carve(K, (int)slots, T, beam_width, workspace, G);
   DS2_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes,
               need);
-  Arena ar(workspace, workspace_bytes);
-  double* pairs_d = ar.take<double>((size_t)K * 2);
-  BeamPool pool = take_pool(ar, (int)slots, T, beam_width, true);
   BeamLm L;
   L.tables = lm;
   L.order = lm_order;
@@ -840,10 +839,10 @@ int ds2_beam_decode_lm_grid(int B, int T, int C, const float* probs, const int32
   L.alpha = 0.0;
   L.beta = 0.0;
   cudaStream_t st = as_stream(stream);
-  DS2_CHECK_CUDA(cudaMemcpyAsync(pairs_d, pairs, (size_t)K * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
+  DS2_CHECK_CUDA(cudaMemcpyAsync(G.pairs, pairs, (size_t)K * 2 * sizeof(double), cudaMemcpyHostToDevice, st));
   DS2_PROF("beam_decode_lm_grid", st);
   DS2_LAUNCH(beam_decode_grid_kernel, (int)slots, BEAM_THREADS, dyn_smem_bytes(beam_width, C, true), st, B, K, T, C,
-             probs, out_len, blank, beam_width, cutoff_top_n, cutoff_prob, pairs_d, labels, lengths, pool, L);
+             probs, out_len, blank, beam_width, cutoff_top_n, cutoff_prob, G.pairs, labels, lengths, G.pool, L);
   return DS2_OK;
 }
 

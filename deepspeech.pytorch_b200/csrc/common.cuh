@@ -84,21 +84,6 @@ __device__ __forceinline__ int cdiv_dev(int a, int b) { return (a + b - 1) / b; 
 #endif
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-// Bump allocator over a caller-provided workspace.
-struct Arena {
-  char* base;
-  size_t cap, off;
-  Arena(void* p, size_t n) : base(static_cast<char*>(p)), cap(n), off(0) {}
-  template <typename T>
-  T* take(size_t count) {
-    size_t bytes = align_up(count * sizeof(T), 256);
-    if (off + bytes > cap) return nullptr;
-    T* r = reinterpret_cast<T*>(base + off);
-    off += bytes;
-    return r;
-  }
-};
-
 // The next `bytes` (256-aligned) of a workspace layout at offset `off`, or null when the base is null (sizing only)
 template <typename T>
 inline T* carve(void* base, size_t& off, size_t bytes) {

@@ -479,24 +479,22 @@ struct ConvWs {
   float* db_part;                  // conv bias gradients: per-block partial sums
   double* sums;   // 4 x 64 doubles: fwd stats 1, fwd stats 2, bwd sums 2, bwd sums 1
 };
-static size_t conv_ws_carve(int B, int T, void* base, ConvWs* w) {
+static size_t conv_ws_carve(int B, int T, void* base, ConvWs& w) {
   const size_t Tp = (size_t)(T - 1) / 2 + 1;
   size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off += align_up(bytes, 256); return base ? (char*)base + o : nullptr; };
-  float* p;
-  p = (float*)take((size_t)41 * 11 * CO * 4); if (w) w->wpk1 = p;
-  p = (float*)take((size_t)CO * 21 * 11 * CO * 4); if (w) w->wpk2 = p;
-  p = (float*)take((size_t)CO * 11 * 11 * CO * 4); if (w) w->wTe = p;
-  p = (float*)take((size_t)CO * 10 * 11 * CO * 4); if (w) w->wTo = p;
-  double* s = (double*)take(4 * 64 * sizeof(double)); if (w) w->sums = s;
-  p = (float*)take((size_t)B * CO * DS2_CONV2_D * Tp * 4); if (w) w->du2 = p;
-  p = (float*)take((size_t)B * CO * DS2_CONV1_D * Tp * 4); if (w) w->da1 = p;
-  p = (float*)take((size_t)21 * 352 * 32 * 4); if (w) w->taps_f = p;
-  p = (float*)take((size_t)21 * 352 * 32 * 4); if (w) w->taps_b = p;
-  p = (float*)take((size_t)B * CO * DS2_CONV1_D * Tp * 4); if (w) w->cl = p;
-  p = (float*)take((size_t)4 * B * CO * DS2_CONV1_D * (Tp + 4) * 4); if (w) w->shifted = p;
-  p = (float*)take(conv_wgrad_tc_partial_floats() * 4); if (w) w->wg_part = p;
-  p = (float*)take((size_t)CO * B * cdiv((long long)DS2_CONV1_D * Tp, 256) * 4); if (w) w->db_part = p;
+  w.wpk1 = carve<float>(base, off, (size_t)41 * 11 * CO * 4);
+  w.wpk2 = carve<float>(base, off, (size_t)CO * 21 * 11 * CO * 4);
+  w.wTe = carve<float>(base, off, (size_t)CO * 11 * 11 * CO * 4);
+  w.wTo = carve<float>(base, off, (size_t)CO * 10 * 11 * CO * 4);
+  w.sums = carve<double>(base, off, 4 * 64 * sizeof(double));
+  w.du2 = carve<float>(base, off, (size_t)B * CO * DS2_CONV2_D * Tp * 4);
+  w.da1 = carve<float>(base, off, (size_t)B * CO * DS2_CONV1_D * Tp * 4);
+  w.taps_f = carve<float>(base, off, (size_t)21 * 352 * 32 * 4);
+  w.taps_b = carve<float>(base, off, (size_t)21 * 352 * 32 * 4);
+  w.cl = carve<float>(base, off, (size_t)B * CO * DS2_CONV1_D * Tp * 4);
+  w.shifted = carve<float>(base, off, (size_t)4 * B * CO * DS2_CONV1_D * (Tp + 4) * 4);
+  w.wg_part = carve<float>(base, off, conv_wgrad_tc_partial_floats() * 4);
+  w.db_part = carve<float>(base, off, (size_t)CO * B * cdiv((long long)DS2_CONV1_D * Tp, 256) * 4);
   return off;
 }
 
@@ -507,7 +505,8 @@ using namespace ds2;
 
 size_t ds2_conv_frontend_workspace_bytes(int B, int T) {
   if (B <= 0 || T <= 0) return 0;
-  return conv_ws_carve(B, T, nullptr, nullptr) + 256;
+  ConvWs w;
+  return conv_ws_carve(B, T, nullptr, w) + 256;
 }
 
 int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, const float* w1, const float* b1,
@@ -520,7 +519,7 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
   cudaStream_t st = as_stream(stream);
   const int Tp = (T - 1) / 2 + 1, D1 = DS2_CONV1_D, D2 = DS2_CONV2_D, F = DS2_NUM_FREQ;
   ConvWs W;
-  conv_ws_carve(B, T, ws, &W);
+  conv_ws_carve(B, T, ws, W);
   DS2_PROF("conv_fwd", st);
   DS2_CHECK_CUDA(cudaMemsetAsync(W.sums, 0, 4 * 64 * sizeof(double), st));
   DS2_LAUNCH(pack_fwd_kernel, cdiv(41 * 11 * CO, 256), 256, 0, st, 1, 41, 11, w1, W.wpk1);
@@ -562,7 +561,7 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
   cudaStream_t st = as_stream(stream);
   const int Tp = (T - 1) / 2 + 1, D1 = DS2_CONV1_D, D2 = DS2_CONV2_D;
   ConvWs W;
-  conv_ws_carve(B, T, ws, &W);
+  conv_ws_carve(B, T, ws, W);
   double* s2 = W.sums + 128;
   double* s1 = W.sums + 192;
   DS2_PROF("conv_bwd", st);

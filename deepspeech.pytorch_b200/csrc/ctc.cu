@@ -207,18 +207,34 @@ __global__ void ctc_offsets_kernel(int B, const int32_t* __restrict__ tgt_len, l
   }
 }
 
+// Workspace of ds2_ctc_loss_fwd_bwd (bytes; with a base, also the addresses), each buffer 256-byte aligned:
+//   log-softmax lp (T,B,C) | alpha | beta (B,T,Smax) | their per-time scale offsets (B,T doubles each) |
+//   log-likelihood (B doubles) | target offsets (B)
+struct CtcWs {
+  float *lp, *alpha, *beta;
+  double *offs_a, *offs_b, *loglik;
+  long long* off;
+};
+static size_t ctc_ws_carve(int T, int B, int C, int max_tgt_len, void* base, CtcWs& w) {
+  const size_t TB = (size_t)T * B, Smax = 2 * (size_t)max_tgt_len + 1;
+  size_t off = 0;
+  w.lp = carve<float>(base, off, TB * C * 4);
+  w.alpha = carve<float>(base, off, TB * Smax * 4);
+  w.beta = carve<float>(base, off, TB * Smax * 4);
+  w.offs_a = carve<double>(base, off, TB * 8);
+  w.offs_b = carve<double>(base, off, TB * 8);
+  w.loglik = carve<double>(base, off, (size_t)B * 8);
+  w.off = carve<long long>(base, off, (size_t)B * 8);
+  return off;
+}
+
 }  // namespace ds2
 
 extern "C" {
 
 size_t ds2_ctc_workspace_bytes(int T, int B, int C, int max_tgt_len) {
-  size_t Smax = 2 * (size_t)max_tgt_len + 1;
-  size_t n = ds2::align_up((size_t)T * B * C * 4, 256)      // lp
-             + 2 * ds2::align_up((size_t)B * T * Smax * 4, 256)  // alpha, beta
-             + 2 * ds2::align_up((size_t)B * T * 8, 256)         // per-time scale offsets (double)
-             + ds2::align_up((size_t)B * 8, 256)                 // loglik (double)
-             + ds2::align_up((size_t)B * 8, 256);                // target offsets
-  return n;
+  ds2::CtcWs w;
+  return ds2::ctc_ws_carve(T, B, C, max_tgt_len, nullptr, w);
 }
 
 int ds2_ctc_loss_fwd_bwd(int T, int B, int C, const float* logits, const int64_t* targets, const int32_t* in_len,
@@ -226,35 +242,27 @@ int ds2_ctc_loss_fwd_bwd(int T, int B, int C, const float* logits, const int64_t
                          size_t ws_bytes, void* stream) {
   using namespace ds2;
   DS2_REQUIRE(T > 0 && B > 0 && C > 0 && max_tgt_len >= 0 && blank >= 0 && blank < C, "ds2_ctc: bad shape");
-  DS2_REQUIRE(ws_bytes >= ds2_ctc_workspace_bytes(T, B, C, max_tgt_len), "ds2_ctc: workspace too small");
+  CtcWs W;
+  const size_t need = ctc_ws_carve(T, B, C, max_tgt_len, ws, W);
+  DS2_REQUIRE(ws && ws_bytes >= need, "ds2_ctc: workspace null or too small (%zu < %zu bytes)", ws_bytes, need);
   cudaStream_t st = as_stream(stream);
   const int Smax = 2 * max_tgt_len + 1;
-  Arena ar(ws, ws_bytes);
-  float* lp = ar.take<float>((size_t)T * B * C);
-  float* alpha = ar.take<float>((size_t)B * T * Smax);
-  float* beta = ar.take<float>((size_t)B * T * Smax);
-  double* offs_a = ar.take<double>((size_t)B * T);
-  double* offs_b = ar.take<double>((size_t)B * T);
-  double* loglik = ar.take<double>(B);
-  long long* off = ar.take<long long>(B);
-  if (!lp || !alpha || !beta || !offs_a || !offs_b || !loglik || !off) { set_error("ds2_ctc: arena"); return DS2_ERR_WORKSPACE; }
-
   int rows = T * B;
   DS2_PROF("ctc", st);
-  DS2_LAUNCH(ctc_logsoftmax_kernel, cdiv(rows, 8), 256, 0, st, rows, C, logits, lp);
-  DS2_LAUNCH(ctc_offsets_kernel, 1, 32, 0, st, B, tgt_len, off);
+  DS2_LAUNCH(ctc_logsoftmax_kernel, cdiv(rows, 8), 256, 0, st, rows, C, logits, W.lp);
+  DS2_LAUNCH(ctc_offsets_kernel, 1, 32, 0, st, B, tgt_len, W.off);
   int threads = (Smax + 31) / 32 * 32;
   if (threads > 1024) threads = 1024;
   if (threads < 64) threads = 64;
   size_t smem = (size_t)Smax * 4 + 2 * ((size_t)Smax + 2) * 4;
   if (smem > 48 * 1024)
     DS2_CHECK_CUDA(cudaFuncSetAttribute(ctc_alpha_beta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  DS2_LAUNCH(ctc_alpha_beta_kernel, dim3(B, 2), threads, smem, st, T, B, C, Smax, lp, targets, in_len, tgt_len, blank,
-             alpha, beta, offs_a, offs_b, loglik);
+  DS2_LAUNCH(ctc_alpha_beta_kernel, dim3(B, 2), threads, smem, st, T, B, C, Smax, W.lp, targets, in_len, tgt_len,
+             blank, W.alpha, W.beta, W.offs_a, W.offs_b, W.loglik);
   const int wpb = 8;
   size_t smem3 = (size_t)wpb * ((C + 31) / 32 * 32) * 4;
-  DS2_LAUNCH(ctc_grad_kernel, cdiv((long long)T * B, wpb), wpb * 32, smem3, st, T, B, C, Smax, lp, targets, in_len,
-             tgt_len, off, blank, alpha, beta, offs_a, offs_b, loglik, nll, grad);
+  DS2_LAUNCH(ctc_grad_kernel, cdiv((long long)T * B, wpb), wpb * 32, smem3, st, T, B, C, Smax, W.lp, targets, in_len,
+             tgt_len, W.off, blank, W.alpha, W.beta, W.offs_a, W.offs_b, W.loglik, nll, grad);
   return DS2_OK;
 }
 

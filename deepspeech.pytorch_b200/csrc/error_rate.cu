@@ -219,11 +219,21 @@ size_t pm_global_blocks(int max_target_size) {
   return need > SH_BLOCKS ? (size_t)need : 0;
 }
 
-size_t error_counts_bytes(int K, int B, long long n_targets, int max_target_size) {
-  if (K <= 0 || B <= 0 || n_targets < 0) return 0;
-  const size_t n = (size_t)(n_targets > 0 ? n_targets : 1);
-  return align_up((size_t)B * 4 * 8, 256) + 4 * align_up(n * 4, 256) + align_up(n * 8, 256) +
-         align_up((size_t)K * B * 2 * pm_global_blocks(max_target_size) * 8, 256);
+// Workspace of ds2_error_counts (bytes; with a base, also the addresses), each buffer 256-byte aligned: the reference
+// tables, meta (B,4) | nb | chars | wstart | wlen | whash (n_targets each, at least 1) | only when a reference is
+// longer than the shared-memory blocks hold: the Myers bit vectors (K x B rows of 2 x pm_global_blocks)
+struct CountsWs { RefTables R; unsigned long long* pm; };
+size_t error_counts_carve(int K, int B, long long n_targets, int max_target_size, void* base, CountsWs& w) {
+  const size_t n = (size_t)(n_targets > 0 ? n_targets : 1), pm_blocks = pm_global_blocks(max_target_size);
+  size_t off = 0;
+  w.R.meta = carve<long long>(base, off, (size_t)B * 4 * 8);
+  w.R.nb = carve<int>(base, off, n * 4);
+  w.R.chars = carve<int>(base, off, n * 4);
+  w.R.wstart = carve<int>(base, off, n * 4);
+  w.R.wlen = carve<int>(base, off, n * 4);
+  w.R.whash = carve<unsigned long long>(base, off, n * 8);
+  w.pm = pm_blocks ? carve<unsigned long long>(base, off, (size_t)K * B * 2 * pm_blocks * 8) : nullptr;
+  return off;
 }
 
 }  // namespace
@@ -233,7 +243,9 @@ extern "C" {
 using namespace ds2;
 
 size_t ds2_error_counts_workspace_bytes(int K, int B, int64_t n_targets, int max_target_size) {
-  return error_counts_bytes(K, B, n_targets, max_target_size);
+  if (K <= 0 || B <= 0 || n_targets < 0) return 0;
+  CountsWs w;
+  return error_counts_carve(K, B, n_targets, max_target_size, nullptr, w);
 }
 
 int ds2_error_counts(int K, int B, int T, const int32_t* labels, const int32_t* lengths, const int64_t* targets,
@@ -246,26 +258,17 @@ int ds2_error_counts(int K, int B, int T, const int32_t* labels, const int32_t* 
   DS2_REQUIRE(n_targets >= 0 && max_target_size >= 0, "%s: n_targets=%lld, max_target_size=%d", fn,
               (long long)n_targets, max_target_size);
   DS2_REQUIRE(labels && lengths && target_sizes && (targets || n_targets == 0), "%s: null pointer", fn);
-  const size_t need = error_counts_bytes(K, B, n_targets, max_target_size);
+  CountsWs W;
+  const size_t need = error_counts_carve(K, B, n_targets, max_target_size, workspace, W);
   DS2_REQUIRE(workspace && workspace_bytes >= need, "%s: workspace too small (%zu < %zu bytes)", fn, workspace_bytes,
               need);
-  const size_t n = (size_t)(n_targets > 0 ? n_targets : 1);
   const int pm_blocks = (int)pm_global_blocks(max_target_size);
-  Arena ar(workspace, workspace_bytes);
-  RefTables R;
-  R.meta = ar.take<long long>((size_t)B * 4);
-  R.nb = ar.take<int>(n);
-  R.chars = ar.take<int>(n);
-  R.wstart = ar.take<int>(n);
-  R.wlen = ar.take<int>(n);
-  R.whash = ar.take<unsigned long long>(n);
-  unsigned long long* pm = pm_blocks ? ar.take<unsigned long long>((size_t)K * B * 2 * pm_blocks) : nullptr;
   cudaStream_t st = as_stream(stream);
   DS2_PROF("error_counts", st);
   DS2_LAUNCH(ref_prep_kernel, cdiv((long long)B, ER_WARPS), ER_THREADS, 0, st, B, targets, (long long)n_targets,
-             target_sizes, blank, space, R);
+             target_sizes, blank, space, W.R);
   DS2_LAUNCH(error_counts_kernel, cdiv((long long)K * B, ER_WARPS), ER_THREADS, 0, st, K, B, T, labels, lengths,
-             space, R, pm, pm_blocks, reinterpret_cast<long long*>(row_counts),
+             space, W.R, W.pm, pm_blocks, reinterpret_cast<long long*>(row_counts),
              reinterpret_cast<unsigned long long*>(pair_counts));
   return DS2_OK;
 }

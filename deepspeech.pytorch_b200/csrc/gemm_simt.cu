@@ -113,7 +113,7 @@ __global__ void sum_splits_kernel(int M, int N, int splits, const float* __restr
 static int simt_splits(int M, int N, int K, int* k_per_split) {
   const int tiles = cdiv(N, BN) * cdiv(M, BM);
   *k_per_split = K > 0 ? K : 1;
-  if (tiles >= 74 || K < 2048) return 1;
+  if (tiles <= 0 || tiles >= 74 || K < 2048) return 1;   // tiles <= 0: an empty C
   int splits = device_sm_count() / tiles;
   if (splits > K / 256) splits = K / 256;
   if (splits <= 1) return 1;

@@ -287,11 +287,19 @@ int transpose(int R, int C, const float* in, float* out, cudaStream_t st) {
 
 static inline size_t k4(int K) { return (size_t)((K + 3) / 4 * 4); }
 
+// Workspace of gemm_tc (bytes; with a base, also the addresses), each buffer 256-byte aligned: the K-major copy of an
+// operand stored the other way round, A^T (M,k4(K)) if transA | B^T (N,k4(K)) if !transB; null for the others.
+struct GemmTcWs { float *At, *Bt; };
+static size_t gemm_tc_ws_carve(int transA, int transB, int M, int N, int K, void* base, GemmTcWs& w) {
+  size_t off = 0;
+  w.At = transA ? carve<float>(base, off, (size_t)M * k4(K) * 4) : nullptr;
+  w.Bt = transB ? nullptr : carve<float>(base, off, (size_t)N * k4(K) * 4);
+  return off;
+}
+
 size_t gemm_tc_workspace_bytes(int transA, int transB, int M, int N, int K) {
-  size_t n = 0;
-  if (transA) n += align_up((size_t)M * k4(K) * 4, 256);
-  if (!transB) n += align_up((size_t)N * k4(K) * 4, 256);
-  return n;
+  GemmTcWs w;
+  return gemm_tc_ws_carve(transA, transB, M, N, K, nullptr, w);
 }
 
 static bool tc_eligible(int M, int N, int K) { return K >= 32 && M >= 32 && N >= 16 && (long long)M * N * K >= (1 << 18); }
@@ -322,29 +330,26 @@ static int launch_gemm_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, int M,
 }
 
 // TF32 wgmma reads both operands K-major: an operand stored the other way round (transA / !transB) is first
-// transposed into the workspace.
+// transposed into the workspace.  Without room for those copies the kernel declines.
 int gemm_tc(int transA, int transB, int M, int N, int K, float alpha, const float* A, int lda, const float* B,
             int ldb, float beta, float* C, int ldc, void* ws, size_t ws_bytes, cudaStream_t st) {
   if (!tc_eligible(M, N, K)) return 1;
-  Arena ar(ws, ws_bytes);
+  GemmTcWs W;
+  if (gemm_tc_ws_carve(transA, transB, M, N, K, ws, W) > (ws ? ws_bytes : 0)) return 1;
   const float* Ak = A;
   int ldak = lda;
   if (transA) {  // stored (K, M)
-    float* t = ar.take<float>((size_t)M * k4(K));
-    if (!t) return 1;
-    int rc = transpose_strided(K, M, A, (size_t)lda, t, k4(K), st);
+    int rc = transpose_strided(K, M, A, (size_t)lda, W.At, k4(K), st);
     if (rc) return rc;
-    Ak = t;
+    Ak = W.At;
     ldak = (int)k4(K);
   }
   const float* Bk = B;
   int ldbk = ldb;
   if (!transB) {  // stored (K, N)
-    float* t = ar.take<float>((size_t)N * k4(K));
-    if (!t) return 1;
-    int rc = transpose_strided(K, N, B, (size_t)ldb, t, k4(K), st);
+    int rc = transpose_strided(K, N, B, (size_t)ldb, W.Bt, k4(K), st);
     if (rc) return rc;
-    Bk = t;
+    Bk = W.Bt;
     ldbk = (int)k4(K);
   }
   if ((ldak & 3) || (ldbk & 3) || (reinterpret_cast<uintptr_t>(Ak) & 15) || (reinterpret_cast<uintptr_t>(Bk) & 15))

@@ -2,6 +2,8 @@
 // decode, and the fused clip + AdamW / SGD-Nesterov step on flat buffers.
 #include <math_constants.h>
 
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace ds2 {
@@ -224,6 +226,16 @@ __global__ void sgd_nesterov_kernel(int64_t n, float* __restrict__ p, const floa
   }
 }
 
+// Workspace of one pass of the fc head (bytes; with a base, also the addresses), each buffer 256-byte aligned: the
+// BatchNorm output, recomputed in bwd (rows,H) | its sums (4*H doubles fwd, 2*H bwd).  ds2_gemm gets the rest.
+struct FcWs { float* x; double* sums; };
+static size_t fc_ws_carve(int rows, int H, bool bwd, void* base, FcWs& w) {
+  size_t off = 0;
+  w.x = carve<float>(base, off, (size_t)rows * H * 4);
+  w.sums = carve<double>(base, off, (size_t)(bwd ? 2 : 4) * H * 8);
+  return off;
+}
+
 }  // namespace ds2
 
 extern "C" {
@@ -251,23 +263,27 @@ int ds2_lookahead_bwd(int T, int B, int H, int ctx, const float* x, const float*
 }
 
 size_t ds2_fc_head_workspace_bytes(int rows, int H, int C) {
-  return align_up((size_t)rows * H * 4, 256) + align_up((size_t)4 * H * 8, 256) +
-         ds2_gemm_workspace_bytes(1, 0, C, H, rows) + 4096;
+  FcWs w;
+  const size_t fwd = fc_ws_carve(rows, H, false, nullptr, w), bwd = fc_ws_carve(rows, H, true, nullptr, w);
+  // the most any ds2_gemm of the head needs: logits, dW, dX
+  const size_t gemm = std::max({ds2_gemm_workspace_bytes(0, 1, rows, C, H), ds2_gemm_workspace_bytes(1, 0, C, H, rows),
+                                ds2_gemm_workspace_bytes(0, 0, rows, H, C)});
+  return std::max(fwd, bwd) + gemm + 4096;
 }
 
 int ds2_fc_head_fwd(int rows, int H, int C, const float* x, const float* g, const float* b, float* rmean,
                     float* rvar, const float* w, int training, float momentum, float eps, int softmax,
                     float* logits, float* xhat, float* stats, void* ws, size_t ws_bytes, void* stream) {
   DS2_REQUIRE(rows > 0 && H > 0 && C > 0, "ds2_fc_head_fwd: bad shape");
-  DS2_REQUIRE(ws_bytes >= ds2_fc_head_workspace_bytes(rows, H, C), "ds2_fc_head_fwd: workspace too small");
+  DS2_REQUIRE(ws && ws_bytes >= ds2_fc_head_workspace_bytes(rows, H, C), "ds2_fc_head_fwd: workspace too small");
   cudaStream_t st = as_stream(stream);
-  Arena ar(ws, ws_bytes);
+  FcWs W;
+  const size_t used = fc_ws_carve(rows, H, false, ws, W);
   DS2_PROF("fc_fwd", st);
-  float* xbn = ar.take<float>((size_t)rows * H);
-  double* sums = ar.take<double>(4 * (size_t)H);
-  int r = bn_rows_fwd(rows, H, x, g, b, rmean, rvar, training, momentum, eps, xbn, xhat, stats, sums, st);
+  int r = bn_rows_fwd(rows, H, x, g, b, rmean, rvar, training, momentum, eps, W.x, xhat, stats, W.sums, st);
   if (r) return r;
-  r = ds2_gemm(0, 1, rows, C, H, 1.f, xbn, H, w, H, 0.f, logits, C, ar.base + ar.off, ar.cap - ar.off, stream);
+  r = ds2_gemm(0, 1, rows, C, H, 1.f, W.x, H, w, H, 0.f, logits, C, static_cast<char*>(ws) + used, ws_bytes - used,
+               stream);
   if (r) return r;
   if (softmax) DS2_LAUNCH(softmax_rows_kernel, cdiv(rows, 8), 256, 0, st, rows, C, logits);
   return DS2_OK;
@@ -277,14 +293,14 @@ int ds2_fc_head_bwd(int rows, int H, int C, const float* g, const float* b, cons
                     const float* stats, const float* dlogits, float* dx, float* dg, float* db, float* dw, void* ws,
                     size_t ws_bytes, void* stream) {
   DS2_REQUIRE(rows > 0 && H > 0 && C > 0, "ds2_fc_head_bwd: bad shape");
-  DS2_REQUIRE(ws_bytes >= ds2_fc_head_workspace_bytes(rows, H, C), "ds2_fc_head_bwd: workspace too small");
+  DS2_REQUIRE(ws && ws_bytes >= ds2_fc_head_workspace_bytes(rows, H, C), "ds2_fc_head_bwd: workspace too small");
   cudaStream_t st = as_stream(stream);
-  Arena ar(ws, ws_bytes);
+  FcWs W;
+  const size_t used = fc_ws_carve(rows, H, true, ws, W);
   DS2_PROF("fc_bwd", st);
-  float* tmp = ar.take<float>((size_t)rows * H);
-  double* sums = ar.take<double>(2 * (size_t)H);
-  void* gws = ar.base + ar.off;
-  size_t gws_bytes = ar.cap - ar.off;
+  float* tmp = W.x;
+  void* gws = static_cast<char*>(ws) + used;
+  const size_t gws_bytes = ws_bytes - used;
   size_t total = (size_t)rows * H;
   int blocks = (int)((total + 1023) / 1024);
   blocks = blocks > 132 * 16 ? 132 * 16 : blocks;
@@ -295,7 +311,7 @@ int ds2_fc_head_bwd(int rows, int H, int C, const float* g, const float* b, cons
   // dxbn = dlogits (rows x C) . W (C x H)
   r = ds2_gemm(0, 0, rows, H, C, 1.f, dlogits, C, w, H, 0.f, tmp, H, gws, gws_bytes, stream);
   if (r) return r;
-  return bn_rows_bwd(rows, H, xhat, g, stats, tmp, dx, dg, db, sums, st);
+  return bn_rows_bwd(rows, H, xhat, g, stats, tmp, dx, dg, db, W.sums, st);
 }
 
 int ds2_greedy_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank, int32_t* labels,
