@@ -3,9 +3,9 @@
 registers the package under that importable name)."""
 from . import _lib
 from ._lib import Ds2Error, get_lib
-from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, EvalConfig, InferenceConfig,
-                      LMConfig, ModelConfig, OptimConfig, OptimizerConfig, SGDConfig, SpectConfig, TranscribeConfig,
-                      UniDirectionalConfig)
+from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, DeepSpeechConfig, EvalConfig,
+                      InferenceConfig, LMConfig, ModelCheckpointConf, ModelConfig, OptimConfig, OptimizerConfig,
+                      SGDConfig, SpectConfig, TrainerConf, TranscribeConfig, UniDirectionalConfig)
 from .enums import DecoderType, RNNType, SpectrogramWindow
 from .labels import LABELS
 
@@ -29,3 +29,5 @@ from .inference import (ChunkSpectrogramParser, decode_results, load_audio, run_
 from .evaluation import (AudioDataLoader, SpectrogramDataset, error_counts, evaluate, load_model,  # noqa: E402
                          run_evaluation)
 from .lm_search import LMParamSearch, search_lm_params  # noqa: E402
+from .checkpoint import FileCheckpointHandler  # noqa: E402
+from .training import DSElasticDistributedSampler, DSRandomSampler, seed_everything, train  # noqa: E402

@@ -3,6 +3,7 @@ deepspeech_pytorch/configs/train_config.py:16-73, restated so that they are lega
 python >= 3.11 (the reference's mutable dataclass defaults at :41,:87-89 are not) and usable
 without hydra/omegaconf installed."""
 from dataclasses import dataclass, field
+from typing import Any, Optional
 
 from .enums import DecoderType, RNNType, SpectrogramWindow
 
@@ -136,6 +137,102 @@ class OptimizerConfig:
     spect_cfg: SpectConfig = field(default_factory=SpectConfig)
     seed: int = 0               # seed of the trial draws (numpy.random.default_rng)
     output_path: str = ''       # where to write [[alpha, beta, wer, cer], ...] (select_lm_params.py's input)
+
+
+@dataclass
+class ModelCheckpointConf:
+    """configs/lightning_config.py:6-22 (the settings of `FileCheckpointHandler`).  `every_n_train_steps`,
+    `train_time_interval`, `save_on_train_epoch_end` and `filepath` must keep their defaults: `train` raises
+    otherwise."""
+    _target_: str = "pytorch_lightning.callbacks.ModelCheckpoint"
+    filepath: Optional[str] = None
+    monitor: Optional[str] = None
+    verbose: bool = False
+    save_last: Optional[bool] = None
+    save_top_k: Optional[int] = 1
+    save_weights_only: bool = False
+    mode: str = "min"
+    dirpath: Any = None
+    filename: Optional[str] = None
+    auto_insert_metric_name: bool = True
+    every_n_train_steps: Optional[int] = None
+    train_time_interval: Optional[str] = None
+    every_n_epochs: Optional[int] = None
+    save_on_train_epoch_end: Optional[bool] = None
+
+
+@dataclass
+class TrainerConf:
+    """configs/lightning_config.py:25-78, the Lightning Trainer's arguments.  `train` honours max_epochs, min_epochs,
+    precision, gradient_clip_val, check_val_every_n_epoch, limit_train_batches, limit_val_batches,
+    log_every_n_steps, enable_checkpointing, default_root_dir and resume_from_checkpoint; it does not read
+    accelerator, devices, strategy, num_nodes (the process count comes from torchrun), logger, enable_progress_bar,
+    enable_model_summary, num_sanity_val_steps and benchmark; any other field away from its default raises."""
+    _target_: str = "pytorch_lightning.trainer.Trainer"
+    logger: Any = True
+    enable_checkpointing: bool = True
+    default_root_dir: Optional[str] = None
+    gradient_clip_val: float = 0
+    callbacks: Any = None
+    num_nodes: int = 1
+    num_processes: int = 1
+    gpus: Any = None
+    auto_select_gpus: bool = False
+    tpu_cores: Any = None
+    overfit_batches: Any = 0.0
+    track_grad_norm: Any = -1
+    check_val_every_n_epoch: int = 1
+    fast_dev_run: Any = False
+    accumulate_grad_batches: Any = 1
+    max_epochs: int = 1000
+    min_epochs: int = 1
+    limit_train_batches: Any = 1.0
+    limit_val_batches: Any = 1.0
+    limit_test_batches: Any = 1.0
+    val_check_interval: Any = 1.0
+    log_every_n_steps: int = 50
+    accelerator: Any = None
+    sync_batchnorm: bool = False
+    precision: int = 32
+    weights_save_path: Optional[str] = None
+    num_sanity_val_steps: int = 2
+    resume_from_checkpoint: Any = None
+    profiler: Any = None
+    benchmark: bool = False
+    deterministic: bool = False
+    auto_lr_find: Any = False
+    replace_sampler_ddp: bool = True
+    detect_anomaly: bool = False
+    auto_scale_batch_size: Any = False
+    plugins: Any = None
+    amp_backend: str = "native"
+    amp_level: Any = None
+    move_metrics_to_cpu: bool = False
+    gradient_clip_algorithm: Optional[str] = None
+    devices: Any = None
+    ipus: Optional[int] = None
+    enable_progress_bar: bool = True
+    max_time: Optional[str] = None
+    limit_predict_batches: float = 1.0
+    strategy: Optional[str] = None
+    enable_model_summary: bool = True
+    reload_dataloaders_every_n_epochs: int = 0
+    multiple_trainloader_mode: str = "max_size_cycle"
+
+
+@dataclass
+class DeepSpeechConfig:
+    """configs/train_config.py:81-91 (the settings of `train`).  Without hydra the defaults list (adam, bidirectional,
+    file checkpoint) becomes the field defaults.  As in the reference, the data loaders read `data.augmentation`;
+    the top-level `augmentation` is carried but unused."""
+    optim: Any = field(default_factory=AdamConfig)
+    model: Any = field(default_factory=BiDirectionalConfig)
+    checkpoint: ModelCheckpointConf = field(default_factory=ModelCheckpointConf)
+    trainer: TrainerConf = field(default_factory=TrainerConf)
+    data: DataConfig = field(default_factory=DataConfig)
+    augmentation: AugmentationConfig = field(default_factory=AugmentationConfig)
+    seed: int = 123456
+    load_auto_checkpoint: bool = False
 
 
 def cfg_type(cfg):

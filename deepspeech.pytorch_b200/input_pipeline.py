@@ -151,6 +151,9 @@ class SpectrogramBatcher:
         self.normalize = int(bool(normalize))
         self._stage = None          # pinned PCM staging buffer (grow-only)
         self._meta = None           # pinned int64 offsets + int32 rows
+        # recorded after the H2D copies out of _stage / _meta: the next call rewrites that pinned memory only once the
+        # copies have run, so a caller that does not synchronise (a training loop) can be at most one batch ahead
+        self._staged = None
 
     @staticmethod
     def order_and_frames(n_samples: Sequence[int], hop: int):
@@ -172,6 +175,8 @@ class SpectrogramBatcher:
         # drawn in the caller's (dataset) order, before the length sort: the reference augments in __getitem__
         draws = spec_augment_draws(frames, F) if aug else None
         total = sum(lens)
+        if self._staged is not None:
+            self._staged.synchronize()
         if self._stage is None or self._stage.numel() < total:
             self._stage = torch.empty(int(total * 1.25) + 1024, dtype=torch.float32).pin_memory()
         # int64 words: offsets (B + 1) | int32 rows (B) + int32 frames (B) | Ds2SpecAugDraws (8 words each)
@@ -199,6 +204,9 @@ class SpectrogramBatcher:
         with torch.cuda.device(dev):
             wave_d = self._stage[:total].to(dev, non_blocking=True)
             meta_d = self._meta[:n_meta].to(dev, non_blocking=True)
+            if self._staged is None:
+                self._staged = torch.cuda.Event()
+            self._staged.record()
             offs_d = meta_d[:B + 1]
             rows_d = meta_d[B + 1:2 * (B + 1)].view(torch.int32)[:B]
             out = torch.empty(B, 1, F, Tmax, device=dev)

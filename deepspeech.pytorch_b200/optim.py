@@ -87,3 +87,69 @@ class FusedOptimizer:
     def anneal(self):
         """ExponentialLR(gamma=learning_anneal) once per epoch (model.py:293-296)"""
         self.lr *= float(self.cfg.learning_anneal)
+
+    def torch_optimizer(self, params=None):
+        """the torch.optim.AdamW / SGD(nesterov=True) that `configure_optimizers` builds (model.py:273-291) over
+        `params` (default: the flat parameters, i.e. `model.parameters()` order), at the current learning rate and
+        without state"""
+        params = self.flat.params if params is None else list(params)
+        c = self.cfg
+        if self.adam:
+            opt = torch.optim.AdamW(params, lr=float(c.learning_rate), betas=tuple(c.betas), eps=float(c.eps),
+                                    weight_decay=float(c.weight_decay))
+        else:
+            opt = torch.optim.SGD(params, lr=float(c.learning_rate), momentum=float(c.momentum), nesterov=True,
+                                  weight_decay=float(c.weight_decay))
+        for g in opt.param_groups:
+            g["initial_lr"] = float(c.learning_rate)    # what ExponentialLR adds to the group
+            g["lr"] = self.lr
+        return opt
+
+    def state_dict(self):
+        """the state in torch.optim.AdamW / SGD's layout: per parameter index (model.parameters() order) `step` and
+        `exp_avg` / `exp_avg_sq` (AdamW) or `momentum_buffer` (SGD), and torch's `param_groups` with the current
+        `lr`.  The state tensors are views of the flat `m` / `v` buffers, not copies; a parameter has no state before
+        the first step, as in torch."""
+        groups = self.torch_optimizer().state_dict()["param_groups"]
+        state = {}
+        if self.step_count > 0:
+            for i, (p, o) in enumerate(zip(self.flat.params, self.flat.offsets)):
+                n = p.numel()
+                s = {"step": torch.tensor(float(self.step_count))}
+                if self.adam:
+                    s["exp_avg"] = self.m[o:o + n].view(p.shape)
+                    s["exp_avg_sq"] = self.v[o:o + n].view(p.shape)
+                else:
+                    s["momentum_buffer"] = self.m[o:o + n].view(p.shape)
+                state[i] = s
+        return {"state": state, "param_groups": groups}
+
+    def load_state_dict(self, sd):
+        """the inverse of `state_dict` (also accepts what torch.optim.AdamW / SGD saved over the same parameters):
+        copies the moments into the flat buffers and restores the step count and the learning rate"""
+        params = self.flat.params
+        if len(sd["param_groups"]) != 1 or len(sd["param_groups"][0]["params"]) != len(params):
+            raise ValueError(f"optimizer state for {[len(g['params']) for g in sd['param_groups']]} parameters, "
+                             f"this optimizer has one group of {len(params)}")
+        keys = ("exp_avg", "exp_avg_sq") if self.adam else ("momentum_buffer",)
+        bufs = (self.m, self.v) if self.adam else (self.m,)
+        state = sd["state"]
+        steps = set()
+        for b in bufs:
+            b.zero_()
+        for i, (p, o) in enumerate(zip(params, self.flat.offsets)):
+            s = state.get(i)
+            if s is None:
+                continue
+            for k, b in zip(keys, bufs):
+                t = s[k]
+                if t.numel() != p.numel():
+                    raise ValueError(f"optimizer state {i}.{k}: {tuple(t.shape)} for a parameter of {tuple(p.shape)}")
+                b[o:o + p.numel()].copy_(t.reshape(-1))
+            if "step" in s:
+                steps.add(int(float(s["step"])))
+        if len(steps) > 1:
+            raise ValueError(f"optimizer state: parameters at different step counts {sorted(steps)}")
+        # torch's SGD keeps no step count: a momentum buffer means at least one step has been taken
+        self.step_count = steps.pop() if steps else (1 if state else 0)
+        self.lr = float(sd["param_groups"][0]["lr"])
