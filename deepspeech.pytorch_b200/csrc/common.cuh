@@ -32,6 +32,13 @@ struct DeviceOnce {
 };
 int device_sm_count();   // SM count of the current device (cached per device)
 
+// A row class of the tensor-core 32->32 convolution (conv_tc_run in conv_tc.cu): its output rows d in [0, R_out) read
+// the vertical taps j in [0, J), input row row_mul * d + row_off + j * row_step with tap matrix w_off + j * w_step, and
+// land in output row out_row_mul * d + out_row_off.  The forward is one class; the data gradient two (even / odd rows).
+struct ConvRows {
+  int R_out, J, row_off, w_off, out_row_off;
+};
+
 // A tensor-core-mode call that had to take the one-launch-per-time-step FFMA kernels (shape not eligible for the
 // persistent sweeps): counted and reported once per shape on stderr, never silent.
 void note_fallback(const char* what, int rnn, int T, int B, int H, int D);

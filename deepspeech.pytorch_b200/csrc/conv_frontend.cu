@@ -459,10 +459,9 @@ static int launch_conv(const float* in, int B, int Cin, int Hin, int Win, const 
 }
 
 // tensor-core 32->32 convolution (conv_tc.cu)
-int conv_tc_run(const float* in_cl, int B, int T, int R_in, int R_out, const float* taps, int n_taps, int J,
-                int row_mul, int row_off, int row_step, int w_off, int w_step, float* out, size_t ob, size_t oc,
-                size_t orow, int out_row_mul, int out_row_off, const float* bias, const int32_t* out_len,
-                double* stat_sums, cudaStream_t st);
+int conv_tc_run(const float* in_cl, int B, int T, int R_in, const float* taps, int n_taps, int row_mul, int row_step,
+                int w_step, int out_row_mul, const ConvRows* rows, int n_classes, float* out, size_t ob, size_t oc,
+                size_t orow, const float* bias, const int32_t* out_len, double* stat_sums, cudaStream_t st);
 int nchw_to_cl(int B, int R, int T, const float* in, float* out, cudaStream_t st);
 int pack_conv2_tc(const float* w2, float* wn_fwd, float* wd_bwd, cudaStream_t st);
 int conv2_wgrad_tc(const float* dz2, const float* a1, float* a1_shifted, float* part, int B, int T, float* dw2,
@@ -536,8 +535,9 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
     if (rc) return rc;
     rc = pack_conv2_tc(w2, W.taps_f, nullptr, st);
     if (rc) return rc;
-    rc = conv_tc_run(W.cl, B, Tp, D1, D2, W.taps_f, 21, 21, 2, -10, 1, 0, 1, z2, (size_t)CO * D2 * Tp, (size_t)D2 * Tp,
-                     (size_t)Tp, 1, 0, b2, out_len, training ? W.sums + 64 : nullptr, st);
+    const ConvRows rows = {D2, 21, -10, 0, 0};
+    rc = conv_tc_run(W.cl, B, Tp, D1, W.taps_f, 21, 2, 1, 1, 1, &rows, 1, z2, (size_t)CO * D2 * Tp, (size_t)D2 * Tp,
+                     (size_t)Tp, b2, out_len, training ? W.sums + 64 : nullptr, st);
   } else {
     rc = launch_conv<21, 11, 2, 1>(a1, B, CO, D1, Tp, W.wpk2, b2, z2, D2, Tp, (size_t)CO * D2 * Tp, (size_t)D2 * Tp,
                                    (size_t)Tp, 10, 5, out_len, training ? W.sums + 64 : nullptr, st);
@@ -613,11 +613,9 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
     if (rc) return rc;
     rc = pack_conv2_tc(w2, nullptr, W.taps_b, st);
     if (rc) return rc;
-    rc = conv_tc_run(W.cl, B, Tp, D2, 41, W.taps_b, 21, 11, 1, 5, -1, 0, 2, W.da1, ob, oc, (size_t)Tp, 2, 0, nullptr,
-                     nullptr, nullptr, st);
-    if (rc) return rc;
-    rc = conv_tc_run(W.cl, B, Tp, D2, 40, W.taps_b, 21, 10, 1, 5, -1, 1, 2, W.da1, ob, oc, (size_t)Tp, 2, 1, nullptr,
-                     nullptr, nullptr, st);
+    const ConvRows rows[2] = {{41, 11, 5, 0, 0}, {40, 10, 5, 1, 1}};
+    rc = conv_tc_run(W.cl, B, Tp, D2, W.taps_b, 21, 1, -1, 2, 2, rows, 2, W.da1, ob, oc, (size_t)Tp, nullptr, nullptr,
+                     nullptr, st);
     if (rc) return rc;
   } else {
     rc = launch_conv<11, 11, 1, 1>(W.du2, B, CO, D2, Tp, W.wTe, nullptr, W.da1, 41, Tp, ob, oc, (size_t)2 * Tp, 5, 5,

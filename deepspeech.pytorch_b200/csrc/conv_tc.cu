@@ -9,13 +9,14 @@
 // The A tile of a tap is ONE contiguous TMA box (64 positions x 32 channels = 128-byte rows, 128B
 // swizzle, out-of-range rows / positions zero-filled by TMA = the convolution padding), the B tile is
 // the packed tap matrix (352 x 32); no descriptor tricks, no im2col buffer.  A tile produces 54
-// outputs (64 positions minus the 10-position halo).  Two MMA warpgroups own one N = 176 half each
-// (88 accumulator registers per thread); their epilogue adds every accumulator at row p-kw into a
-// shared-memory output tile, then bias, length mask, NCHW store and the BatchNorm sum / sum-of-squares
-// partials of the forward pass.
+// outputs (64 positions minus the 10-position halo).  The kernel is persistent with two MMA warpgroups
+// that take turns (see conv_tc_kernel); a warpgroup holds a whole tile's 64 x 352 accumulator (176
+// registers per thread), and its epilogue adds every accumulator at row p-kw into its own shared-memory
+// output tile, then bias, length mask, NCHW store and the BatchNorm sum / sum-of-squares partials of the
+// forward pass.
 //
-// The data gradient of the stride-(2,1) convolution is the same kernel run twice (even / odd output
-// rows) with transposed, horizontally flipped taps (see pack kernels below).
+// The data gradient of the stride-(2,1) convolution is the same kernel over two row classes (even / odd
+// output rows) with transposed, horizontally flipped taps (see pack kernels below), in one launch.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -32,9 +33,13 @@ constexpr int A_BYTES = MP * 128;                   // 8 KB
 constexpr int W_HALF = (NN / 2) * 128;              // 176 rows x 128 B = 22528
 constexpr int STAGE_BYTES = A_BYTES + 2 * W_HALF;   // 53248
 constexpr int STAGES = 3;
-constexpr int OUT_LD = 33;
+constexpr int OUT_LD = 33, OUT_FLOATS = TO * OUT_LD;
 constexpr int THREADS = 384;                        // warp 0 TMA producer, warps 4..11 two MMA warpgroups
-constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + (TO + 10) * OUT_LD * 4 + 256;
+// registers per thread after the producer warpgroup hands its surplus to the MMA warpgroups (128 x 40 + 256 x 232 =
+// 384 x 168): an MMA warpgroup holds 176 fp32 accumulators
+constexpr int PRODUCER_REGS = 40, MMA_REGS = 232;
+constexpr int ORDER_BAR = 1, EPI_BAR = 3;           // named barriers: + warpgroup (0 is __syncthreads)
+constexpr int SMEM_BYTES = 1024 + STAGES * STAGE_BYTES + 2 * OUT_FLOATS * 4 + 256;
 }  // namespace cv
 
 // Warp-converged TMA issue (see tc_common.cuh): 4-D / 5-D boxes of the conv kernels
@@ -60,123 +65,173 @@ __device__ __forceinline__ void tma_load_5d_w(void* dst, const CUtensorMap* m, u
 struct ConvTcParams {
   CUtensorMap tmA;   // 4-D (32 c, T, R_in, B) channels-last input
   CUtensorMap tmW;   // 3-D (32 c, 352 n, taps) packed tap matrices
-  int B, T, R_in, R_out;
-  int J;                                   // vertical taps per output row
-  int row_mul, row_off, row_step;          // input row  = row_mul * d + row_off + j * row_step
-  int w_off, w_step;                       // tap matrix = w_off + j * w_step
+  int B, T, R_in;
+  int ntt;                                 // time tiles per output row
+  ConvRows rows[2];
+  int tiles0, tiles;                       // tiles of class 0, of both classes
+  int row_mul, row_step, w_step, out_row_mul;
   float* out;                              // out[b*ob + c*oc + (out_row_mul*d + out_row_off)*orow + t]
   size_t ob, oc, orow;
-  int out_row_mul, out_row_off;
   const float* bias;                       // [32] or null
   const int32_t* out_len;                  // [B] or null: positions t >= out_len[b] are written as 0
   double* stat_sums;                       // [64] or null
 };
 
+// Tile u of the list: class 0's tiles, then class 1's, each ordered (b, d, time tile) with the time tile fastest.
+struct ConvTile {
+  int t0, d, b, cls, j_lo, nj;
+};
+__device__ __forceinline__ ConvTile conv_tile(const ConvTcParams& p, int u) {
+  ConvTile t;
+  t.cls = u >= p.tiles0;
+  if (t.cls) u -= p.tiles0;
+  const ConvRows& rc = p.rows[t.cls];
+  t.t0 = (u % p.ntt) * cv::TO;
+  u /= p.ntt;
+  t.d = u % rc.R_out;
+  t.b = u / rc.R_out;
+  // vertical taps whose input row exists (the others contribute zeros: skip them)
+  int j_lo = 0, j_hi = rc.J;
+  const int r0 = p.row_mul * t.d + rc.row_off;
+  while (j_lo < j_hi && (r0 + j_lo * p.row_step < 0 || r0 + j_lo * p.row_step >= p.R_in)) ++j_lo;
+  while (j_hi > j_lo && (r0 + (j_hi - 1) * p.row_step < 0 || r0 + (j_hi - 1) * p.row_step >= p.R_in)) --j_hi;
+  t.j_lo = j_lo;
+  t.nj = j_hi - j_lo;
+  return t;
+}
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// Persistent: CTA c takes the tiles c, c + gridDim.x, ...  Warp 0 streams their stages through the ring in that order;
+// MMA warpgroup k takes the CTA's tiles k, k + 2, ... and computes all N = 352 columns of each (two m64n176 per
+// k-step).  The two warpgroups issue their tiles' MMAs in turn (named barriers ORDER_BAR + k), so the ring is consumed
+// in the order it was filled; a warpgroup that has issued its tile's MMAs hands the turn over and runs that tile's
+// epilogue in its own out_s while the other warpgroup's MMAs keep the tensor cores busy.
 __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   using namespace cv;
   using namespace tc;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* out_s = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);       // [TO+10][33]
-  uint64_t* full = reinterpret_cast<uint64_t*>(out_s + (TO + 10) * OUT_LD);   // 64*33 floats: 8-byte aligned
+  float* out_s0 = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [2 warpgroups][TO][33]
+  uint64_t* full = reinterpret_cast<uint64_t*>(out_s0 + 2 * OUT_FLOATS);   // 8-byte aligned
   uint64_t* empty = full + STAGES;
 
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const int t0 = blockIdx.x * TO, d = blockIdx.y, b = blockIdx.z;
-
-  // vertical taps whose input row exists (the others contribute zeros: skip them)
-  int j_lo = 0, j_hi = p.J;
-  {
-    const int r0 = p.row_mul * d + p.row_off;
-    while (j_lo < j_hi && (r0 + j_lo * p.row_step < 0 || r0 + j_lo * p.row_step >= p.R_in)) ++j_lo;
-    while (j_hi > j_lo && (r0 + (j_hi - 1) * p.row_step < 0 || r0 + (j_hi - 1) * p.row_step >= p.R_in)) --j_hi;
-  }
-  const int nj = j_hi - j_lo;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmA);
     tma_prefetch_desc(&p.tmW);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // two MMA warpgroups
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }   // one consumer per stage
     fence_barrier_init();
   }
-  for (int i = threadIdx.x; i < (TO + 10) * OUT_LD; i += THREADS) out_s[i] = 0.f;
   __syncthreads();
 
-  if (warp == 0) {
-    int s = 0;
-    uint32_t ph = 0;
-    for (int jj = 0; jj < nj; ++jj) {
-      const int j = j_lo + jj;
-      const int r = p.row_mul * d + p.row_off + j * p.row_step;
-      const int wi = p.w_off + j * p.w_step;
-      mbar_wait(&empty[s], ph ^ 1);
-      mbar_arrive_expect_tx_w(&full[s], (uint32_t)STAGE_BYTES);
-      uint8_t* st = smem + s * STAGE_BYTES;
-      // A: 64 positions starting at t0-5 (negative / beyond-T coordinates are zero-filled = padding)
-      tma_load_4d_w(st, &p.tmA, &full[s], 0, t0 - 5, r, b);
-      tma_load_3d_w(st + A_BYTES, &p.tmW, &full[s], 0, 0, wi);
-      tma_load_3d_w(st + A_BYTES + W_HALF, &p.tmW, &full[s], 0, NN / 2, wi);
-      if (++s == STAGES) { s = 0; ph ^= 1; }
+  if (warp < 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 0) {
+      int g = 0;                                      // stages issued by this CTA so far
+      for (int u = blockIdx.x; u < p.tiles; u += gridDim.x) {
+        const ConvTile t = conv_tile(p, u);
+        const ConvRows& rc = p.rows[t.cls];
+        for (int jj = 0; jj < t.nj; ++jj, ++g) {
+          const int j = t.j_lo + jj;
+          const int r = p.row_mul * t.d + rc.row_off + j * p.row_step;
+          const int wi = rc.w_off + j * p.w_step;
+          const int s = g % STAGES;
+          mbar_wait(&empty[s], ((g / STAGES) & 1) ^ 1);
+          mbar_arrive_expect_tx_w(&full[s], (uint32_t)STAGE_BYTES);
+          uint8_t* st = smem + s * STAGE_BYTES;
+          // A: 64 positions starting at t0-5 (negative / beyond-T coordinates are zero-filled = padding)
+          tma_load_4d_w(st, &p.tmA, &full[s], 0, t.t0 - 5, r, t.b);
+          tma_load_3d_w(st + A_BYTES, &p.tmW, &full[s], 0, 0, wi);
+          tma_load_3d_w(st + A_BYTES + W_HALF, &p.tmW, &full[s], 0, NN / 2, wi);
+        }
+      }
     }
-  } else if (warp >= 4 && nj > 0) {
-    const int wg = warp / 4 - 1;                      // N half: columns 176 wg .. 176 wg + 175
-    float acc[NN / 4];
+    return;
+  }
+
+  setmaxnreg_inc<MMA_REGS>();
+  const int wg = warp / 4 - 1, w = warp % 4;
+  const bool leader = (threadIdx.x & 127) == 0;
+  float* out_s = out_s0 + wg * OUT_FLOATS;
+  int g = 0;                                          // stages of this CTA's earlier tiles (both warpgroups)
+  int i = 0;                                          // index of the tile among the CTA's tiles
+  for (int u = blockIdx.x; u < p.tiles; u += gridDim.x, ++i) {
+    const ConvTile t = conv_tile(p, u);
+    if ((i & 1) != wg) {
+      g += t.nj;
+      continue;
+    }
+    if (i > 0) named_bar_sync(ORDER_BAR + wg, 256);   // the other warpgroup has issued the previous tile's MMAs
+    float acc[NN / 2];                                // columns 0..175 in acc[0..87], 176..351 in acc[88..175]
 #pragma unroll
-    for (int i = 0; i < NN / 4; ++i) acc[i] = 0.f;
-    int s = 0;
-    uint32_t ph = 0;
-    for (int jj = 0; jj < nj; ++jj) {
-      mbar_wait(&full[s], ph);
+    for (int k = 0; k < NN / 2; ++k) acc[k] = 0.f;
+    // one wgmma group stays in flight: stage g is released once stage g + 1's group is issued and g's has completed
+    for (int jj = 0; jj < t.nj; ++jj, ++g) {
+      const int s = g % STAGES;
+      mbar_wait(&full[s], (g / STAGES) & 1);
       const uint64_t ad = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES));
-      const uint64_t bd = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES + wg * W_HALF));
+      const uint64_t bd = smem_desc_sw128(smem_u32(smem + s * STAGE_BYTES + A_BYTES));
       wg_fence();
 #pragma unroll
-      for (int k = 0; k < 4; ++k) Wgmma<NN / 2, false>::mma(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1u);
-      wg_release(&empty[s]);
-      if (++s == STAGES) { s = 0; ph ^= 1; }
+      for (int k = 0; k < 4; ++k) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)   // N half h: the B tile's rows 176 h .. 176 h + 175
+          Wgmma<NN / 2, false>::mma(acc + (NN / 4) * h, ad + (uint64_t)(2 * k),
+                                    bd + (uint64_t)(W_HALF / 16 * h + 2 * k), 1u);
+      }
+      wg_commit();
+      wg_wait<1>();
+      if (jj > 0 && leader) mbar_arrive(&empty[(g - 1) % STAGES]);
     }
-    // accumulator (position pl, column (kw, co)) feeds output pl - kw.  One kw at a time (the two warpgroups hold
-    // different column blocks; inside a block every output has one contributor): the sum over kw always runs in the
-    // same order, so the result is bit-repeatable.
-    // The 8-column block i of warpgroup wg holds tap column kw = (22 wg + i) / 4 (a block never straddles two taps), so
-    // with kw and i unrolled each pass touches only the (at most 4) blocks of its own tap instead of testing all 88
-    // accumulators: the epilogue runs while the tensor cores of the SM idle, so its instruction count is paid per CTA.
-    const int w = warp % 4;
+    if (u + (int)gridDim.x < p.tiles) named_bar_arrive(ORDER_BAR + (wg ^ 1), 256);   // the next tile's turn
+    wg_wait<0>();
+    if (t.nj > 0 && leader) mbar_arrive(&empty[(g - 1) % STAGES]);
+
+    // accumulator (position pl, column (kw, co)) feeds output pl - kw.  One kw at a time (inside a pass every output
+    // has one contributor), starting from 0: the sum over kw always runs in the same order, so the result is
+    // bit-repeatable.
+    // The 8-column block i holds tap column kw = i / 4, so with kw and i unrolled each pass touches only the 4 blocks
+    // of its own tap.
+    named_bar_sync(EPI_BAR + wg, 128);                // this warpgroup's previous tile has been stored from out_s
 #pragma unroll
     for (int kw = 0; kw < KW; ++kw) {
 #pragma unroll
-      for (int i = 0; i < NN / 16; ++i) {
-        const bool in0 = (i >> 2) == kw, in1 = ((NN / 16 + i) >> 2) == kw;   // block i of warpgroup 0 / 1 is tap kw
-        if (!in0 && !in1) continue;
-        if (wg == 0 ? !in0 : !in1) continue;
+      for (int ib = 4 * kw; ib < 4 * kw + 4; ++ib) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
           const int pl = 16 * w + (lane >> 2) + 8 * (e >> 1);
-          const int n = NN / 2 * wg + 8 * i + 2 * (lane & 3) + (e & 1);
+          const int co = 8 * (ib % 4) + 2 * (lane & 3) + (e & 1);
           const int to = pl - kw;
-          if (to >= 0 && to < TO) out_s[to * OUT_LD + n % CH] += acc[4 * i + e];
+          if (to >= 0 && to < TO) {
+            float* o = out_s + to * OUT_LD + co;
+            *o = (kw == 0 ? 0.f : *o) + acc[4 * ib + e];
+          }
         }
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+      named_bar_sync(EPI_BAR + wg, 128);
     }
-  }
-  __syncthreads();
-  if (warp >= 4 && warp < 8) {
-    // bias, mask, NCHW store: warp q owns channels 8q..8q+7, lanes run along time;
+
+    // bias, mask, NCHW store: warp w owns channels 8w..8w+7, lanes run along time;
     // per-channel sum / sum of squares for the BatchNorm of the forward pass
-    const int q = warp % 4;
-    const int L = p.out_len ? p.out_len[b] : p.T;
-    const int orow_idx = p.out_row_mul * d + p.out_row_off;
+    const int L = p.out_len ? p.out_len[t.b] : p.T;
+    const int orow_idx = p.out_row_mul * t.d + p.rows[t.cls].out_row_off;
     for (int cc = 0; cc < 8; ++cc) {
-      const int c = q * 8 + cc;
+      const int c = w * 8 + cc;
       const float bv = p.bias ? p.bias[c] : 0.f;
-      float* op = p.out + (size_t)b * p.ob + (size_t)c * p.oc + (size_t)orow_idx * p.orow;
+      float* op = p.out + (size_t)t.b * p.ob + (size_t)c * p.oc + (size_t)orow_idx * p.orow;
       float s1 = 0.f, s2 = 0.f;
       for (int to = lane; to < TO; to += 32) {
-        const int t = t0 + to;
-        if (t < p.T) {
-          const float val = (t < L) ? out_s[to * OUT_LD + c] + bv : 0.f;
-          op[t] = val;
+        const int tt = t.t0 + to;
+        if (tt < p.T) {
+          const float val = (tt < L) ? out_s[to * OUT_LD + c] + bv : 0.f;
+          op[tt] = val;
           s1 += val;
           s2 = fmaf(val, val, s2);
         }
@@ -241,26 +296,32 @@ int pack_conv2_tc(const float* w2, float* wn_fwd, float* wd_bwd, cudaStream_t st
 // 4-D channels-last tensor map (32 c, T, R, B), box (32, 128, 1, 1)
 static int make_tmap_cl(CUtensorMap* out, const float* base, int T, int R, int B);
 
-// Runs the 32->32 tap-in-N convolution.  in_cl: (B, R_in, T, 32) channels-last; taps: (n_taps, 352, 32).
-int conv_tc_run(const float* in_cl, int B, int T, int R_in, int R_out, const float* taps, int n_taps, int J,
-                int row_mul, int row_off, int row_step, int w_off, int w_step, float* out, size_t ob, size_t oc,
-                size_t orow, int out_row_mul, int out_row_off, const float* bias, const int32_t* out_len,
-                double* stat_sums, cudaStream_t st) {
+// Runs the 32->32 tap-in-N convolution over one or two row classes in one launch.  in_cl: (B, R_in, T, 32)
+// channels-last; taps: (n_taps, 352, 32).
+int conv_tc_run(const float* in_cl, int B, int T, int R_in, const float* taps, int n_taps, int row_mul, int row_step,
+                int w_step, int out_row_mul, const ConvRows* rows, int n_classes, float* out, size_t ob, size_t oc,
+                size_t orow, const float* bias, const int32_t* out_len, double* stat_sums, cudaStream_t st) {
   ConvTcParams p{};
   int rc = make_tmap_cl(&p.tmA, in_cl, T, R_in, B);
   if (rc) return rc;
   rc = make_tmap_3d(&p.tmW, taps, 32, cv::NN, n_taps, 32, (size_t)32 * cv::NN, 32, cv::NN / 2, 1);
   if (rc) return rc;
-  p.B = B; p.T = T; p.R_in = R_in; p.R_out = R_out; p.J = J;
-  p.row_mul = row_mul; p.row_off = row_off; p.row_step = row_step; p.w_off = w_off; p.w_step = w_step;
-  p.out = out; p.ob = ob; p.oc = oc; p.orow = orow; p.out_row_mul = out_row_mul; p.out_row_off = out_row_off;
+  p.B = B; p.T = T; p.R_in = R_in; p.ntt = cdiv(T, cv::TO);
+  p.tiles = 0;
+  for (int c = 0; c < n_classes; ++c) {
+    p.rows[c] = rows[c];
+    p.tiles += p.ntt * rows[c].R_out * B;
+    if (c == 0) p.tiles0 = p.tiles;
+  }
+  p.row_mul = row_mul; p.row_step = row_step; p.w_step = w_step; p.out_row_mul = out_row_mul;
+  p.out = out; p.ob = ob; p.oc = oc; p.orow = orow;
   p.bias = bias; p.out_len = out_len; p.stat_sums = stat_sums;
   static DeviceOnce attr_once;
   if (attr_once.first()) {
     DS2_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cv::SMEM_BYTES));
     attr_once.done();
   }
-  dim3 grid(cdiv(T, cv::TO), R_out, B);
+  const int grid = p.tiles < device_sm_count() ? p.tiles : device_sm_count();   // persistent: at most one CTA per SM
   DS2_LAUNCH(conv_tc_kernel, grid, cv::THREADS, cv::SMEM_BYTES, st, p);
   return DS2_OK;
 }
