@@ -3,7 +3,7 @@
 registers the package under that importable name)."""
 from . import _lib
 from ._lib import Ds2Error, get_lib
-from .configs import (AdamConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, DeepSpeechConfig, EvalConfig,
+from .configs import (AdamConfig, AlignConfig, AugmentationConfig, BiDirectionalConfig, DataConfig, DeepSpeechConfig, EvalConfig,
                       InferenceConfig, LMConfig, ModelCheckpointConf, ModelConfig, OptimConfig, OptimizerConfig,
                       SGDConfig, SpectConfig, TrainerConf, TranscribeConfig, UniDirectionalConfig)
 from .enums import DecoderType, RNNType, SpectrogramWindow
@@ -31,3 +31,4 @@ from .evaluation import (AudioDataLoader, SpectrogramDataset, error_counts, eval
 from .lm_search import LMParamSearch, search_lm_params  # noqa: E402
 from .checkpoint import FileCheckpointHandler  # noqa: E402
 from .training import DSElasticDistributedSampler, DSRandomSampler, seed_everything, train  # noqa: E402
+from .alignment import align_audio, align_manifest, forced_align  # noqa: E402

@@ -47,6 +47,8 @@ PROTOTYPES = {
     "ds2_fc_head_bwd": (i32, [i32, i32, i32] + [vp] * 11 + [sz, vp]),
     "ds2_ctc_workspace_bytes": (sz, [i32, i32, i32, i32]),
     "ds2_ctc_loss_fwd_bwd": (i32, [i32, i32, i32] + [vp] * 4 + [i32, i32] + [vp] * 3 + [sz, vp]),
+    "ds2_ctc_align_workspace_bytes": (sz, [i32, i32, i32, i32]),
+    "ds2_ctc_align": (i32, [i32, i32, i32, vp, i32] + [vp] * 3 + [i32, i32] + [vp] * 5 + [sz, vp]),
     "ds2_greedy_decode": (i32, [i32, i32, i32, vp, vp, i32, vp, vp, vp, vp]),
     "ds2_beam_decode_workspace_bytes": (sz, [i32] * 4),
     "ds2_beam_decode": (i32, [i32, i32, i32, vp, vp, i32, i32, i32, f32] + [vp] * 6 + [sz, vp]),

@@ -116,6 +116,17 @@ class EvalConfig(InferenceConfig):
 
 
 @dataclass
+class AlignConfig:
+    """the settings of `align_manifest` (no counterpart in the reference): forced alignment of a manifest's
+    transcripts to its audio"""
+    model: ModelConfig = field(default_factory=ModelConfig)
+    manifest_path: str = ''     # JSON manifest or directory of .wav files with transcripts under /txt/
+    output_path: str = ''       # JSON lines, one record per utterance in manifest order
+    batch_size: int = 20
+    num_workers: int = 4
+
+
+@dataclass
 class OptimizerConfig:
     """search_lm_params.py:15-31 (the settings of `search_lm_params`) plus `seed` and `output_path`.  `n_jobs` and
     the decoding use of `num_workers` have no effect on the GPU search; `num_workers` still sets the loader's file

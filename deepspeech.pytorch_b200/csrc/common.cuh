@@ -149,5 +149,10 @@ int transpose_strided(int R, int C, const float* in, size_t ldi, float* out, siz
 // dx = gamma*invstd*(dy - mean(dy) - xhat*mean(dy*xhat)); dgamma, dbeta written.
 int bn_rows_bwd(int rows, int F, const float* xhat, const float* gamma, const float* mean_invstd, const float* dy,
                 float* dx, float* dgamma, float* dbeta, double* ws_sums /*2F doubles*/, cudaStream_t st);
+// CTC helpers (ctc.cu), shared by the loss and the forced alignment (ctc_align.cu):
+// fp32 log-softmax of `rows` rows of C values; the exclusive prefix sum of the target lengths (offsets into the flat
+// targets)
+int ctc_log_softmax(int rows, int C, const float* logits, float* lp, cudaStream_t st);
+int ctc_target_offsets(int B, const int32_t* tgt_len, long long* off, cudaStream_t st);
 
 }  // namespace ds2

@@ -207,6 +207,16 @@ __global__ void ctc_offsets_kernel(int B, const int32_t* __restrict__ tgt_len, l
   }
 }
 
+int ctc_log_softmax(int rows, int C, const float* logits, float* lp, cudaStream_t st) {
+  DS2_LAUNCH(ctc_logsoftmax_kernel, cdiv(rows, 8), 256, 0, st, rows, C, logits, lp);
+  return DS2_OK;
+}
+
+int ctc_target_offsets(int B, const int32_t* tgt_len, long long* off, cudaStream_t st) {
+  DS2_LAUNCH(ctc_offsets_kernel, 1, 32, 0, st, B, tgt_len, off);
+  return DS2_OK;
+}
+
 // Workspace of ds2_ctc_loss_fwd_bwd (bytes; with a base, also the addresses), each buffer 256-byte aligned:
 //   log-softmax lp (T,B,C) | alpha | beta (B,T,Smax) | their per-time scale offsets (B,T doubles each) |
 //   log-likelihood (B doubles) | target offsets (B)
@@ -247,10 +257,9 @@ int ds2_ctc_loss_fwd_bwd(int T, int B, int C, const float* logits, const int64_t
   DS2_REQUIRE(ws && ws_bytes >= need, "ds2_ctc: workspace null or too small (%zu < %zu bytes)", ws_bytes, need);
   cudaStream_t st = as_stream(stream);
   const int Smax = 2 * max_tgt_len + 1;
-  int rows = T * B;
   DS2_PROF("ctc", st);
-  DS2_LAUNCH(ctc_logsoftmax_kernel, cdiv(rows, 8), 256, 0, st, rows, C, logits, W.lp);
-  DS2_LAUNCH(ctc_offsets_kernel, 1, 32, 0, st, B, tgt_len, W.off);
+  if (int rc = ctc_log_softmax(T * B, C, logits, W.lp, st)) return rc;
+  if (int rc = ctc_target_offsets(B, tgt_len, W.off, st)) return rc;
   int threads = (Smax + 31) / 32 * 32;
   if (threads > 1024) threads = 1024;
   if (threads < 64) threads = 64;

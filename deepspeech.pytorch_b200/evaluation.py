@@ -200,15 +200,15 @@ def _on_device_path(decoder, target_decoder):
             and list(decoder.labels) == list(target_decoder.labels))
 
 
-def model_forward(model, inputs, input_sizes, precision):
+def model_forward(model, inputs, input_sizes, precision, logits=False):
     """the eval forward of validation.py:160-161: precision 16 runs in the library's fp16 mode (the reference's
-    autocast), as run_transcribe does"""
+    autocast), as run_transcribe does.  `logits=True` returns the logits instead of the eval softmax."""
     lib = get_lib()
     saved = lib.ds2_get_precision()
     if precision == 16:
         lib.ds2_set_precision(_lib.PREC_F16)
     try:
-        return model(inputs, input_sizes)
+        return model(inputs, input_sizes, logits=True) if logits else model(inputs, input_sizes)
     finally:
         lib.ds2_set_precision(saved)
 

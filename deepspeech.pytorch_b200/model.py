@@ -122,11 +122,12 @@ class DeepSpeech(_Base):
         return torch.from_numpy(out).int()
 
     # ------------------------------------------------------------------ forward (model.py:214-239)
-    def forward(self, x, lengths, hs: Optional[list] = None):
+    def forward(self, x, lengths, hs: Optional[list] = None, *, logits: bool = False):
         """model.py:214-239.  `precision == 16` (the reference wraps this call in autocast, model.py:255 /
         inference.py:94, and Lightning does so for training) selects the library's precision-16 mode for the duration
         of the call; the autograd nodes remember it for their backward.  Any other value leaves the process-wide
-        switch (`set_precision`) alone."""
+        switch (`set_precision`) alone.  `logits=True` returns the fc head's logits in eval mode too, without the
+        eval softmax (forced alignment wants log-probabilities, not probabilities)."""
         if not x.is_cuda:
             raise _lib.Ds2Error("DeepSpeech (CUDA shell): input must be a CUDA tensor; there is no CPU path")
         if self.precision == 16:
@@ -135,12 +136,12 @@ class DeepSpeech(_Base):
             if saved != _lib.PREC_F16:
                 lib.ds2_set_precision(_lib.PREC_F16)
                 try:
-                    return self._forward(x, lengths, hs)
+                    return self._forward(x, lengths, hs, logits)
                 finally:
                     lib.ds2_set_precision(saved)
-        return self._forward(x, lengths, hs)
+        return self._forward(x, lengths, hs, logits)
 
-    def _forward(self, x, lengths, hs: Optional[list] = None):
+    def _forward(self, x, lengths, hs: Optional[list] = None, logits: bool = False):
         lengths = torch.as_tensor(lengths).cpu().int()
         output_lengths = self.get_seq_lens(lengths)
         ol = output_lengths.tolist()
@@ -196,11 +197,11 @@ class DeepSpeech(_Base):
         if not self.bidirectional:
             y = ops.Lookahead.apply(y, self.lookahead[0].conv.weight)
         fbn, flin = self.fc[0].module[0], self.fc[0].module[1]
-        logits = ops.FcHead.apply(y, fbn.weight, fbn.bias, fbn.running_mean, fbn.running_var, flin.weight, training,
-                                  BN_MOMENTUM, BN_EPS, not training)            # eval: softmax (model.py:72-77)
+        out = ops.FcHead.apply(y, fbn.weight, fbn.bias, fbn.running_mean, fbn.running_var, flin.weight, training,
+                               BN_MOMENTUM, BN_EPS, not (training or logits))   # eval: softmax (model.py:72-77)
         if training:
             fbn.num_batches_tracked += 1
-        return logits.transpose(0, 1), output_lengths, new_hs
+        return out.transpose(0, 1), output_lengths, new_hs
 
     # ------------------------------------------------------------------ loss (model.py:203,241-249)
     def _ctc_criterion(self, logits_tbc, targets, input_sizes, target_sizes):

@@ -186,6 +186,35 @@ int ds2_ctc_loss_fwd_bwd(int T, int B, int C, const float* logits, const int64_t
                          const int32_t* in_len, const int32_t* tgt_len, int max_tgt_len, int blank,
                          float* nll, float* grad, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- CTC forced alignment: the Viterbi path of each known target through the CTC lattice ---------------------
+ *   x (T,B,C) fp32: logits (apply_log_softmax = 1: the log-softmax of ds2_ctc_loss_fwd_bwd is applied first) or
+ *   log-probabilities used as given (apply_log_softmax = 0; -inf allowed).  targets, in_len, tgt_len, max_tgt_len and
+ *   blank as for ds2_ctc_loss_fwd_bwd; in_len is clamped to [0, T] and frames t >= in_len[b] are never read.
+ *   Extended sequence of S = 2L+1 states (blank, y1, blank, ..., yL, blank); fp64 scores
+ *     score_t(s) = max(score_{t-1}(s), score_{t-1}(s-1), score_{t-1}(s-2)) + (double)lp[t][ext[s]]
+ *   where s-2 counts only if ext[s] != blank && ext[s] != ext[s-2]; at t = 0 only states 0 and 1 are live; ties
+ *   prefer s, then s-1, then s-2; the path ends in S-1 if score(S-1) >= score(S-2), else in S-2.
+ *   Outputs (device):
+ *     frame_labels (B,T) int32    label on the path, blank included; -1 for t >= in_len[b]      (may be NULL)
+ *     frame_log_probs (B,T) fp32  log-prob of that label; 0 where the label is -1                 (may be NULL)
+ *     token_spans (B,max_tgt_len,2) int32  [start, end) frames of target token k; -1 for k >= tgt_len[b]
+ *     path_score (B) fp64         the path's total log-prob
+ *   An utterance without a finite path (too few frames, every path through a -inf entry, in_len 0 with a non-empty
+ *   target), or with tgt_len outside [0, max_tgt_len] or a target label outside [0, C), gets path_score = -inf, all
+ *   labels and spans -1; the rest of the batch is aligned.  L = 0 gives the all-blank path (score 0 when in_len = 0).
+ *   Limits: max_tgt_len <= DS2_CTC_ALIGN_MAX_TGT_LEN and C <= DS2_CTC_ALIGN_MAX_CLASSES (the two fp64 DP rows live in
+ *   shared memory); beyond them the call returns DS2_ERR_INVALID.  Deterministic (no atomics); three launches.
+ *   Workspace (bytes), each term rounded up to a multiple of 256:
+ *     T*B*C*4 (log-probs) + B*T*ceil((2*max_tgt_len+1)/32)*8 (2-bit backpointers) + B*8 (target offsets)
+ *   e.g. 3,904,256 bytes at T = 500, B = 32, C = 29, max_tgt_len = 250.                                                     */
+#define DS2_CTC_ALIGN_MAX_TGT_LEN 6144
+#define DS2_CTC_ALIGN_MAX_CLASSES 1024
+size_t ds2_ctc_align_workspace_bytes(int T, int B, int C, int max_tgt_len);
+int ds2_ctc_align(int T, int B, int C, const float* x, int apply_log_softmax, const int64_t* targets,
+                  const int32_t* in_len, const int32_t* tgt_len, int max_tgt_len, int blank,
+                  int32_t* frame_labels, float* frame_log_probs, int32_t* token_spans, double* path_score,
+                  void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- greedy decode (row N2): argmax -> collapse repeats -> drop blank, decoder.py:144-181 -----
  *   probs (B,T,C); out_len (B) ; labels/offsets (B,T) int32, counts (B) int32                   */
 int ds2_greedy_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
