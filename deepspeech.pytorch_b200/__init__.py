@@ -32,3 +32,4 @@ from .lm_search import LMParamSearch, search_lm_params  # noqa: E402
 from .checkpoint import FileCheckpointHandler  # noqa: E402
 from .training import DSElasticDistributedSampler, DSRandomSampler, seed_everything, train  # noqa: E402
 from .alignment import align_audio, align_manifest, forced_align  # noqa: E402
+from .streaming import StreamingTranscriber, StreamResult  # noqa: E402

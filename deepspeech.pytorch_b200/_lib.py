@@ -50,6 +50,7 @@ PROTOTYPES = {
     "ds2_ctc_align_workspace_bytes": (sz, [i32, i32, i32, i32]),
     "ds2_ctc_align": (i32, [i32, i32, i32, vp, i32] + [vp] * 3 + [i32, i32] + [vp] * 5 + [sz, vp]),
     "ds2_greedy_decode": (i32, [i32, i32, i32, vp, vp, i32, vp, vp, vp, vp]),
+    "ds2_greedy_decode_stream": (i32, [i32, i32, vp, vp, vp, i32, vp, vp, vp]),
     "ds2_beam_decode_workspace_bytes": (sz, [i32] * 4),
     "ds2_beam_decode": (i32, [i32, i32, i32, vp, vp, i32, i32, i32, f32] + [vp] * 6 + [sz, vp]),
     "ds2_lm_bytes": (sz, [i32, vp, i64]),
@@ -60,10 +61,18 @@ PROTOTYPES = {
     "ds2_beam_decode_lm_grid_workspace_bytes": (sz, [i32] * 5),
     "ds2_beam_decode_lm_grid": (i32, [i32, i32, i32, vp, vp, i32, i32, i32, f32, vp, i32, i32, vp, i32]
                                 + [vp] * 3 + [sz, vp]),
+    "ds2_beam_decode_stream_state_bytes": (sz, [i32] * 3),
+    "ds2_beam_decode_lm_stream_state_bytes": (sz, [i32] * 3),
+    "ds2_beam_decode_stream": (i32, [i32, i32, vp, vp, i32, i32, i32, f32, i32, i32, i32] + [vp] * 6 + [sz, vp]),
+    "ds2_beam_decode_lm_stream": (i32, [i32, i32, vp, vp, i32, i32, i32, f32, vp, i32, C.c_double, C.c_double, i32,
+                                        i32, i32, i32] + [vp] * 6 + [sz, vp]),
     "ds2_error_counts_workspace_bytes": (sz, [i32, i32, i64, i32]),
     "ds2_error_counts": (i32, [i32, i32, i32, vp, vp, vp, i64, vp, i32, i32, i32] + [vp] * 3 + [sz, vp]),
     "ds2_spectrogram_workspace_bytes": (sz, [i32]),
     "ds2_spectrogram_batch": (i32, [i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, vp, i32, vp, sz, vp]),
+    "ds2_spectrogram_stream_state_bytes": (sz, [i32]),
+    "ds2_spectrogram_stream_workspace_bytes": (sz, [i32, i32]),
+    "ds2_spectrogram_stream": (i32, [i32, vp, vp, i32, i32, i32, vp, vp, i32, vp, vp, sz, vp]),
     "ds2_spec_augment_workspace_bytes": (sz, [i32]),
     "ds2_spec_augment": (i32, [i32, i32, i32] + [vp] * 5 + [sz, vp]),
     "ds2_optim_workspace_bytes": (sz, []),

@@ -175,17 +175,34 @@ __device__ __forceinline__ long long hash_slot(unsigned long long k, long long H
   return (long long)(k & (unsigned long long)(HC - 1));
 }
 
+// Streaming (ds2_beam_decode_stream): the beam list of a session between calls, one record per pool slot.  Record:
+// n_list, pool_next, frames decoded so far, 0 (4 ints) | lb, lnb, sc, lmv (W doubles each) | kids, amask (W u64 each) |
+// lab, node, pnode, pslot, tn (W ints each) | ctx (W * LM_CTX ints); every array 16-byte aligned.
+size_t stream_rec_bytes(int W) {
+  return align_up(16 + (size_t)W * (4 * 8 + 2 * 8 + 5 * 4) + (size_t)W * LM_CTX * 4, 256);
+}
+
+// The session a streaming CTA runs: items[5 * s ..] = {row0, n_frames, slot, flags, out_row}; flags bit 0: the session's
+// first call (clear its hash, start from the empty prefix), bit 1: final (write all W beams, else only the best);
+// probability rows [row0, row0 + n_frames) of the packed (rows, C) array; beams to rows out_row.. of (rows, Tout).
+struct StreamArgs {
+  const int32_t* items;
+  unsigned char* recs;
+  size_t rec_bytes;
+  int Tout;
+};
+
 // One beam search: utterance u, in pool slot `slot`, written to output row `out`.  TOP = false writes every beam
 // (rule 6) at out = u; TOP = true writes only the best beam: labels row `out` of (rows, T) and lengths[out] (the grid
 // entry, where timesteps, scores and n_beams are NULL).  Both kernels below run this body.
-template <bool LM, bool TOP>
+template <bool LM, bool TOP, bool STREAM = false>
 __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T, int C,
                                                  const float* __restrict__ probs, const int32_t* __restrict__ out_len,
                                                  int blank, int W, int top_n, float cutoff_prob,
                                                  int32_t* __restrict__ labels, int32_t* __restrict__ timesteps,
                                                  int32_t* __restrict__ lengths, double* __restrict__ scores,
                                                  int32_t* __restrict__ n_beams, const BeamPool& pool,
-                                                 const BeamLm& lmp) {
+                                                 const BeamLm& lmp, const StreamArgs sa = StreamArgs{}) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long* key = reinterpret_cast<unsigned long long*>(smem_raw);
@@ -221,7 +238,7 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
   __shared__ int hist[256];
   __shared__ unsigned warp_new[BEAM_MAX_W / 32];
   __shared__ unsigned long long kmask, pre_hi;
-  __shared__ int n_list, nK, n_valid, n_sel, need, passes, done, pre_e, pool_next;
+  __shared__ int n_list, nK, n_valid, n_sel, need, passes, done, pre_e, pool_next, t_base;
 
   const long long NP = pool.NP, HC = pool.HC;
   int* P_par = pool.parent + (size_t)slot * NP;
@@ -232,9 +249,41 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
   unsigned long long* hk = pool.hkey + (size_t)slot * HC;
   int* hv = pool.hval + (size_t)slot * HC;
 
-  for (long long i = tid; i < HC; i += BEAM_THREADS) hk[i] = 0ull;
-  const int Tu = out_len ? min(max(out_len[u], 0), T) : T;
-  if (tid == 0) {
+  // streaming: the session's item and its saved list (a resumed call loads it instead of starting afresh)
+  const int32_t* it = STREAM ? sa.items + 5 * (size_t)u : nullptr;
+  const bool resume = STREAM && !(it[3] & 1);
+  unsigned char* rec = STREAM ? sa.recs + (size_t)slot * sa.rec_bytes : nullptr;
+  double* R_lb = reinterpret_cast<double*>(rec + 16);
+  double* R_lnb = R_lb + W;
+  double* R_sc = R_lnb + W;
+  double* R_lmv = R_sc + W;
+  unsigned long long* R_kids = reinterpret_cast<unsigned long long*>(R_lmv + W);
+  unsigned long long* R_amask = R_kids + W;
+  int* R_lab = reinterpret_cast<int*>(R_amask + W);
+  int* R_node = R_lab + W;
+  int* R_pnode = R_node + W;
+  int* R_pslot = R_pnode + W;
+  int* R_tn = R_pslot + W;
+  int* R_ctx = R_tn + W;
+  if (!resume)
+    for (long long i = tid; i < HC; i += BEAM_THREADS) hk[i] = 0ull;
+  const int Tu = STREAM ? it[1] : (out_len ? min(max(out_len[u], 0), T) : T);
+  const float* prow = STREAM ? probs + (size_t)it[0] * C : probs + (size_t)u * T * C;
+  if (tid == 0) t_base = resume ? reinterpret_cast<const int*>(rec)[2] : 0;
+  if (resume) {
+    if (tid == 0) {
+      n_list = reinterpret_cast<const int*>(rec)[0];
+      pool_next = reinterpret_cast<const int*>(rec)[1];
+    }
+    if (tid < W) {
+      lb[tid] = R_lb[tid]; lnb[tid] = R_lnb[tid]; sc[tid] = R_sc[tid]; kids[tid] = R_kids[tid];
+      lab[tid] = R_lab[tid]; node[tid] = R_node[tid]; pnode[tid] = R_pnode[tid]; pslot[tid] = R_pslot[tid];
+      if constexpr (LM) {
+        lmv[tid] = R_lmv[tid]; amask[tid] = R_amask[tid]; tn[tid] = R_tn[tid];
+        for (int k = 0; k < LM_CTX; ++k) ctx[tid * LM_CTX + k] = R_ctx[tid * LM_CTX + k];
+      }
+    }
+  } else if (tid == 0) {
     P_par[0] = -1; P_lab[0] = -1; P_ts[0] = 0; P_depth[0] = 0; P_best[0] = -CUDART_INF;
     lb[0] = 0.0; lnb[0] = -CUDART_INF; sc[0] = 0.0;
     lab[0] = -1; node[0] = 0; pnode[0] = -1; pslot[0] = -1; kids[0] = 0ull;
@@ -244,7 +293,7 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
   const int order = LM ? lmp.order : 1, space = LM ? lmp.space : -1;
   if constexpr (LM) {
     lmt = lm_view(lmp.tables);
-    if (tid == 0) {
+    if (tid == 0 && !resume) {
       tn[0] = 0;                                     // the root: the empty partial word, not a word itself
       amask[0] = lmt.mask[0];
       lmv[0] = 0.0;
@@ -254,10 +303,12 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
   __syncthreads();
 
   const bool prune = cutoff_prob < 1.f || top_n < C;
+  const int t0 = STREAM ? t_base : 0;                 // stream frame of this call's first row
   for (int t = 0; t < Tu; ++t) {
+    const int tg = t0 + t;
     // ---- A. probabilities, logs, the kept set K (rule 3)
     if (warp == 0) {
-      const float* p = probs + ((size_t)u * T + t) * C;
+      const float* p = prow + (size_t)t * C;
       for (int c = lane; c < C; c += 32) {
         const float v = p[c];
         pf[c] = v;
@@ -343,12 +394,12 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
               if (l == space) v2 = __dadd_rn(v2, lm_term(lmp, lmv[pi]));            // L3
               nn = lse(nn, v2);
               const int nd = node[i];
-              if (lpl > P_best[nd]) { P_best[nd] = lpl; P_ts[nd] = t; }
+              if (lpl > P_best[nd]) { P_best[nd] = lpl; P_ts[nd] = tg; }
             }
           } else if (pi >= 0) {
             nn = lse(nn, lpl + (lab[pi] == l ? lb[pi] : sc[pi]));
             const int nd = node[i];
-            if (lpl > P_best[nd]) { P_best[nd] = lpl; P_ts[nd] = t; }
+            if (lpl > P_best[nd]) { P_best[nd] = lpl; P_ts[nd] = tg; }
           }
         }
         sb[i] = bb;
@@ -528,7 +579,7 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
         int id = first_new + __popc(warp_new[warp] & ((1u << lane) - 1u));
         for (int w = 0; w < warp; ++w) id += __popc(warp_new[w]);
         const int pn = pnode2[tid], c = lab2[tid];
-        P_par[id] = pn; P_lab[id] = c; P_ts[id] = t; P_best[id] = lp[c]; P_depth[id] = P_depth[pn] + 1;
+        P_par[id] = pn; P_lab[id] = c; P_ts[id] = tg; P_best[id] = lp[c]; P_depth[id] = P_depth[pn] + 1;
         for (;;) {                                       // hs: the empty slot the lookup stopped at, or later
           const unsigned long long prev = atomicCAS(&hk[hs], 0ull, hkey_new);
           if (prev == 0ull) { hv[hs] = id; break; }
@@ -563,6 +614,22 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
     __syncthreads();
   }
 
+  // ---- streaming: save the list for the session's next call (the end term below does not change it)
+  if constexpr (STREAM) {
+    if (tid < W) {
+      R_lb[tid] = lb[tid]; R_lnb[tid] = lnb[tid]; R_sc[tid] = sc[tid]; R_kids[tid] = kids[tid];
+      R_lab[tid] = lab[tid]; R_node[tid] = node[tid]; R_pnode[tid] = pnode[tid]; R_pslot[tid] = pslot[tid];
+      if constexpr (LM) {
+        R_lmv[tid] = lmv[tid]; R_amask[tid] = amask[tid]; R_tn[tid] = tn[tid];
+        for (int k = 0; k < LM_CTX; ++k) R_ctx[tid * LM_CTX + k] = ctx[tid * LM_CTX + k];
+      }
+    }
+    if (tid == 0) {
+      int* h = reinterpret_cast<int*>(rec);
+      h[0] = n_list; h[1] = pool_next; h[2] = t0 + Tu; h[3] = 0;
+    }
+  }
+
   // ---- LM: the end-of-utterance term and the reorder (rule L5); the final score goes to sb, the position to rnk
   if constexpr (LM) {
     const int n = n_list;
@@ -582,6 +649,38 @@ __device__ __forceinline__ void beam_search_item(int u, int slot, int out, int T
   }
 
   // ---- output (rule 6): zero the rows, then walk each beam's parent chain
+  if constexpr (STREAM) {   // final: all W beams in rows out_row.., else the best one in row out_row
+    const int rows = (it[3] & 2) ? W : 1, Tout = sa.Tout;
+    const size_t r0 = (size_t)it[4];
+    for (size_t x = tid; x < (size_t)rows * Tout; x += BEAM_THREADS) {
+      labels[r0 * Tout + x] = 0;
+      timesteps[r0 * Tout + x] = 0;
+    }
+    __syncthreads();
+    if (tid < W) {
+      const int r = LM && tid < n_list ? rnk[tid] : tid;
+      if (r < rows) {
+        if (tid < n_list) {
+          int nd = node[tid];
+          const int len = P_depth[nd];
+          lengths[r0 + r] = len;
+          scores[r0 + r] = -(LM ? sb[tid] : sc[tid]) + 0.0;
+          int32_t* L = labels + (r0 + r) * Tout;
+          int32_t* S = timesteps + (r0 + r) * Tout;
+          for (int pos = len - 1; pos >= 0; --pos) {
+            L[pos] = P_lab[nd];
+            S[pos] = P_ts[nd];
+            nd = P_par[nd];
+          }
+        } else {
+          lengths[r0 + r] = 0;
+          scores[r0 + r] = CUDART_INF;
+        }
+      }
+    }
+    if (tid == 0) n_beams[u] = n_list;
+    return;
+  }
   if constexpr (TOP) {
     int32_t* L = labels + (size_t)out * T;
     for (int x = tid; x < T; x += BEAM_THREADS) L[x] = 0;
@@ -659,6 +758,18 @@ beam_decode_grid_kernel(int B, int K, int T, int C, const float* __restrict__ pr
                                  labels, nullptr, lengths, nullptr, nullptr, pool, L);
     __syncthreads();   // the next item's set-up overwrites the list this one's output read
   }
+}
+
+// ds2_beam_decode_stream / ds2_beam_decode_lm_stream: one CTA per session of the call, in its own pool slot
+template <bool LM>
+__global__ void __launch_bounds__(BEAM_THREADS)
+beam_decode_stream_kernel(int C, const float* __restrict__ probs, int blank, int W, int top_n, float cutoff_prob,
+                          int32_t* __restrict__ labels, int32_t* __restrict__ timesteps, int32_t* __restrict__ lengths,
+                          double* __restrict__ scores, int32_t* __restrict__ n_beams, BeamPool pool, BeamLm lmp,
+                          StreamArgs sa) {
+  const int s = blockIdx.x;
+  beam_search_item<LM, false, true>(s, sa.items[5 * s + 2], s, 0, C, probs, nullptr, blank, W, top_n, cutoff_prob,
+                                    labels, timesteps, lengths, scores, n_beams, pool, lmp, sa);
 }
 
 // The pools of `slots` CTAs at offset `off` of a workspace, each array 256-byte aligned:
@@ -762,6 +873,42 @@ size_t grid_ws_carve(int K, int slots, int T, int W, void* base, GridWs& w) {
   return off;
 }
 
+// Streaming state of max_sessions slots: the pools (sized for max_frames), then one list record per slot
+struct StreamState { BeamPool pool; unsigned char* recs; size_t rec_bytes; };
+size_t stream_state_carve(int S, int max_frames, int W, bool lm, void* base, StreamState& st) {
+  size_t off = 0;
+  st.pool = carve_pool(base, off, S, max_frames, W, lm);
+  st.rec_bytes = stream_rec_bytes(W);
+  st.recs = carve<unsigned char>(base, off, (size_t)S * st.rec_bytes);
+  return off;
+}
+
+template <bool LM>
+int beam_stream_launch(const char* fn, int n_sess, int C, const float* probs, const int32_t* items, int blank,
+                       int beam_width, int cutoff_top_n, float cutoff_prob, BeamLm lm, int max_sessions,
+                       int max_frames, int Tout, int32_t* labels, int32_t* timesteps, int32_t* lengths,
+                       double* scores, int32_t* n_beams, void* state, size_t state_bytes, void* stream) {
+  const int rc = beam_check_args(fn, max_sessions, max_frames, C, blank, beam_width, cutoff_top_n, cutoff_prob);
+  if (rc != DS2_OK) return rc;
+  DS2_REQUIRE(n_sess > 0 && n_sess <= max_sessions && Tout > 0, "%s: bad shape n_sess=%d Tout=%d", fn, n_sess, Tout);
+  DS2_REQUIRE(probs && items && labels && timesteps && lengths && scores && n_beams, "%s: null pointer", fn);
+  StreamState S;
+  const size_t need = stream_state_carve(max_sessions, max_frames, beam_width, LM, state, S);
+  DS2_REQUIRE(state && state_bytes >= need, "%s: state too small (%zu < %zu bytes)", fn, state_bytes, need);
+  static DeviceOnce attr_once;
+  if (attr_once.first()) {
+    DS2_CHECK_CUDA(cudaFuncSetAttribute(beam_decode_stream_kernel<LM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)dyn_smem_bytes(BEAM_MAX_W, BEAM_MAX_C, LM)));
+    attr_once.done();
+  }
+  StreamArgs sa{items, S.recs, S.rec_bytes, Tout};
+  cudaStream_t st = as_stream(stream);
+  DS2_PROF(LM ? "beam_decode_lm_stream" : "beam_decode_stream", st);
+  DS2_LAUNCH(beam_decode_stream_kernel<LM>, n_sess, BEAM_THREADS, dyn_smem_bytes(beam_width, C, LM), st, C, probs,
+             blank, beam_width, cutoff_top_n, cutoff_prob, labels, timesteps, lengths, scores, n_beams, S.pool, lm, sa);
+  return DS2_OK;
+}
+
 }  // namespace
 }  // namespace ds2
 
@@ -844,6 +991,47 @@ int ds2_beam_decode_lm_grid(int B, int T, int C, const float* probs, const int32
   DS2_LAUNCH(beam_decode_grid_kernel, (int)slots, BEAM_THREADS, dyn_smem_bytes(beam_width, C, true), st, B, K, T, C,
              probs, out_len, blank, beam_width, cutoff_top_n, cutoff_prob, G.pairs, labels, lengths, G.pool, L);
   return DS2_OK;
+}
+
+size_t ds2_beam_decode_stream_state_bytes(int max_sessions, int max_frames, int beam_width) {
+  if (max_sessions <= 0 || max_frames <= 0 || beam_width <= 0) return 0;
+  StreamState S;
+  return stream_state_carve(max_sessions, max_frames, beam_width, false, nullptr, S);
+}
+
+size_t ds2_beam_decode_lm_stream_state_bytes(int max_sessions, int max_frames, int beam_width) {
+  if (max_sessions <= 0 || max_frames <= 0 || beam_width <= 0) return 0;
+  StreamState S;
+  return stream_state_carve(max_sessions, max_frames, beam_width, true, nullptr, S);
+}
+
+int ds2_beam_decode_stream(int n_sess, int C, const float* probs, const int32_t* items, int blank, int beam_width,
+                           int cutoff_top_n, float cutoff_prob, int max_sessions, int max_frames, int Tout,
+                           int32_t* labels, int32_t* timesteps, int32_t* lengths, double* scores, int32_t* n_beams,
+                           void* state, size_t state_bytes, void* stream) {
+  return beam_stream_launch<false>("ds2_beam_decode_stream", n_sess, C, probs, items, blank, beam_width, cutoff_top_n,
+                                   cutoff_prob, BeamLm{}, max_sessions, max_frames, Tout, labels, timesteps, lengths,
+                                   scores, n_beams, state, state_bytes, stream);
+}
+
+int ds2_beam_decode_lm_stream(int n_sess, int C, const float* probs, const int32_t* items, int blank, int beam_width,
+                              int cutoff_top_n, float cutoff_prob, const void* lm, int lm_order, double alpha,
+                              double beta, int space, int max_sessions, int max_frames, int Tout, int32_t* labels,
+                              int32_t* timesteps, int32_t* lengths, double* scores, int32_t* n_beams, void* state,
+                              size_t state_bytes, void* stream) {
+  const int rc = lm_check_args("ds2_beam_decode_lm_stream", C, blank, lm, lm_order, space);
+  if (rc != DS2_OK) return rc;
+  DS2_REQUIRE(std::isfinite(alpha) && std::isfinite(beta), "ds2_beam_decode_lm_stream: alpha=%g, beta=%g not finite",
+              alpha, beta);
+  BeamLm L;
+  L.tables = lm;
+  L.order = lm_order;
+  L.space = space;
+  L.alpha = alpha;
+  L.beta = beta;
+  return beam_stream_launch<true>("ds2_beam_decode_lm_stream", n_sess, C, probs, items, blank, beam_width,
+                                  cutoff_top_n, cutoff_prob, L, max_sessions, max_frames, Tout, labels, timesteps,
+                                  lengths, scores, n_beams, state, state_bytes, stream);
 }
 
 }  // extern "C"

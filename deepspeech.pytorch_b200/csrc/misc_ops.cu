@@ -118,6 +118,33 @@ __global__ void greedy_decode_kernel(int B, int T, int C, const float* __restric
   }
 }
 
+// streaming: one CTA per session; argmax of the session's new rows in parallel, then the collapse in order from the
+// carried argmax of the previous call's last row
+__global__ void greedy_decode_stream_kernel(int C, const float* __restrict__ probs, const int32_t* __restrict__ row_off,
+                                            const int32_t* __restrict__ slot, int blank, int32_t* __restrict__ carry,
+                                            int32_t* __restrict__ labels) {
+  const int s = blockIdx.x, r0 = row_off[s], r1 = row_off[s + 1];
+  if (r1 <= r0) return;
+  for (int r = r0 + threadIdx.x; r < r1; r += blockDim.x) {
+    const float* p = probs + (size_t)r * C;
+    int best = 0;
+    float bv = p[0];
+    for (int c = 1; c < C; ++c)
+      if (p[c] > bv) { bv = p[c]; best = c; }
+    labels[r] = best;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int prev = carry[slot[s]];
+    for (int r = r0; r < r1; ++r) {
+      const int c = labels[r];
+      labels[r] = (c != blank && c != prev) ? c : -1;
+      prev = c;
+    }
+    carry[slot[s]] = prev;
+  }
+}
+
 // ------------------------------------------------------------------ optimizer (model.py:273-297 + clip 400)
 // Squared gradient norm, bit-repeatable: a fixed grid of NORM_PARTS blocks (every block's share of the vector and its
 // summation order depend on n only) writes one double partial each to ws[1 + block]; sumsq_final_kernel adds them in
@@ -322,6 +349,15 @@ int ds2_greedy_decode(int B, int T, int C, const float* probs, const int32_t* ou
     DS2_CHECK_CUDA(cudaFuncSetAttribute(greedy_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   DS2_LAUNCH(greedy_decode_kernel, B, 256, smem, as_stream(stream), B, T, C, probs, out_len, blank, labels, offsets,
              counts);
+  return DS2_OK;
+}
+
+int ds2_greedy_decode_stream(int n_sess, int C, const float* probs, const int32_t* row_off, const int32_t* slot,
+                             int blank, int32_t* carry, int32_t* labels, void* stream) {
+  DS2_REQUIRE(n_sess > 0 && C > 0 && probs && row_off && slot && carry && labels,
+              "ds2_greedy_decode_stream: bad arguments");
+  DS2_LAUNCH(greedy_decode_stream_kernel, n_sess, 256, 0, as_stream(stream), C, probs, row_off, slot, blank, carry,
+             labels);
   return DS2_OK;
 }
 

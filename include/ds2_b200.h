@@ -219,6 +219,13 @@ int ds2_ctc_align(int T, int B, int C, const float* x, int apply_log_softmax, co
  *   probs (B,T,C); out_len (B) ; labels/offsets (B,T) int32, counts (B) int32                   */
 int ds2_greedy_decode(int B, int T, int C, const float* probs, const int32_t* out_len, int blank,
                       int32_t* labels, int32_t* offsets, int32_t* counts, void* stream);
+/* streaming greedy decode (row N9): the probabilities of each session's newly decided frames, packed session after
+ * session: rows [row_off[s], row_off[s+1]) of probs (rows, C) belong to session s, whose carried argmax is
+ * carry[slot[s]] (-1 at the stream start; ds2_greedy_decode's frame-0 rule).  labels (rows) int32 gets the label a
+ * row emits (argmax, lowest index on ties, not blank, not equal to the previous frame's argmax) or -1; the last
+ * row's argmax goes back to carry.  Over a stream the emitted labels equal ds2_greedy_decode of the whole output. */
+int ds2_greedy_decode_stream(int n_sess, int C, const float* probs, const int32_t* row_off, const int32_t* slot,
+                             int blank, int32_t* carry, int32_t* labels, void* stream);
 
 /* ---- beam-search decode (row N5): CTC prefix beam search without a language model, what decoder.py:56-118
  * (BeamCTCDecoder) gets from ctcdecode with an empty lm_path; the rules are in csrc/beam_decode.cu.
@@ -280,6 +287,38 @@ int ds2_beam_decode_lm_grid(int B, int T, int C, const float* probs, const int32
                             int32_t* labels, int32_t* lengths,
                             void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- streaming beam search (row N9): ds2_beam_decode(_lm) resumed across calls, one CTA per session -------------
+ * The search of a session is the one ds2_beam_decode(_lm) runs on the concatenation of its calls' rows: the same
+ * rules 1-7 / L0-L5, tie rules and fp64 arithmetic, so after a final call its W beams (labels, timesteps, lengths,
+ * scores, n_beams) equal the one-shot search on the whole output bit for bit, and the best beam reported after t
+ * frames is the one-shot search's first beam on the first t frames (including the L5 end term and reorder).
+ *   items     (n_sess, 5) int32 on the device: {row0, n_frames, slot, flags, out_row}.  Rows [row0, row0+n_frames) of
+ *             probs (rows, C) are the session's new frames (n_frames may be 0).  flags bit 0: the session's first call
+ *             (reset: its hash is cleared and the list starts from the empty prefix); bit 1: final (write all W beams
+ *             to output rows out_row .. out_row+W-1, as ds2_beam_decode writes them; otherwise only the current best
+ *             to row out_row).  Slots of one call must differ.
+ *   labels, timesteps (rows_out, Tout) int32; lengths (rows_out) int32; scores (rows_out) double; n_beams (n_sess).
+ *             Tout >= the frames the session has decoded so far (a beam is at most that long); timesteps are stream
+ *             frame indices.
+ *   state     ds2_beam_decode(_lm)_stream_state_bytes(max_sessions, max_frames, beam_width), kept across calls:
+ *             per slot a node pool of max_frames * W + 1 nodes with its (parent, label) hash, never compacted (rule
+ *             2: a returning prefix keeps its node, so nodes of dropped prefixes stay), and the list record (lb, lnb,
+ *             sc, lab, node, pnode, pslot, kids; with the LM amask, lmv, tn, ctx; n_list, pool_next, frames so far).
+ *             Per slot: NP = max_frames*W + 1 nodes of 24 bytes (+8 with the LM) plus HC = the power of two >= 2 NP
+ *             hash entries of 12 bytes: 600 s (30 001 frames) at W = 100 is about 173 MB (197 MB with the LM).
+ *             A session must not see more than max_frames frames in total.  No workspace.                    */
+size_t ds2_beam_decode_stream_state_bytes(int max_sessions, int max_frames, int beam_width);
+size_t ds2_beam_decode_lm_stream_state_bytes(int max_sessions, int max_frames, int beam_width);
+int ds2_beam_decode_stream(int n_sess, int C, const float* probs, const int32_t* items, int blank, int beam_width,
+                           int cutoff_top_n, float cutoff_prob, int max_sessions, int max_frames, int Tout,
+                           int32_t* labels, int32_t* timesteps, int32_t* lengths, double* scores, int32_t* n_beams,
+                           void* state, size_t state_bytes, void* stream);
+int ds2_beam_decode_lm_stream(int n_sess, int C, const float* probs, const int32_t* items, int blank, int beam_width,
+                              int cutoff_top_n, float cutoff_prob, const void* lm, int lm_order, double alpha,
+                              double beta, int space, int max_sessions, int max_frames, int Tout, int32_t* labels,
+                              int32_t* timesteps, int32_t* lengths, double* scores, int32_t* n_beams, void* state,
+                              size_t state_bytes, void* stream);
+
 /* ---- WER / CER edit counts (validation.py:48-126, the Lev.distance calls of WordErrorRate / CharErrorRate) ----
  * Rows are hypotheses: labels (R,T) int32 with lengths (R) int32 (clamped to [0, T]), R = K x B, row k*B + b
  * scored against reference b.  References: targets flat int64 (n_targets) with target_sizes (B) int32, all on the
@@ -325,6 +364,42 @@ size_t ds2_spectrogram_workspace_bytes(int n_utts);
 int ds2_spectrogram_batch(int n_utts, const float* wave, const int64_t* offsets, const int32_t* dst_row,
                           int max_samples, int n_fft, int hop, const float* window, int pad_reflect, int normalize,
                           float* out, int Tmax, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- streaming spectrogram (row N9, DESIGN.md §5.11): the frames of live streams, a call at a time ---------
+ * Frame j of a stream covers samples [j*hop - n_fft/2, j*hop + n_fft/2), zero outside the stream: the frames of
+ * ds2_spectrogram_batch with pad_reflect = 0, through the same DFT code, so un-normalised frames are bit-identical.
+ * The host keeps each session's undecided PCM tail and packs tail + new audio into `wave`; a call emits the frames
+ * j = first_frame .. first_frame + n_frames - 1 of each session (the host emits a frame once its last sample has
+ * arrived, and at the stream end the frames up to 1 + n // hop with zero padding).
+ *   out       (n_sess, F, Tcap) fp32, session s's frames at columns 0 .. n_frames-1, normalised by `norm`:
+ *               1  fixed: (x - mean) / std with the record's mean / std;
+ *               0  running: frame j with the mean and unbiased std of all values of frames 0..j of the stream,
+ *                  from fp64 sums carried per session in `state` and added frame by frame in stream order, so the
+ *                  result does not depend on how the stream was split into calls (a causal departure from the
+ *                  offline per-utterance statistics and from per-chunk statistics);
+ *              -1  none (the raw log-magnitudes).
+ *   state     ds2_spectrogram_stream_state_bytes(max_sessions): DS2_STREAM_SPECT_STATE_DOUBLES fp64 per slot
+ *             (running sum, sum of squares); a call with first_frame == 0 starts the slot's sums from zero.
+ *   workspace ds2_spectrogram_stream_workspace_bytes(n_sess, Tcap) = n_sess * Tcap * 16 bytes (frame sums),
+ *             rounded up to 256; max_frames = the largest n_frames (grid sizing), Tcap >= max_frames.       */
+#define DS2_STREAM_SPECT_STATE_DOUBLES 2
+typedef struct {
+  int64_t wave_off;     /* first sample of the session's packed PCM in wave                                */
+  int64_t wave_len;     /* packed samples: stream samples [base, base + wave_len)                          */
+  int64_t base;         /* stream index of the first packed sample                                         */
+  int64_t first_frame;  /* stream index of the first frame of this call                                    */
+  int32_t n_frames;     /* frames emitted by this call (0: nothing to do)                                  */
+  int32_t slot;         /* state record of the session                                                     */
+  int32_t norm;         /* 1 fixed, 0 running, -1 none                                                     */
+  float mean, std;      /* fixed normalisation                                                             */
+  int32_t reserved[3];
+} Ds2StreamSpect;
+
+size_t ds2_spectrogram_stream_state_bytes(int max_sessions);
+size_t ds2_spectrogram_stream_workspace_bytes(int n_sess, int Tcap);
+int ds2_spectrogram_stream(int n_sess, const float* wave, const Ds2StreamSpect* sessions, int max_frames, int n_fft,
+                           int hop, const float* window, float* out, int Tcap, void* state, void* workspace,
+                           size_t workspace_bytes, void* stream);
 
 /* ---- input pipeline: SpecAugment on a padded spectrogram batch ----------------------------------
  * Replaces, per utterance, spec_augment (loader/spec_augment.py:68-115 with sparse_image_warp.py:88-410, the
