@@ -38,14 +38,15 @@ struct ConvGeom {
 
 // out[b,co,d,t] = bias[co] + sum_{ci,kh,kw} wpk[ci][kh][kw][co] * in[b,ci,d*SH+kh-PH,t*SW+kw-PW]
 // out address = b*ob + co*oc + d*orow + t ; positions t >= out_len[b] are written as 0 (if out_len)
-// stat_sums (double[64]) += per-channel sum / sum of squares of what was written (if non-null)
+// stat_sums (double[64]) += per-channel sum / sum of squares of what was written (if non-null), and with it
+// piv_sums (double[64]) += the same of what was written minus the channel's bias (the BatchNorm pivot, see bn2d_finalize)
 template <int KH, int KW, int SH, int SW>
 __global__ void __launch_bounds__(256) conv_fwd_kernel(const float* __restrict__ in, int Cin, int Hin, int Win,
                                                        const float* __restrict__ wpk, const float* __restrict__ bias,
                                                        float* __restrict__ out, int Hout, int Wout, size_t ob,
                                                        size_t oc, size_t orow, int PH, int PW,
                                                        const int32_t* __restrict__ out_len,
-                                                       double* __restrict__ stat_sums) {
+                                                       double* __restrict__ stat_sums, double* __restrict__ piv_sums) {
   using Gm = ConvGeom<KH, KW, SH, SW>;
   extern __shared__ __align__(16) float smem[];
   float* slab = smem;
@@ -96,9 +97,9 @@ __global__ void __launch_bounds__(256) conv_fwd_kernel(const float* __restrict__
   // epilogue: bias, mask, store, statistics
   const int d = d0 + dl;
   const int L = out_len ? out_len[b] : Wout;
-  float s1[8], s2[8];
+  float s1[8], s2[8], e1[8], e2[8];
 #pragma unroll
-  for (int c = 0; c < 8; ++c) s1[c] = s2[c] = 0.f;
+  for (int c = 0; c < 8; ++c) s1[c] = s2[c] = e1[c] = e2[c] = 0.f;
   if (d < Hout) {
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
@@ -113,23 +114,30 @@ __global__ void __launch_bounds__(256) conv_fwd_kernel(const float* __restrict__
           op[t] = v;
           s1[c] += v;
           s2[c] = fmaf(v, v, s2[c]);
+          const float dv = v - bv;
+          e1[c] += dv;
+          e2[c] = fmaf(dv, dv, e2[c]);
         }
       }
     }
   }
   if (stat_sums) {
-    __shared__ float red[2][8][CO];   // [sum|sumsq][warp][co]
+    __shared__ float red[4][8][CO];   // [sum|sumsq|pivoted sum|pivoted sumsq][warp][co]
     const int warp = tid / 32, lane = tid % 32;
 #pragma unroll
     for (int c = 0; c < 8; ++c) {
-      float a = warp_sum(s1[c]), q = warp_sum(s2[c]);
-      if (lane == 0) { red[0][warp][(warp / 2) * 8 + c] = a; red[1][warp][(warp / 2) * 8 + c] = q; }
+      float a = warp_sum(s1[c]), q = warp_sum(s2[c]), ea = warp_sum(e1[c]), eq = warp_sum(e2[c]);
+      if (lane == 0) {
+        red[0][warp][(warp / 2) * 8 + c] = a; red[1][warp][(warp / 2) * 8 + c] = q;
+        red[2][warp][(warp / 2) * 8 + c] = ea; red[3][warp][(warp / 2) * 8 + c] = eq;
+      }
     }
     __syncthreads();
-    if (tid < 2 * CO) {
+    if (tid < 4 * CO) {
       int which = tid / CO, co = tid % CO, w0 = (co / 8) * 2;
       double v = (double)red[which][w0][co] + (double)red[which][w0 + 1][co];
-      atomicAdd(&stat_sums[which * CO + co], v);
+      if (which < 2) atomicAdd(&stat_sums[which * CO + co], v);
+      else if (piv_sums) atomicAdd(&piv_sums[(which - 2) * CO + co], v);
     }
   }
 }
@@ -155,7 +163,14 @@ __global__ void pack_bwd_data_kernel(int parity, const float* __restrict__ w2, f
 }
 
 // ---- BatchNorm2d pieces -----------------------------------------------------------------------
-__global__ void bn2d_finalize_kernel(double count, const double* __restrict__ sums, const float* __restrict__ gamma,
+// The statistics come from raw sums, E[z^2] - E[z]^2, which cancel when a channel's mean is large against its spread;
+// the conv bias is what usually puts it there, so the conv epilogues also sum z - K and (z - K)^2 with the pivot
+// K = the channel's bias (piv, known before the conv runs), and a channel whose E[z^2] exceeds BN2D_RAW_MAX_CANCEL var
+// takes mean = K + S1/n, var = S2/n - (S1/n)^2 from those.  Channels below the threshold keep the raw result bit for
+// bit (as the sequence-wise BatchNorm of bn.cu does); there the raw variance is within a few 1e-7 of float64.
+constexpr double BN2D_RAW_MAX_CANCEL = 16.0;
+__global__ void bn2d_finalize_kernel(double count, const double* __restrict__ sums, const double* __restrict__ piv_sums,
+                                     const float* __restrict__ piv, const float* __restrict__ gamma,
                                      const float* __restrict__ beta, float* __restrict__ rmean,
                                      float* __restrict__ rvar, int training, float momentum, float eps,
                                      float* __restrict__ mean_invstd /*[2][32]*/) {
@@ -165,6 +180,13 @@ __global__ void bn2d_finalize_kernel(double count, const double* __restrict__ su
   if (training) {
     double m = sums[c] / count, v = sums[CO + c] / count - m * m;
     if (v < 0.0) v = 0.0;
+    const double ms = piv_sums[c] / count;      // mean - K
+    double vs = piv_sums[CO + c] / count - ms * ms;
+    if (vs < 0.0) vs = 0.0;
+    if (!(sums[CO + c] / count <= BN2D_RAW_MAX_CANCEL * vs)) {   // the raw sums cancel: take the pivoted ones
+      m = (double)piv[c] + ms;
+      v = vs;
+    }
     mean = (float)m;
     var = (float)v;
     double unb = count > 1.0 ? v * count / (count - 1.0) : v;
@@ -448,20 +470,21 @@ __global__ void __launch_bounds__(128) conv1_dw_kernel(int B, int Tin, int T, co
 template <int KH, int KW, int SH, int SW>
 static int launch_conv(const float* in, int B, int Cin, int Hin, int Win, const float* wpk, const float* bias,
                        float* out, int Hout, int Wout, size_t ob, size_t oc, size_t orow, int PH, int PW,
-                       const int32_t* out_len, double* sums, cudaStream_t st) {
+                       const int32_t* out_len, double* sums, double* piv_sums, cudaStream_t st) {
   using Gm = ConvGeom<KH, KW, SH, SW>;
   auto kern = conv_fwd_kernel<KH, KW, SH, SW>;
   DS2_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Gm::SMEM));
   dim3 grid(cdiv(Wout, TT), cdiv(Hout, TD), B);
   DS2_LAUNCH(kern, grid, 256, Gm::SMEM, st, in, Cin, Hin, Win, wpk, bias, out, Hout, Wout, ob, oc, orow, PH, PW,
-             out_len, sums);
+             out_len, sums, piv_sums);
   return DS2_OK;
 }
 
 // tensor-core 32->32 convolution (conv_tc.cu)
 int conv_tc_run(const float* in_cl, int B, int T, int R_in, const float* taps, int n_taps, int row_mul, int row_step,
                 int w_step, int out_row_mul, const ConvRows* rows, int n_classes, float* out, size_t ob, size_t oc,
-                size_t orow, const float* bias, const int32_t* out_len, double* stat_sums, cudaStream_t st);
+                size_t orow, const float* bias, const int32_t* out_len, double* stat_sums, double* piv_sums,
+                cudaStream_t st);
 int nchw_to_cl(int B, int R, int T, const float* in, float* out, cudaStream_t st);
 int pack_conv2_tc(const float* w2, float* wn_fwd, float* wd_bwd, cudaStream_t st);
 int conv2_wgrad_tc(const float* dz2, const float* a1, float* a1_shifted, float* part, int B, int T, float* dw2,
@@ -476,7 +499,8 @@ struct ConvWs {
   float* shifted;                  // tensor-core weight gradient: a1 delayed by 0,1,2,3 time steps
   float* wg_part;                  // tensor-core weight gradients: per-CTA partial tiles (conv_tc.cu)
   float* db_part;                  // conv bias gradients: per-block partial sums
-  double* sums;   // 4 x 64 doubles: fwd stats 1, fwd stats 2, bwd sums 2, bwd sums 1
+  double* sums;   // 4 x 64 doubles: fwd stats 1, fwd stats 2, then bwd sums 2, bwd sums 1 in the backward and the
+                  // pivoted fwd stats 1, 2 in the forward
 };
 static size_t conv_ws_carve(int B, int T, void* base, ConvWs& w) {
   const size_t Tp = (size_t)(T - 1) / 2 + 1;
@@ -521,13 +545,15 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
   conv_ws_carve(B, T, ws, W);
   DS2_PROF("conv_fwd", st);
   DS2_CHECK_CUDA(cudaMemsetAsync(W.sums, 0, 4 * 64 * sizeof(double), st));
+  double* piv1 = training ? W.sums + 128 : nullptr;
+  double* piv2 = training ? W.sums + 192 : nullptr;
   DS2_LAUNCH(pack_fwd_kernel, cdiv(41 * 11 * CO, 256), 256, 0, st, 1, 41, 11, w1, W.wpk1);
   DS2_LAUNCH(pack_fwd_kernel, cdiv(CO * 21 * 11 * CO, 256), 256, 0, st, CO, 21, 11, w2, W.wpk2);
   int rc = launch_conv<41, 11, 2, 2>(x, B, 1, F, T, W.wpk1, b1, z1, D1, Tp, (size_t)CO * D1 * Tp, (size_t)D1 * Tp,
-                                     (size_t)Tp, 20, 5, out_len, training ? W.sums : nullptr, st);
+                                     (size_t)Tp, 20, 5, out_len, training ? W.sums : nullptr, piv1, st);
   if (rc) return rc;
-  DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D1 * Tp, W.sums, g1, be1, rm1, rv1, training, momentum,
-             eps, stats);
+  DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D1 * Tp, W.sums, W.sums + 128, b1, g1, be1, rm1, rv1,
+             training, momentum, eps, stats);
   DS2_LAUNCH(bn_act_kernel, 132 * 8, 256, 0, st, B, D1, Tp, z1, stats, g1, be1, out_len, a1);
   if (tensor_core_mode()) {
     // conv2 on wgmma: channels-last copy of a1, packed taps, implicit GEMM with the kw taps folded into N
@@ -537,14 +563,14 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
     if (rc) return rc;
     const ConvRows rows = {D2, 21, -10, 0, 0};
     rc = conv_tc_run(W.cl, B, Tp, D1, W.taps_f, 21, 2, 1, 1, 1, &rows, 1, z2, (size_t)CO * D2 * Tp, (size_t)D2 * Tp,
-                     (size_t)Tp, b2, out_len, training ? W.sums + 64 : nullptr, st);
+                     (size_t)Tp, b2, out_len, training ? W.sums + 64 : nullptr, piv2, st);
   } else {
     rc = launch_conv<21, 11, 2, 1>(a1, B, CO, D1, Tp, W.wpk2, b2, z2, D2, Tp, (size_t)CO * D2 * Tp, (size_t)D2 * Tp,
-                                   (size_t)Tp, 10, 5, out_len, training ? W.sums + 64 : nullptr, st);
+                                   (size_t)Tp, 10, 5, out_len, training ? W.sums + 64 : nullptr, piv2, st);
   }
   if (rc) return rc;
-  DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D2 * Tp, W.sums + 64, g2, be2, rm2, rv2, training,
-             momentum, eps, stats + 64);
+  DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D2 * Tp, W.sums + 64, W.sums + 192, b2, g2, be2, rm2,
+             rv2, training, momentum, eps, stats + 64);
   DS2_LAUNCH(bn_act_transpose_kernel, dim3(cdiv(Tp, 32), cdiv(CO * D2, 32), B), dim3(32, 8), 0, st, B, D2, Tp, z2,
              stats + 64, g2, be2, out_len, y);
   return DS2_OK;
@@ -615,14 +641,14 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
     if (rc) return rc;
     const ConvRows rows[2] = {{41, 11, 5, 0, 0}, {40, 10, 5, 1, 1}};
     rc = conv_tc_run(W.cl, B, Tp, D2, W.taps_b, 21, 1, -1, 2, 2, rows, 2, W.da1, ob, oc, (size_t)Tp, nullptr, nullptr,
-                     nullptr, st);
+                     nullptr, nullptr, st);
     if (rc) return rc;
   } else {
     rc = launch_conv<11, 11, 1, 1>(W.du2, B, CO, D2, Tp, W.wTe, nullptr, W.da1, 41, Tp, ob, oc, (size_t)2 * Tp, 5, 5,
-                                   nullptr, nullptr, st);
+                                   nullptr, nullptr, nullptr, st);
     if (rc) return rc;
     rc = launch_conv<10, 11, 1, 1>(W.du2, B, CO, D2, Tp, W.wTo, nullptr, W.da1 + Tp, 40, Tp, ob, oc, (size_t)2 * Tp, 4, 5,
-                                   nullptr, nullptr, st);
+                                   nullptr, nullptr, nullptr, st);
     if (rc) return rc;
   }
   // ---- stage 1: BN1 + Hardtanh + mask backward (natural layout, in place over da1)

@@ -75,6 +75,7 @@ struct ConvTcParams {
   const float* bias;                       // [32] or null
   const int32_t* out_len;                  // [B] or null: positions t >= out_len[b] are written as 0
   double* stat_sums;                       // [64] or null
+  double* piv_sums;                        // [64] or null: the same sums of the output minus the bias (BatchNorm pivot)
 };
 
 // Tile u of the list: class 0's tiles, then class 1's, each ordered (b, d, time tile) with the time tile fastest.
@@ -226,7 +227,7 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
       const int c = w * 8 + cc;
       const float bv = p.bias ? p.bias[c] : 0.f;
       float* op = p.out + (size_t)t.b * p.ob + (size_t)c * p.oc + (size_t)orow_idx * p.orow;
-      float s1 = 0.f, s2 = 0.f;
+      float s1 = 0.f, s2 = 0.f, e1 = 0.f, e2 = 0.f;
       for (int to = lane; to < TO; to += 32) {
         const int tt = t.t0 + to;
         if (tt < p.T) {
@@ -234,6 +235,9 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
           op[tt] = val;
           s1 += val;
           s2 = fmaf(val, val, s2);
+          const float dv = val - bv;
+          e1 += dv;
+          e2 = fmaf(dv, dv, e2);
         }
       }
       if (p.stat_sums) {
@@ -242,6 +246,14 @@ __global__ void __launch_bounds__(cv::THREADS, 1) conv_tc_kernel(const __grid_co
         if (lane == 0) {
           atomicAdd(&p.stat_sums[c], (double)s1);
           atomicAdd(&p.stat_sums[CH + c], (double)s2);
+        }
+      }
+      if (p.piv_sums) {
+        e1 = warp_sum(e1);
+        e2 = warp_sum(e2);
+        if (lane == 0) {
+          atomicAdd(&p.piv_sums[c], (double)e1);
+          atomicAdd(&p.piv_sums[CH + c], (double)e2);
         }
       }
     }
@@ -300,7 +312,8 @@ static int make_tmap_cl(CUtensorMap* out, const float* base, int T, int R, int B
 // channels-last; taps: (n_taps, 352, 32).
 int conv_tc_run(const float* in_cl, int B, int T, int R_in, const float* taps, int n_taps, int row_mul, int row_step,
                 int w_step, int out_row_mul, const ConvRows* rows, int n_classes, float* out, size_t ob, size_t oc,
-                size_t orow, const float* bias, const int32_t* out_len, double* stat_sums, cudaStream_t st) {
+                size_t orow, const float* bias, const int32_t* out_len, double* stat_sums, double* piv_sums,
+                cudaStream_t st) {
   ConvTcParams p{};
   int rc = make_tmap_cl(&p.tmA, in_cl, T, R_in, B);
   if (rc) return rc;
@@ -315,7 +328,7 @@ int conv_tc_run(const float* in_cl, int B, int T, int R_in, const float* taps, i
   }
   p.row_mul = row_mul; p.row_step = row_step; p.w_step = w_step; p.out_row_mul = out_row_mul;
   p.out = out; p.ob = ob; p.oc = oc; p.orow = orow;
-  p.bias = bias; p.out_len = out_len; p.stat_sums = stat_sums;
+  p.bias = bias; p.out_len = out_len; p.stat_sums = stat_sums; p.piv_sums = piv_sums;
   static DeviceOnce attr_once;
   if (attr_once.first()) {
     DS2_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cv::SMEM_BYTES));
