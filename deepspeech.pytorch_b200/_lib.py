@@ -2,8 +2,11 @@
 
 There is no fallback: if the shared library is missing or a call fails, an exception is raised.
 """
+import contextlib
 import ctypes as C
 import os
+
+import torch  # also loads libcudart.so.12, which the library links against
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libds2_b200.so")
@@ -97,7 +100,6 @@ def get_lib():
         if not os.path.exists(LIB_PATH):
             raise Ds2Error(f"{LIB_PATH} not found: build it with `make -C deepspeech.pytorch_b200/csrc` "
                            "(or __graft_entry__.build()); there is no CPU / eager fallback")
-        import torch  # noqa: F401  (loads libcudart.so.12 that the library links against)
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in PROTOTYPES.items():
             fn = getattr(lib, name)
@@ -110,6 +112,35 @@ def check(rc, what=""):
     if rc != 0:
         msg = get_lib().ds2_last_error().decode(errors="replace")
         raise Ds2Error(f"{what} failed with code {rc}: {msg}")
+
+
+def current_stream():
+    """the `stream` argument of the C-ABI: the current stream of the CURRENT device, so callers make the tensors'
+    device current first (kernels, TMA descriptors and the per-device shared-memory opt-ins all bind to it)"""
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+@contextlib.contextmanager
+def precision_mode(code):
+    """run the block in the library's precision mode `code` (PREC_*) and restore the mode it found on exit, also on
+    an exception; `None` leaves the mode alone"""
+    if code is None:
+        yield
+        return
+    lib = get_lib()
+    saved = lib.ds2_get_precision()
+    if saved != code:
+        check(lib.ds2_set_precision(code), "ds2_set_precision")
+    try:
+        yield
+    finally:
+        lib.ds2_set_precision(saved)
+
+
+def autocast(precision):
+    """the reference's autocast around a forward at the model's `precision`: 16 selects the fp16 mode for the block,
+    any other value leaves the process-wide mode (`set_precision`) alone"""
+    return precision_mode(PREC_F16 if precision == 16 else None)
 
 
 def ptr(t):

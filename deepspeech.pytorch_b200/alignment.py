@@ -10,13 +10,12 @@ at the default 10 ms stride).  A character's score is the mean posterior probabi
 word (a maximal run of non-space characters) scores the frame-weighted mean of its characters; the record's `score`
 is the path's total log-probability.  A transcript the audio cannot hold (too few frames for its characters) is
 reported with `feasible: false`, `score: null` and no character or word records."""
-import ctypes as C
 import json
 
 import torch
 
 from . import _lib
-from ._lib import check, get_lib, ptr
+from ._lib import check, current_stream, get_lib, ptr
 from .input_pipeline import SpectrogramBatcher
 
 __all__ = ["forced_align", "frame_seconds", "char_scores", "alignment_record", "unsort_rows", "align_audio",
@@ -82,7 +81,7 @@ def forced_align(emissions, input_lengths, targets, target_lengths, blank=0, log
         check(lib.ds2_ctc_align(T, B, Cn, ptr(x), int(not log_probs), ptr(targets) if targets.numel() else None,
                                 ptr(in_len_d), ptr(tgt_len_d), max_l, int(blank), ptr(labels), ptr(frame_lp),
                                 ptr(spans) if max_l else None, ptr(scores), ptr(ws), nws,
-                                C.c_void_p(torch.cuda.current_stream().cuda_stream)), "ds2_ctc_align")
+                                current_stream()), "ds2_ctc_align")
     return labels, frame_lp, spans, scores
 
 

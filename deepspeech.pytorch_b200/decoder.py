@@ -9,7 +9,7 @@ defined by the rules in csrc/beam_decode.cu (DESIGN.md §5.7); ctcdecode and Ken
 import torch
 
 from . import _lib
-from ._lib import check, get_lib, ptr
+from ._lib import check, current_stream, get_lib, ptr
 
 
 class GreedyDecoder:
@@ -21,9 +21,13 @@ class GreedyDecoder:
 
     def decode_indices(self, probs, sizes=None):
         """probs (B,T,C) CUDA -> (labels (B,T) int32, offsets (B,T) int32, counts (B) int32) on the CPU"""
+        labels, offsets, counts = self.decode_indices_device(probs, sizes)
+        return labels.cpu(), offsets.cpu(), counts.cpu()
+
+    def decode_indices_device(self, probs, sizes=None):
+        """`decode_indices` left on the device: the first counts[b] entries of row b are set, the rest are 0"""
         if not probs.is_cuda:
             raise _lib.Ds2Error("GreedyDecoder: probs must be a CUDA tensor")
-        import ctypes as C
         probs = probs.float().contiguous()
         B, T, Cn = probs.shape
         dev = probs.device
@@ -33,10 +37,8 @@ class GreedyDecoder:
         sz = None if sizes is None else torch.as_tensor(sizes).int().to(dev)
         with torch.cuda.device(dev):                         # launches bind to the current device
             check(get_lib().ds2_greedy_decode(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, ptr(labels),
-                                              ptr(offsets), ptr(counts),
-                                              C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                  "ds2_greedy_decode")
-        return labels.cpu(), offsets.cpu(), counts.cpu()
+                                              ptr(offsets), ptr(counts), current_stream()), "ds2_greedy_decode")
+        return labels, offsets, counts
 
     def convert_to_strings(self, sequences, sizes=None, remove_repetitions=False, return_offsets=False):
         """label-index sequences -> [[str]] (decoder.py:125-163): blanks dropped, optional repeat collapsing; used by
@@ -96,7 +98,6 @@ class BeamCTCDecoder:
         """probs (B,T,C) fp32 probabilities (a CPU tensor is copied to the current CUDA device) -> on the CPU:
         labels (B,W,T) int32, scores (B,W) float64 (-log-likelihood, +inf for unused slots), timesteps (B,W,T) int32,
         lengths (B,W) int32, n_beams (B) int32.  With a language model the scores include its terms (rule L5)"""
-        import ctypes as C
         if probs.dim() != 3:
             raise _lib.Ds2Error(f"BeamCTCDecoder: probs must be (B, T, C), got {tuple(probs.shape)}")
         if sizes is not None:                                # the kernel reads one length per utterance
@@ -121,7 +122,7 @@ class BeamCTCDecoder:
             scores = torch.empty(B, Wa, dtype=torch.float64, device=dev)
             n_beams = torch.empty(B, dtype=torch.int32, device=dev)
             sz = None if sizes is None else sizes.to(device=dev, dtype=torch.int32).contiguous()
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+            stream = current_stream()
             if lm is None:
                 check(lib.ds2_beam_decode(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
                                           self.cutoff_prob, ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores),
@@ -138,7 +139,6 @@ class BeamCTCDecoder:
         if self.lm is not None:
             labels, lengths = self.decode_best_grid(probs, sizes, [(self.alpha, self.beta)])
             return labels[0], lengths[0]
-        import ctypes as C
         probs = probs.to(torch.float32).contiguous()
         B, T, Cn = probs.shape
         dev, W = probs.device, self.beam_width
@@ -155,8 +155,7 @@ class BeamCTCDecoder:
             sz = None if sizes is None else torch.as_tensor(sizes).to(device=dev, dtype=torch.int32).contiguous()
             check(lib.ds2_beam_decode(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
                                       self.cutoff_prob, ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores),
-                                      ptr(n_beams), ptr(ws), nws, C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                  "ds2_beam_decode")
+                                      ptr(n_beams), ptr(ws), nws, current_stream()), "ds2_beam_decode")
         return labels[:, 0].contiguous(), lengths[:, 0].contiguous()
 
     def decode_best_grid(self, probs, sizes, pairs):
@@ -190,9 +189,7 @@ class BeamCTCDecoder:
             check(lib.ds2_beam_decode_lm_grid(B, T, Cn, ptr(probs), ptr(sz), self.blank_index, W, self.cutoff_top_n,
                                               self.cutoff_prob, ptr(lm), self.lm.order, K,
                                               pr.ctypes.data_as(C.c_void_p), self.lm.space, ptr(labels),
-                                              ptr(lengths), ptr(ws), nws,
-                                              C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                  "ds2_beam_decode_lm_grid")
+                                              ptr(lengths), ptr(ws), nws, current_stream()), "ds2_beam_decode_lm_grid")
         return labels, lengths
 
     def convert_to_strings(self, out, seq_len):

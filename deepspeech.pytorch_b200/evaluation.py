@@ -9,7 +9,6 @@ other decoder object goes through the `metrics.py` classes, as in the reference.
 Differences from the reference: audio is read with `inference.load_audio` (WAV only); the rates use `max(1, n)` as
 `metrics.py` does where the reference would divide by zero on empty references; noise injection and speed / volume
 perturbation are refused by the batcher."""
-import ctypes as C
 import json
 import os
 from pathlib import Path
@@ -17,7 +16,7 @@ from pathlib import Path
 import torch
 
 from . import _lib
-from ._lib import check, get_lib, ptr
+from ._lib import check, current_stream, get_lib, ptr
 from .decoder import BeamCTCDecoder, GreedyDecoder, load_decoder
 from .inference import load_audio
 from .input_pipeline import SpectrogramBatcher
@@ -155,8 +154,7 @@ def error_counts(labels, lengths, targets, target_sizes, blank, space, pair_coun
         ws = torch.empty(max(nws, 1), dtype=torch.uint8, device=dev)
         check(lib.ds2_error_counts(K, B, T, ptr(labels), ptr(lengths), ptr(targets) if targets.numel() else None,
                                    targets.numel(), ptr(sizes), max_size, int(blank), int(space), ptr(out),
-                                   ptr(pair_counts), ptr(ws), nws,
-                                   C.c_void_p(torch.cuda.current_stream().cuda_stream)), "ds2_error_counts")
+                                   ptr(pair_counts), ptr(ws), nws, current_stream()), "ds2_error_counts")
     return out
 
 
@@ -175,23 +173,14 @@ def best_path(decoder, probs, sizes):
     """the best path of `decoder` on the device: -> labels (B,T) int32, lengths (B) int32, CUDA.  GreedyDecoder: the
     greedy kernel; BeamCTCDecoder: beam 0 of `ds2_beam_decode`, or of the grid search with the decoder's (alpha,
     beta) when it has a language model"""
-    dev = probs.device
     probs = probs.to(torch.float32).contiguous()
-    B, T, Cn = probs.shape
-    sz = None if sizes is None else torch.as_tensor(sizes).to(device=dev, dtype=torch.int32).contiguous()
+    sz = None if sizes is None else torch.as_tensor(sizes).to(device=probs.device, dtype=torch.int32).contiguous()
     if isinstance(decoder, BeamCTCDecoder):
         if decoder.lm is not None:
             labels, lengths = decoder.decode_best_grid(probs, sz, [(decoder.alpha, decoder.beta)])
             return labels[0], lengths[0]
         return decoder.decode_best(probs, sz)
-    lib = get_lib()
-    with torch.cuda.device(dev):
-        labels = torch.empty(B, T, dtype=torch.int32, device=dev)
-        offsets = torch.empty_like(labels)
-        counts = torch.empty(B, dtype=torch.int32, device=dev)
-        check(lib.ds2_greedy_decode(B, T, Cn, ptr(probs), ptr(sz), decoder.blank_index, ptr(labels), ptr(offsets),
-                                    ptr(counts), C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-              "ds2_greedy_decode")
+    labels, _, counts = decoder.decode_indices_device(probs, sz)
     return labels, counts
 
 
@@ -203,14 +192,8 @@ def _on_device_path(decoder, target_decoder):
 def model_forward(model, inputs, input_sizes, precision, logits=False):
     """the eval forward of validation.py:160-161: precision 16 runs in the library's fp16 mode (the reference's
     autocast), as run_transcribe does.  `logits=True` returns the logits instead of the eval softmax."""
-    lib = get_lib()
-    saved = lib.ds2_get_precision()
-    if precision == 16:
-        lib.ds2_set_precision(_lib.PREC_F16)
-    try:
-        return model(inputs, input_sizes, logits=True) if logits else model(inputs, input_sizes)
-    finally:
-        lib.ds2_set_precision(saved)
+    with _lib.autocast(precision):
+        return model(inputs, input_sizes, logits=logits)
 
 
 @torch.no_grad()

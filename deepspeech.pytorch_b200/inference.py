@@ -9,7 +9,6 @@ a file in one `ds2_spectrogram_batch` launch.
 Deviation: the reference's `get_chunks` can produce an empty trailing chunk (the duration is rounded up to whole
 seconds first, e.g. 1.01 s at 0.5 s chunks gives [1.5 s, 2 s) of a 1.01 s signal).  Its spectrogram would be a single
 all-zero frame; here that chunk is skipped."""
-import ctypes as C
 import math
 from typing import Iterator, List, Tuple
 
@@ -17,8 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import check, get_lib, ptr
-from .input_pipeline import analysis_window
+from .input_pipeline import SpectrogramBatcher, spect_geometry
 
 __all__ = ["load_audio", "chunk_bounds", "ChunkSpectrogramParser", "run_transcribe", "decode_results"]
 
@@ -79,44 +77,20 @@ class ChunkSpectrogramParser:
     constant padding (librosa >= 0.10)."""
 
     def __init__(self, audio_conf, normalize: bool = False, device="cuda"):
-        self.sample_rate = int(audio_conf.sample_rate)
-        self.n_fft = int(audio_conf.sample_rate * audio_conf.window_size)
-        self.hop = int(audio_conf.sample_rate * audio_conf.window_stride)
+        self.sample_rate, self.n_fft, self.hop, _ = spect_geometry(audio_conf)
         self.normalize = normalize
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise _lib.Ds2Error("ChunkSpectrogramParser: needs a CUDA device; there is no CPU path")
-        wname = audio_conf.window.value if hasattr(audio_conf.window, "value") else str(audio_conf.window)
-        self.window_np = analysis_window(wname, self.n_fft)
-        self._window = None
+        self._batcher = SpectrogramBatcher(audio_conf, normalize=normalize, device=self.device)
 
     def spectrograms(self, y: np.ndarray, chunk_size_seconds: float = -1) -> List[torch.Tensor]:
+        # every chunk but a clipped last one has int(chunk * sr) samples, so the batcher's stable sort by descending
+        # length leaves them in file order: row i is chunk i
         y = np.ascontiguousarray(y, dtype=np.float32)
         bounds = chunk_bounds(len(y), self.sample_rate, chunk_size_seconds)
-        n = len(bounds)
-        lens = [e - s for s, e in bounds]
-        frames = [1 + l // self.hop for l in lens]
-        offs = np.zeros(n + 1, np.int64)
-        offs[1:] = np.cumsum(lens)
-        # the chunks are packed back to back: int(i * chunk * sr) can make neighbouring chunks overlap by a sample
-        wave = np.concatenate([y[s:e] for s, e in bounds])
-        F, Tmax = self.n_fft // 2 + 1, max(frames)
-        dev = self.device
-        with torch.cuda.device(dev):
-            if self._window is None:
-                self._window = torch.from_numpy(self.window_np).to(dev)
-            wave_d = torch.from_numpy(wave).to(dev)
-            offs_d = torch.from_numpy(offs).to(dev)
-            rows_d = torch.arange(n, dtype=torch.int32, device=dev)      # file order
-            out = torch.empty(n, 1, F, Tmax, device=dev)
-            lib = get_lib()
-            nws = lib.ds2_spectrogram_workspace_bytes(n)
-            ws = torch.empty(nws, dtype=torch.uint8, device=dev)
-            check(lib.ds2_spectrogram_batch(n, ptr(wave_d), ptr(offs_d), ptr(rows_d), max(lens), self.n_fft, self.hop,
-                                            ptr(self._window), 0, int(bool(self.normalize)), ptr(out), Tmax, ptr(ws),
-                                            nws, C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                  "ds2_spectrogram_batch")
-        return [out[i, 0, :, :frames[i]] for i in range(n)]
+        out = self._batcher([y[s:e] for s, e in bounds], [()] * len(bounds))[0]
+        return [out[i, 0, :, :1 + (e - s) // self.hop] for i, (s, e) in enumerate(bounds)]
 
     def parse_audio(self, audio_path, chunk_size_seconds: float = -1) -> Iterator[torch.Tensor]:
         yield from self.spectrograms(load_audio(audio_path), chunk_size_seconds)
@@ -127,20 +101,14 @@ def run_transcribe(audio_path, spect_parser: ChunkSpectrogramParser, model, deco
     """inference.py:79-99: the chunks' forwards carry the recurrent states `hs`; the outputs are concatenated along
     time (on the device) and decoded.  `precision == 16` runs each forward in the fp16 mode (the reference's
     autocast); otherwise the model's own `precision` applies.  -> decoder.decode(all_outs)."""
-    lib = get_lib()
     hs = None
     outs = []
     with torch.no_grad():
         for spect in spect_parser.parse_audio(audio_path, chunk_size_seconds):
             spect = spect.contiguous().view(1, 1, spect.size(0), spect.size(1)).to(device)
             input_sizes = torch.IntTensor([spect.size(3)]).int()
-            saved = lib.ds2_get_precision()
-            if precision == 16:
-                lib.ds2_set_precision(_lib.PREC_F16)
-            try:
+            with _lib.autocast(precision):
                 out, _, hs = model(spect, input_sizes, hs)
-            finally:
-                lib.ds2_set_precision(saved)
             outs.append(out)
     return decoder.decode(torch.cat(outs, dim=1))
 

@@ -18,7 +18,6 @@ With `augmentation_conf.spec_augment` set, it also replaces the reference's per-
 random numbers (`spec_augment_draws`, the reference's generators in the reference's order) and `ds2_spec_augment`
 (csrc/spec_augment.cu) does the time warp and the masks on the batch.
 """
-import ctypes as C
 import math
 import random
 from typing import List, Sequence
@@ -27,7 +26,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import check, get_lib, ptr
+from ._lib import check, current_stream, get_lib, ptr
 
 # Ds2SpecAugDraws (include/ds2_b200.h), one record per utterance
 SPEC_AUG_DRAWS_DTYPE = np.dtype([("idx", "<i4"), ("d", "<i4"), ("f0", "<i4"), ("f", "<i4"), ("t0", "<i4"),
@@ -68,7 +67,7 @@ def spec_augment_draws(frames: Sequence[int], n_freq: int = 161) -> np.ndarray:
 def _launch_spec_augment(spec, out, frames_d, draws_d, ws, nws):
     B, _, F, Tmax = spec.shape
     check(get_lib().ds2_spec_augment(B, F, Tmax, ptr(spec), ptr(frames_d), ptr(draws_d), ptr(out), ptr(ws), nws,
-                                     C.c_void_p(torch.cuda.current_stream().cuda_stream)), "ds2_spec_augment")
+                                     current_stream()), "ds2_spec_augment")
 
 
 def spec_augment_batch(inputs: torch.Tensor, frames: Sequence[int], draws: np.ndarray = None) -> torch.Tensor:
@@ -118,6 +117,14 @@ def analysis_window(name: str, n: int) -> np.ndarray:
     return w.astype(np.float32)
 
 
+def spect_geometry(spect_cfg):
+    """-> (sample_rate, n_fft, hop, window name) of a SpectConfig: n_fft = win_length = sample_rate * window_size,
+    hop = sample_rate * window_stride (data_loader.py:78-80)"""
+    window = spect_cfg.window.value if hasattr(spect_cfg.window, "value") else str(spect_cfg.window)
+    return (int(spect_cfg.sample_rate), int(spect_cfg.sample_rate * spect_cfg.window_size),
+            int(spect_cfg.sample_rate * spect_cfg.window_stride), window)
+
+
 class SpectrogramBatcher:
     """callable: (waves, transcripts) -> (inputs cuda (B,1,F,Tmax), targets int64, input_percentages f32,
     target_sizes int32) — the `_collate_fn` tuple, with `inputs` already on the device.
@@ -141,9 +148,7 @@ class SpectrogramBatcher:
                 raise _lib.Ds2Error("SpectrogramBatcher: speed / volume perturbation (augmentation."
                                     "speed_volume_perturb) is not implemented on the GPU input pipeline")
             self.spec_augment = bool(augmentation_conf.spec_augment)
-        self.n_fft = int(spect_cfg.sample_rate * spect_cfg.window_size)
-        self.hop = int(spect_cfg.sample_rate * spect_cfg.window_stride)
-        wname = spect_cfg.window.value if hasattr(spect_cfg.window, "value") else str(spect_cfg.window)
+        _, self.n_fft, self.hop, wname = spect_geometry(spect_cfg)
         self.window = torch.from_numpy(analysis_window(wname, self.n_fft)).to(self.device)
         if pad_mode not in ("constant", "reflect"):
             raise ValueError("pad_mode must be 'constant' (librosa >= 0.10) or 'reflect' (librosa < 0.10)")
@@ -217,8 +222,7 @@ class SpectrogramBatcher:
             ws = torch.empty(nws + nws_aug, dtype=torch.uint8, device=dev)
             check(lib.ds2_spectrogram_batch(B, ptr(wave_d), ptr(offs_d), ptr(rows_d), max(lens), self.n_fft, self.hop,
                                             ptr(self.window), self.pad_reflect, self.normalize, ptr(spec), Tmax, ptr(ws),
-                                            nws, C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                  "ds2_spectrogram_batch")
+                                            nws, current_stream()), "ds2_spectrogram_batch")
             if aug:
                 frames_d = meta_d[B + 1:2 * (B + 1)].view(torch.int32)[B:2 * B]
                 draws_d = meta_d[2 * (B + 1):n_meta]

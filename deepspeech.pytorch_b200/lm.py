@@ -262,7 +262,7 @@ class LanguageModel:
         """the ds2_lm_build buffer on `device` (a CUDA torch.device), built on the current stream at the first call"""
         import ctypes as C
         import torch
-        from ._lib import check, get_lib, ptr
+        from ._lib import check, current_stream, get_lib, ptr
         key = torch.device(device).index
         if key in self._tables:
             return self._tables[key]
@@ -283,7 +283,7 @@ class LanguageModel:
         with torch.cuda.device(dev):
             check(lib.ds2_lm_build(n, counts, arr(up[:n]), arr(up[n:2 * n]), arr(up[2 * n:]), len(m.words),
                                    m.index[b"<s>"], len(tr.mask), ptr(tmask), ptr(tfirst), ptr(tword), ptr(buf),
-                                   nbytes, C.c_void_p(torch.cuda.current_stream().cuda_stream)), "ds2_lm_build")
+                                   nbytes, current_stream()), "ds2_lm_build")
         self._tables[key] = buf
         return buf
 

@@ -130,16 +130,8 @@ class DeepSpeech(_Base):
         eval softmax (forced alignment wants log-probabilities, not probabilities)."""
         if not x.is_cuda:
             raise _lib.Ds2Error("DeepSpeech (CUDA shell): input must be a CUDA tensor; there is no CPU path")
-        if self.precision == 16:
-            lib = _lib.get_lib()
-            saved = lib.ds2_get_precision()
-            if saved != _lib.PREC_F16:
-                lib.ds2_set_precision(_lib.PREC_F16)
-                try:
-                    return self._forward(x, lengths, hs, logits)
-                finally:
-                    lib.ds2_set_precision(saved)
-        return self._forward(x, lengths, hs, logits)
+        with _lib.autocast(self.precision):
+            return self._forward(x, lengths, hs, logits)
 
     def _forward(self, x, lengths, hs: Optional[list] = None, logits: bool = False):
         lengths = torch.as_tensor(lengths).cpu().int()
@@ -153,13 +145,8 @@ class DeepSpeech(_Base):
         dev = x.device
         len_dev = output_lengths.to(dev, non_blocking=True)
         training = self.training
-        sm = self.conv.seq_module
-        y = ops.ConvFrontend.apply(x.float(), len_dev, sm[0].weight, sm[0].bias, sm[1].weight, sm[1].bias,
-                                   sm[1].running_mean, sm[1].running_var, sm[3].weight, sm[3].bias, sm[4].weight,
-                                   sm[4].bias, sm[4].running_mean, sm[4].running_var, training, BN_MOMENTUM, BN_EPS)
+        y = self.conv_block(x.float(), len_dev, training)
         if training:
-            sm[1].num_batches_tracked += 1
-            sm[4].num_batches_tracked += 1
             hook = getattr(self, "front_end_grad_hook", None)
             if hook is not None and y.requires_grad:
                 # fires when autograd reaches the front-end, i.e. when every other gradient is final
@@ -185,23 +172,52 @@ class DeepSpeech(_Base):
                     h0, c0 = hs[i]
                 else:
                     h0 = hs[i]
-            bn = layer.batch_norm.module if layer.batch_norm is not None else None
-            y, hn, cn = ops.RnnLayer.apply(y, len_dev, layer.rnn_code, self.bidirectional, training, BN_MOMENTUM,
-                                           BN_EPS, bn.weight if bn else None, bn.bias if bn else None,
-                                           bn.running_mean if bn else None, bn.running_var if bn else None, h0, c0,
-                                           *layer.weights())
-            if bn is not None and training:
-                bn.num_batches_tracked += 1
+            y, hn, cn = self.rnn_block(i, y, len_dev, training, h0, c0)
             new_hs.append((hn, cn) if layer.rnn_code == _lib.RNN_LSTM else hn)
         _mark(y, "head")
         if not self.bidirectional:
-            y = ops.Lookahead.apply(y, self.lookahead[0].conv.weight)
+            y = self.lookahead_block(y)
+        out = self.head_block(y, training, not (training or logits))   # eval: softmax (model.py:72-77)
+        return out.transpose(0, 1), output_lengths, new_hs
+
+    # ------------------------------------------------------------------ blocks (model.py:157-201)
+    # Each runs one op on this model's parameters and counts a BatchNorm batch when `training` is set.  `training` is
+    # an argument, not `self.training`: the streaming forward runs the blocks in eval mode whatever the module's mode.
+    def conv_block(self, x, len_dev, training):
+        """x (B, 1, 161, T) fp32, len_dev (B) int32 output lengths -> (T', B, 1312), T' = (T - 1) // 2 + 1"""
+        sm = self.conv.seq_module
+        y = ops.ConvFrontend.apply(x, len_dev, sm[0].weight, sm[0].bias, sm[1].weight, sm[1].bias, sm[1].running_mean,
+                                   sm[1].running_var, sm[3].weight, sm[3].bias, sm[4].weight, sm[4].bias,
+                                   sm[4].running_mean, sm[4].running_var, training, BN_MOMENTUM, BN_EPS)
+        if training:
+            sm[1].num_batches_tracked += 1
+            sm[4].num_batches_tracked += 1
+        return y
+
+    def rnn_block(self, i, x, len_dev, training, h0=None, c0=None):
+        """recurrent layer i: x (T, B, In), len_dev (B) int32 descending, initial state h0 (and c0 for an LSTM)
+        (D, B, H) or None -> (y (T, B, H), hn, cn or None)"""
+        layer = self.rnns[i]
+        bn = layer.batch_norm.module if layer.batch_norm is not None else None
+        out = ops.RnnLayer.apply(x, len_dev, layer.rnn_code, self.bidirectional, training, BN_MOMENTUM, BN_EPS,
+                                 bn.weight if bn else None, bn.bias if bn else None, bn.running_mean if bn else None,
+                                 bn.running_var if bn else None, h0, c0, *layer.weights())
+        if bn is not None and training:
+            bn.num_batches_tracked += 1
+        return out
+
+    def lookahead_block(self, x):
+        """x (T, B, H) -> (T, B, H), the Hardtanh included (unidirectional models only)"""
+        return ops.Lookahead.apply(x, self.lookahead[0].conv.weight)
+
+    def head_block(self, x, training, softmax):
+        """x (T, B, H) -> (T, B, C): logits, or their softmax over C when `softmax` is set"""
         fbn, flin = self.fc[0].module[0], self.fc[0].module[1]
-        out = ops.FcHead.apply(y, fbn.weight, fbn.bias, fbn.running_mean, fbn.running_var, flin.weight, training,
-                               BN_MOMENTUM, BN_EPS, not (training or logits))   # eval: softmax (model.py:72-77)
+        out = ops.FcHead.apply(x, fbn.weight, fbn.bias, fbn.running_mean, fbn.running_var, flin.weight, training,
+                               BN_MOMENTUM, BN_EPS, softmax)
         if training:
             fbn.num_batches_tracked += 1
-        return out.transpose(0, 1), output_lengths, new_hs
+        return out
 
     # ------------------------------------------------------------------ loss (model.py:203,241-249)
     def _ctc_criterion(self, logits_tbc, targets, input_sizes, target_sizes):

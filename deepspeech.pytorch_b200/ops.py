@@ -13,7 +13,7 @@ import weakref
 import torch
 
 from . import _lib
-from ._lib import RnnDesc, check, get_lib, ptr, ptr_array
+from ._lib import RnnDesc, check, current_stream, get_lib, precision_mode, ptr, ptr_array
 
 _workspaces = {}
 # Gradient sinks: parameter storage address -> the tensor its gradient must be WRITTEN into (a view of the flat
@@ -56,12 +56,6 @@ def _out(sink, like):
     return t, t
 
 
-def _stream():
-    """current stream of the CURRENT device — every op runs under `_on_device`, which makes the tensors' device
-    current first (kernels, TMA descriptors and the per-device shared-memory opt-ins all bind to it)"""
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _on_device(fn):
     """run a Function.forward/backward with the device of its first CUDA tensor argument made current: the C
     library launches on the current device, so a model on cuda:1 in a process whose current device is cuda:0
@@ -73,21 +67,13 @@ def _on_device(fn):
             raise _lib.Ds2Error(f"{fn.__qualname__}: no CUDA tensor among the arguments (the CUDA path has no CPU "
                                 "fallback)")
         with torch.cuda.device(dev):
-            lib = get_lib()
             if fn.__name__ == "forward":
-                ctx.ds2_prec = lib.ds2_get_precision()
+                ctx.ds2_prec = get_lib().ds2_get_precision()
                 return fn(ctx, *args)
             # backward: same arithmetic mode as the forward that recorded the graph (the switch is process-global
             # and a precision-16 model sets it only for the duration of its own forward)
-            cur = lib.ds2_get_precision()
-            want = getattr(ctx, "ds2_prec", cur)
-            if want == cur:
+            with precision_mode(ctx.ds2_prec):
                 return fn(ctx, *args)
-            lib.ds2_set_precision(want)
-            try:
-                return fn(ctx, *args)
-            finally:
-                lib.ds2_set_precision(cur)
     return wrapped
 
 
@@ -135,7 +121,7 @@ def side_stream():
 def join_deferred():
     """order the current stream after every deferred weight-gradient GEMM queued so far"""
     if _side["stream"] is not None:
-        check(get_lib().ds2_join_side_stream(_stream()), "ds2_join_side_stream")
+        check(get_lib().ds2_join_side_stream(current_stream()), "ds2_join_side_stream")
 
 
 def _req(t, name):
@@ -167,7 +153,7 @@ class ConvFrontend(torch.autograd.Function):
         params = [_req(t, "conv param") for t in (w1, b1, g1, be1, rm1, rv1, w2, b2, g2, be2, rm2, rv2)]
         check(lib.ds2_conv_frontend_fwd(B, T, ptr(x), ptr(out_len), *[ptr(t) for t in params], int(training),
                                         float(momentum), float(eps), ptr(y), ptr(z1), ptr(a1), ptr(z2), ptr(stats),
-                                        ptr(ws), ws.numel(), _stream()), "ds2_conv_frontend_fwd")
+                                        ptr(ws), ws.numel(), current_stream()), "ds2_conv_frontend_fwd")
         ctx.save_for_backward(x, out_len, params[0], params[2], params[3], params[6], params[8], params[9],
                               z1, a1, z2, stats)
         ctx.dims = (B, T)
@@ -192,7 +178,7 @@ class ConvFrontend(torch.autograd.Function):
         check(lib.ds2_conv_frontend_bwd(B, T, ptr(x), ptr(out_len), ptr(w1), ptr(g1), ptr(be1), ptr(w2), ptr(g2),
                                         ptr(be2), ptr(z1), ptr(a1), ptr(z2), ptr(stats), ptr(dy), ptr(dw1), ptr(db1),
                                         ptr(dg1), ptr(dbe1), ptr(dw2), ptr(db2), ptr(dg2), ptr(dbe2), ptr(ws),
-                                        ws.numel(), _stream()), "ds2_conv_frontend_bwd")
+                                        ws.numel(), current_stream()), "ds2_conv_frontend_bwd")
         return (None, None, rets[0], rets[1], rets[2], rets[3], None, None, rets[4], rets[5], rets[6], rets[7], None,
                 None, None, None, None)
 
@@ -225,7 +211,7 @@ class RnnLayer(torch.autograd.Function):
         h0, c0 = _req(h0, "h0"), _req(c0, "c0")
         check(lib.ds2_rnn_layer_fwd(C.byref(desc), ptr(x), ptr(len_dev), ptr(bn_g), ptr(bn_b), ptr(bn_rm), ptr(bn_rv),
                                     w_ih, w_hh, b_ih, b_hh, ptr(h0), ptr(c0), ptr(y), ptr(hn), ptr(cn), ptr(reserve),
-                                    ptr(ws), ws.numel(), _stream()), "ds2_rnn_layer_fwd")
+                                    ptr(ws), ws.numel(), current_stream()), "ds2_rnn_layer_fwd")
         if training and _side["stream"] is not None:
             # a tensor-core-mode training forward writes the fp16 W_hh^T of the backward sweep into `reserve` on the
             # side stream: if the graph is dropped early, the block must not be handed out before that copy has run
@@ -278,7 +264,7 @@ class RnnLayer(torch.autograd.Function):
                                     ptr_array(weights[0::4]), ptr_array(weights[1::4]), ptr_array(weights[2::4]),
                                     ptr_array(weights[3::4]), ptr(dy), ptr(reserve), ptr(dx), ptr(dg), ptr(db),
                                     ptr_array(grads[0::4]), ptr_array(grads[1::4]), ptr_array(grads[2::4]),
-                                    ptr_array(grads[3::4]), ptr(ws), ws.numel(), _stream()), "ds2_rnn_layer_bwd")
+                                    ptr_array(grads[3::4]), ptr(ws), ws.numel(), current_stream()), "ds2_rnn_layer_bwd")
         assert len(grads) == 4 * D
         if desc.deferred_dw:
             # the side stream still reads the layer input and the saved sequences (operand copies of the deferred
@@ -297,7 +283,7 @@ class Lookahead(torch.autograd.Function):
         T, B, H = x.shape
         ctxlen = w.shape[-1]
         y = torch.empty_like(x)
-        check(lib.ds2_lookahead_fwd(T, B, H, ctxlen, ptr(x), ptr(w), ptr(y), _stream()), "ds2_lookahead_fwd")
+        check(lib.ds2_lookahead_fwd(T, B, H, ctxlen, ptr(x), ptr(w), ptr(y), current_stream()), "ds2_lookahead_fwd")
         ctx.save_for_backward(x, w)
         ctx.sink = _sink(w)
         return y
@@ -312,7 +298,7 @@ class Lookahead(torch.autograd.Function):
         dz, dx = torch.empty_like(x), torch.empty_like(x)
         dw, rdw = _out(ctx.sink, w)
         check(lib.ds2_lookahead_bwd(T, B, H, w.shape[-1], ptr(x), ptr(w), ptr(dy), ptr(dz), ptr(dx), ptr(dw),
-                                    _stream()), "ds2_lookahead_bwd")
+                                    current_stream()), "ds2_lookahead_bwd")
         return dx, rdw
 
 
@@ -332,7 +318,7 @@ class FcHead(torch.autograd.Function):
         ws = workspace(lib.ds2_fc_head_workspace_bytes(rows, H, Cn), dev)
         check(lib.ds2_fc_head_fwd(rows, H, Cn, ptr(x), ptr(g), ptr(b), ptr(rm), ptr(rv), ptr(w), int(training),
                                   float(momentum), float(eps), int(softmax), ptr(logits), ptr(xhat), ptr(stats),
-                                  ptr(ws), ws.numel(), _stream()), "ds2_fc_head_fwd")
+                                  ptr(ws), ws.numel(), current_stream()), "ds2_fc_head_fwd")
         ctx.save_for_backward(g, b, w, xhat, stats)
         ctx.dims = (rows, H, Cn, T, B)
         ctx.eval_mode = not training
@@ -354,7 +340,7 @@ class FcHead(torch.autograd.Function):
         (dg, rdg), (db, rdb), (dw, rdw) = (_out(sk, like) for sk, like in zip(ctx.sinks, (g, b, w)))
         ws = workspace(lib.ds2_fc_head_workspace_bytes(rows, H, Cn), dev)
         check(lib.ds2_fc_head_bwd(rows, H, Cn, ptr(g), ptr(b), ptr(w), ptr(xhat), ptr(stats), ptr(dlogits), ptr(dx),
-                                  ptr(dg), ptr(db), ptr(dw), ptr(ws), ws.numel(), _stream()), "ds2_fc_head_bwd")
+                                  ptr(dg), ptr(db), ptr(dw), ptr(ws), ws.numel(), current_stream()), "ds2_fc_head_bwd")
         return dx, rdg, rdb, None, None, rdw, None, None, None, None
 
 
@@ -373,7 +359,7 @@ class CtcLoss(torch.autograd.Function):
         ws = workspace(lib.ds2_ctc_workspace_bytes(T, B, Cn, int(max_tgt_len)), dev)
         check(lib.ds2_ctc_loss_fwd_bwd(T, B, Cn, ptr(logits), ptr(targets), ptr(in_len), ptr(tgt_len),
                                        int(max_tgt_len), int(blank), ptr(nll), ptr(grad), ptr(ws), ws.numel(),
-                                       _stream()), "ds2_ctc_loss_fwd_bwd")
+                                       current_stream()), "ds2_ctc_loss_fwd_bwd")
         ctx.save_for_backward(grad)
         ctx.nll = nll
         return nll.sum()
@@ -400,5 +386,5 @@ def _gemm(lib, a, b, trans_a, trans_b, out, alpha, beta):
         out = torch.empty(M, N, device=a.device)
     ws = workspace(max(256, lib.ds2_gemm_workspace_bytes(int(trans_a), int(trans_b), M, N, K)), a.device)
     check(lib.ds2_gemm(int(trans_a), int(trans_b), M, N, K, float(alpha), ptr(a), a.shape[1], ptr(b), b.shape[1],
-                       float(beta), ptr(out), N, ptr(ws), ws.numel(), _stream()), "ds2_gemm")
+                       float(beta), ptr(out), N, ptr(ws), ws.numel(), current_stream()), "ds2_gemm")
     return out

@@ -5,11 +5,9 @@ The reference steps `torch.optim.AdamW` / SGD-Nesterov (model.py:273-297) after 
 contiguous buffer (so the data-parallel exchange is a single all-reduce, dist.py) and the update is
 two kernels over that buffer: a sum-of-squares reduction, then clip-scale + AdamW/SGD fused.
 """
-import ctypes as C
-
 import torch
 
-from ._lib import check, get_lib
+from ._lib import check, current_stream, get_lib
 
 _ALIGN = 64  # floats: 256-byte aligned views (TMA / float4 friendly)
 
@@ -70,7 +68,7 @@ class FusedOptimizer:
     def _step(self, grad_scale):
         lib = get_lib()
         f = self.flat
-        st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        st = current_stream()
         self.step_count += 1
         if self.adam:
             b1, b2 = self.cfg.betas

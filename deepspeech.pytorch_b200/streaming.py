@@ -25,18 +25,18 @@ Normalisation is causal: either fixed (mean, std given at `open`) or running (fr
 `StreamCore` is the bookkeeping: it takes the four model blocks as callables, so it runs on the GPU with the library's
 ops and on the CPU with the oracle blocks of `oracle/ds2_oracle.py` (tests/test_streaming_host.py).
 """
-import ctypes as C
+import functools
 from dataclasses import dataclass, field
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
-from . import _lib, ops
-from ._lib import Ds2Error, check, get_lib, ptr
+from . import _lib
+from ._lib import Ds2Error, check, current_stream, get_lib, ptr
 from .configs import is_kind
 from .decoder import BeamCTCDecoder, GreedyDecoder
-from .input_pipeline import analysis_window
+from .input_pipeline import analysis_window, spect_geometry
 
 __all__ = ["StreamingTranscriber", "StreamResult", "StreamCore", "StreamSpectrogram", "StreamBeamSearch",
            "spect_frames_ready",
@@ -221,12 +221,9 @@ class StreamSpectrogram:
 
     def __init__(self, spect_cfg, max_sessions: int, device="cuda"):
         self.device = torch.device(device)
-        self.sample_rate = int(spect_cfg.sample_rate)
-        self.n_fft = int(spect_cfg.sample_rate * spect_cfg.window_size)
-        self.hop = int(spect_cfg.sample_rate * spect_cfg.window_stride)
+        self.sample_rate, self.n_fft, self.hop, wname = spect_geometry(spect_cfg)
         if self.n_fft // 2 + 1 != N_FREQ:
             raise Ds2Error(f"streaming: the front-end needs {N_FREQ} frequency bins, got {self.n_fft // 2 + 1}")
-        wname = spect_cfg.window.value if hasattr(spect_cfg.window, "value") else str(spect_cfg.window)
         lib = get_lib()
         with torch.cuda.device(self.device):
             self.window = torch.from_numpy(analysis_window(wname, self.n_fft)).to(self.device)
@@ -289,8 +286,7 @@ class StreamSpectrogram:
                 self._ws = torch.empty(int(nws * 1.25) + 256, dtype=torch.uint8, device=self.device)
             check(lib.ds2_spectrogram_stream(B, ptr(dev[mb:]), ptr(dev), Tcap, self.n_fft, self.hop, ptr(self.window),
                                              ptr(out), Tcap, ptr(self.state), ptr(self._ws), self._ws.numel(),
-                                             C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                  "ds2_spectrogram_stream")
+                                             current_stream()), "ds2_spectrogram_stream")
         return out, counts
 
 
@@ -343,9 +339,8 @@ class StreamBeamSearch:
             lengths = torch.empty(out_row, dtype=torch.int32, device=self.device)
             scores = torch.empty(out_row, dtype=torch.float64, device=self.device)
             n_beams = torch.empty(n, dtype=torch.int32, device=self.device)
-            stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
             common = (ptr(labels), ptr(timesteps), ptr(lengths), ptr(scores), ptr(n_beams), ptr(self.state),
-                      self.state.numel(), stream)
+                      self.state.numel(), current_stream())
             if self.lm is None:
                 check(lib.ds2_beam_decode_stream(n, p.shape[1], ptr(p), ptr(it), d.blank_index, W, d.cutoff_top_n,
                                                  d.cutoff_prob, self.S, self.max_frames, Tout, *common),
@@ -374,38 +369,6 @@ class StreamResult:
     final: bool
     beams: Optional[list] = None     # beam decoder, on finish: (text, offsets, score) of each of the n_beams beams
     outputs: Optional[torch.Tensor] = field(default=None, repr=False)   # this step's decided head outputs
-
-
-def _model_blocks(model, logits: bool):
-    """the four blocks of StreamCore on the library's ops, eval mode"""
-    from .model import BN_EPS, BN_MOMENTUM
-    sm = model.conv.seq_module
-    conv_params = (sm[0].weight, sm[0].bias, sm[1].weight, sm[1].bias, sm[1].running_mean, sm[1].running_var,
-                   sm[3].weight, sm[3].bias, sm[4].weight, sm[4].bias, sm[4].running_mean, sm[4].running_var)
-
-    def conv(x, out_len):
-        return ops.ConvFrontend.apply(x, out_len, *conv_params, False, BN_MOMENTUM, BN_EPS)
-
-    def rnn(l, x, lens, h0, c0):
-        layer = model.rnns[l]
-        bn = layer.batch_norm.module if layer.batch_norm is not None else None
-        return ops.RnnLayer.apply(x, lens, layer.rnn_code, False, False, BN_MOMENTUM, BN_EPS,
-                                  bn.weight if bn else None, bn.bias if bn else None,
-                                  bn.running_mean if bn else None, bn.running_var if bn else None, h0, c0,
-                                  *layer.weights())
-
-    w_la = model.lookahead[0].conv.weight
-
-    def lookahead(x):
-        return ops.Lookahead.apply(x, w_la)
-
-    fbn, flin = model.fc[0].module[0], model.fc[0].module[1]
-
-    def head(x):
-        return ops.FcHead.apply(x, fbn.weight, fbn.bias, fbn.running_mean, fbn.running_var, flin.weight, False,
-                                BN_MOMENTUM, BN_EPS, not logits)
-
-    return conv, rnn, lookahead, head
 
 
 class StreamingTranscriber:
@@ -439,7 +402,11 @@ class StreamingTranscriber:
         self.spect = StreamSpectrogram(model.spect_cfg, self.max_sessions, self.device)
         self.max_samples = int(max_seconds * self.spect.sample_rate)
         cfg = model.model_cfg
-        self.core = StreamCore(*_model_blocks(model, logits), n_layers=len(model.rnns), hidden=cfg.hidden_size,
+        # the model's blocks in eval mode, whatever model.train() may later set
+        blocks = (functools.partial(model.conv_block, training=False),
+                  lambda l, x, lens, h0, c0: model.rnn_block(l, x, lens, False, h0, c0), model.lookahead_block,
+                  functools.partial(model.head_block, training=False, softmax=not logits))
+        self.core = StreamCore(*blocks, n_layers=len(model.rnns), hidden=cfg.hidden_size,
                                lstm=model.rnns[0].rnn_code == _lib.RNN_LSTM, context=cfg.lookahead_context,
                                max_sessions=self.max_sessions, device=self.device)
         self.carry = torch.full((self.max_sessions,), -1, dtype=torch.int32, device=self.device)
@@ -501,34 +468,26 @@ class StreamingTranscriber:
             return {}
         slots = [self._slot[s] for s in sids]
         fin = [s in finish for s in sids]
-        lib = get_lib()
-        saved = lib.ds2_get_precision()
-        if self.model.precision == 16:
-            lib.ds2_set_precision(_lib.PREC_F16)
-        try:
-            with torch.no_grad(), torch.cuda.device(self.device):
-                fresh = [s for s in slots if s in self._fresh]
-                if fresh:
-                    self.carry.index_fill_(0, torch.tensor(fresh, device=self.device), -1)
-                    self._fresh.difference_update(fresh)
-                frames, counts = self.spect.step([(s, pcm[sid], f) for s, sid, f in zip(slots, sids, fin)])
-                out, spans = self.core.step([(s, n, f) for s, n, f in zip(slots, counts, fin)], frames)
-                labels = beams = None
-                if self.beam is not None:
-                    beams = self.beam.step(out, [(s, n, f) for s, (_, n), f in zip(slots, spans, fin)])
-                elif out is not None:
-                    rows = np.zeros(len(sids) + 1, np.int32)
-                    rows[1:] = np.cumsum([n for _, n in spans])
-                    meta = torch.from_numpy(np.concatenate([rows, np.asarray(slots, np.int32)])).to(self.device)
-                    lab = torch.empty(out.shape[0], dtype=torch.int32, device=self.device)
-                    check(lib.ds2_greedy_decode_stream(len(sids), out.shape[1], ptr(out), ptr(meta),
-                                                       ptr(meta[len(sids) + 1:]), self.decoder.blank_index,
-                                                       ptr(self.carry), ptr(lab),
-                                                       C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                          "ds2_greedy_decode_stream")
-                    labels = lab.cpu().numpy()
-        finally:
-            lib.ds2_set_precision(saved)
+        with _lib.autocast(self.model.precision), torch.no_grad(), torch.cuda.device(self.device):
+            fresh = [s for s in slots if s in self._fresh]
+            if fresh:
+                self.carry.index_fill_(0, torch.tensor(fresh, device=self.device), -1)
+                self._fresh.difference_update(fresh)
+            frames, counts = self.spect.step([(s, pcm[sid], f) for s, sid, f in zip(slots, sids, fin)])
+            out, spans = self.core.step([(s, n, f) for s, n, f in zip(slots, counts, fin)], frames)
+            labels = beams = None
+            if self.beam is not None:
+                beams = self.beam.step(out, [(s, n, f) for s, (_, n), f in zip(slots, spans, fin)])
+            elif out is not None:
+                rows = np.zeros(len(sids) + 1, np.int32)
+                rows[1:] = np.cumsum([n for _, n in spans])
+                meta = torch.from_numpy(np.concatenate([rows, np.asarray(slots, np.int32)])).to(self.device)
+                lab = torch.empty(out.shape[0], dtype=torch.int32, device=self.device)
+                check(get_lib().ds2_greedy_decode_stream(len(sids), out.shape[1], ptr(out), ptr(meta),
+                                                         ptr(meta[len(sids) + 1:]), self.decoder.blank_index,
+                                                         ptr(self.carry), ptr(lab), current_stream()),
+                      "ds2_greedy_decode_stream")
+                labels = lab.cpu().numpy()
         res, r0 = {}, 0
         i2c = self.decoder.int_to_char
         for i, sid in enumerate(sids):
