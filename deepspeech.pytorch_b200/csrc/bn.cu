@@ -1,21 +1,24 @@
 // BatchNorm over the rows of a (rows, F) matrix: the SequenceWise(BatchNorm1d) of the reference
 // (model.py:18-33, :86 per RNN layer, :196 in the fc head).  Statistics are over ALL T*B rows,
-// padded rows included (SURVEY.md §8c quirks).
+// padded rows included (SURVEY.md §8c quirks).  bn_finalize also finalizes the conv front-end's BatchNorm2d, whose
+// sums the conv epilogues accumulate (conv_frontend.cu).
 //
-// Forward statistics: E[x^2] - E[x]^2 from raw sums (fp32 partials of 64 rows, flushed into double) cancels on
-// near-constant features, which is what saturated LSTM units feed the next layer (the sum of the two directions of h
-// sits near +-2 with a tiny spread): for mean 10 and std 0.001 the variance is 1e-8 of E[x^2], below fp32 rounding.
-// So the forward pass also sums (x - K) and (x - K)^2 in double per element, with K = the feature's first row:
-// mean = K + S1/n, var = S2/n - (S1/n)^2, where S2/n stays within a small factor of (S1/n)^2.  The raw result is kept
-// wherever it is accurate, E[x^2] <= RAW_MAX_CANCEL * var (raw variance error there: about 1e-6 relative, typical),
-// so a well-conditioned feature gets exactly the bits it always had: a last-bit change in the statistics, carried
-// through fp16 operand copies and AdamW, moves the loss of the benchmark step by 0.1 % after 11 steps.  Every feature
-// of the benchmark's model is well-conditioned (E[x^2] / var <= 18).  The FP64 adds are hidden under the loads.
+// Forward statistics: E[x^2] - E[x]^2 from raw sums (fp32 partials, flushed into double) cancels when a feature's mean
+// is large against its spread.  Saturated LSTM units feed the next layer such features (the sum of the two directions
+// of h sits near +-2 with a tiny spread: for mean 10 and std 0.001 the variance is 1e-8 of E[x^2], below fp32
+// rounding); in the front-end the conv bias moves a channel's mean.  So the statistics pass also sums (x - K) and
+// (x - K)^2 with a pivot K per feature: here the feature's first row (summed in double per element, the FP64 adds
+// hidden under the loads), in the front-end the channel's conv bias (known before the convolution runs).  From those,
+// mean = K + S1/n and var = S2/n - (S1/n)^2, where S2/n stays within a small factor of (S1/n)^2.  bn_finalize_kernel
+// takes them for a feature whose E[x^2] exceeds max_cancel * var and keeps the raw result everywhere else, so a
+// well-conditioned feature gets exactly the bits it always had: a last-bit change in the statistics, carried through
+// fp16 operand copies and AdamW, moves the loss of the benchmark step by 0.1 % after 11 steps.  The thresholds
+// (common.cuh): RAW_MAX_CANCEL = 256 for the rows, where the raw variance error below it is about 1e-6 relative,
+// typical, and every feature of the benchmark's model is below it (E[x^2] / var <= 18); BN2D_RAW_MAX_CANCEL = 16 for
+// the front-end, where the raw variance below it is within a few 1e-7 of float64.
 #include "common.cuh"
 
 namespace ds2 {
-
-constexpr double RAW_MAX_CANCEL = 256.0;
 
 // blockDim = (32, 8): 32 consecutive features x 8 row lanes; grid = (ceil(F/32), row_chunks)
 __global__ void bn_colsum_kernel(int rows, int F, const float* __restrict__ a, const float* __restrict__ b,
@@ -63,10 +66,11 @@ __global__ void bn_colsum_kernel(int rows, int F, const float* __restrict__ a, c
   }
 }
 
+// sums: sum x [F], sum x^2 [F]; piv_sums: sum (x - K) [F], sum (x - K)^2 [F], K = pivot[f]
 __global__ void bn_finalize_kernel(int F, double count, const double* __restrict__ sums,
-                                   const float* __restrict__ pivot, float* __restrict__ rmean,
-                                   float* __restrict__ rvar, int training, float momentum, float eps,
-                                   float* __restrict__ mean_invstd) {
+                                   const double* __restrict__ piv_sums, const float* __restrict__ pivot,
+                                   double max_cancel, float* __restrict__ rmean, float* __restrict__ rvar,
+                                   int training, float momentum, float eps, float* __restrict__ mean_invstd) {
   int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
   float mean, var;
@@ -74,10 +78,10 @@ __global__ void bn_finalize_kernel(int F, double count, const double* __restrict
     double m = sums[f] / count;
     double v = sums[F + f] / count - m * m;
     if (v < 0.0) v = 0.0;
-    const double ms = sums[2 * F + f] / count;  // mean - K
-    double vs = sums[3 * F + f] / count - ms * ms;
+    const double ms = piv_sums[f] / count;  // mean - K
+    double vs = piv_sums[F + f] / count - ms * ms;
     if (vs < 0.0) vs = 0.0;
-    if (!(sums[F + f] / count <= RAW_MAX_CANCEL * vs)) {  // the raw sums cancel: take the pivoted ones
+    if (!(sums[F + f] / count <= max_cancel * vs)) {  // the raw sums cancel: take the pivoted ones
       m = (double)pivot[f] + ms;
       v = vs;
     }
@@ -133,6 +137,25 @@ static int colsum_grid_y(int rows) {
   return g < 1 ? 1 : (g > 64 ? 64 : g);
 }
 
+// blocks of 256 threads for the grid-stride elementwise kernels: about 4 entries per thread, at most 16 blocks per SM
+static int elementwise_blocks(size_t total) {
+  const size_t blocks = (total + 1023) / 1024;
+  return blocks < 1 ? 1 : (blocks > 132 * 16 ? 132 * 16 : (int)blocks);
+}
+
+int bn_finalize(int F, double count, const double* sums, const double* piv_sums, const float* pivot,
+                double max_cancel, float* rmean, float* rvar, int training, float momentum, float eps,
+                float* mean_invstd, cudaStream_t st) {
+  DS2_LAUNCH(bn_finalize_kernel, cdiv(F, 128), 128, 0, st, F, count, sums, piv_sums, pivot, max_cancel, rmean, rvar,
+             training, momentum, eps, mean_invstd);
+  return DS2_OK;
+}
+
+int bn_bwd_params(int F, const double* sums, float* dgamma, float* dbeta, cudaStream_t st) {
+  DS2_LAUNCH(bn_bwd_params_kernel, cdiv(F, 128), 128, 0, st, F, sums, dgamma, dbeta);
+  return DS2_OK;
+}
+
 int bn_rows_fwd(int rows, int F, const float* x, const float* gamma, const float* beta, float* rmean, float* rvar,
                 int training, float momentum, float eps, float* y, float* xhat, float* mean_invstd,
                 double* ws_sums, cudaStream_t st) {
@@ -141,23 +164,16 @@ int bn_rows_fwd(int rows, int F, const float* x, const float* gamma, const float
     dim3 grid(cdiv(F, 32), colsum_grid_y(rows)), block(32, 8);
     DS2_LAUNCH(bn_colsum_kernel, grid, block, 0, st, rows, F, x, x, x /* pivot: row 0 */, ws_sums);
   }
-  DS2_LAUNCH(bn_finalize_kernel, cdiv(F, 128), 128, 0, st, F, (double)rows, ws_sums, x, rmean, rvar, training, momentum,
-             eps, mean_invstd);
-  size_t total = (size_t)rows * F;
-  int blocks = (int)((total + 1023) / 1024);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  if (blocks < 1) blocks = 1;
-  DS2_LAUNCH(bn_apply_kernel, blocks, 256, 0, st, total, F, x, gamma, beta, mean_invstd, y, xhat);
-  return DS2_OK;
+  int rc = bn_finalize(F, (double)rows, ws_sums, ws_sums + 2 * F, x, RAW_MAX_CANCEL, rmean, rvar, training, momentum,
+                       eps, mean_invstd, st);
+  if (rc) return rc;
+  return bn_rows_reapply(rows, F, x, gamma, beta, mean_invstd, y, xhat, st);
 }
 
 int bn_rows_reapply(int rows, int F, const float* x, const float* gamma, const float* beta,
                     const float* mean_invstd, float* y, float* xhat, cudaStream_t st) {
-  size_t total = (size_t)rows * F;
-  int blocks = (int)((total + 1023) / 1024);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  if (blocks < 1) blocks = 1;
-  DS2_LAUNCH(bn_apply_kernel, blocks, 256, 0, st, total, F, x, gamma, beta, mean_invstd, y, xhat);
+  const size_t total = (size_t)rows * F;
+  DS2_LAUNCH(bn_apply_kernel, elementwise_blocks(total), 256, 0, st, total, F, x, gamma, beta, mean_invstd, y, xhat);
   return DS2_OK;
 }
 
@@ -166,13 +182,11 @@ int bn_rows_bwd(int rows, int F, const float* xhat, const float* gamma, const fl
   DS2_CHECK_CUDA(cudaMemsetAsync(ws_sums, 0, sizeof(double) * 2 * F, st));
   dim3 grid(cdiv(F, 32), colsum_grid_y(rows)), block(32, 8);
   DS2_LAUNCH(bn_colsum_kernel, grid, block, 0, st, rows, F, dy, xhat, nullptr, ws_sums);
-  DS2_LAUNCH(bn_bwd_params_kernel, cdiv(F, 128), 128, 0, st, F, ws_sums, dgamma, dbeta);
-  size_t total = (size_t)rows * F;
-  int blocks = (int)((total + 1023) / 1024);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  if (blocks < 1) blocks = 1;
-  DS2_LAUNCH(bn_bwd_apply_kernel, blocks, 256, 0, st, total, F, 1.0 / (double)rows, xhat, gamma, mean_invstd, dy,
-             ws_sums, dx);
+  int rc = bn_bwd_params(F, ws_sums, dgamma, dbeta, st);
+  if (rc) return rc;
+  const size_t total = (size_t)rows * F;
+  DS2_LAUNCH(bn_bwd_apply_kernel, elementwise_blocks(total), 256, 0, st, total, F, 1.0 / (double)rows, xhat, gamma,
+             mean_invstd, dy, ws_sums, dx);
   return DS2_OK;
 }
 

@@ -149,6 +149,16 @@ int transpose_strided(int R, int C, const float* in, size_t ldi, float* out, siz
 // dx = gamma*invstd*(dy - mean(dy) - xhat*mean(dy*xhat)); dgamma, dbeta written.
 int bn_rows_bwd(int rows, int F, const float* xhat, const float* gamma, const float* mean_invstd, const float* dy,
                 float* dx, float* dgamma, float* dbeta, double* ws_sums /*2F doubles*/, cudaStream_t st);
+// The BatchNorm steps the conv front-end's BatchNorm2d shares with bn_rows_fwd / bn_rows_bwd.
+// mean_invstd (2F) of F features over `count` values each; training: from the raw sums (sum x, sum x^2) or, where
+// E[x^2] > max_cancel * var, from the pivoted ones (sum (x - K), sum (x - K)^2, K = pivot[f]), running stats updated;
+// else from the running stats.  The cancellation thresholds of the two BatchNorms: bn.cu's header says why each.
+constexpr double RAW_MAX_CANCEL = 256.0, BN2D_RAW_MAX_CANCEL = 16.0;
+int bn_finalize(int F, double count, const double* sums, const double* piv_sums, const float* pivot,
+                double max_cancel, float* rmean, float* rvar, int training, float momentum, float eps,
+                float* mean_invstd, cudaStream_t st);
+// dbeta = sums[0..F), dgamma = sums[F..2F) (the backward's sum dy, sum dy*xhat)
+int bn_bwd_params(int F, const double* sums, float* dgamma, float* dbeta, cudaStream_t st);
 // CTC helpers (ctc.cu), shared by the loss and the forced alignment (ctc_align.cu):
 // fp32 log-softmax of `rows` rows of C values; the exclusive prefix sum of the target lengths (offsets into the flat
 // targets)

@@ -39,7 +39,7 @@ struct ConvGeom {
 // out[b,co,d,t] = bias[co] + sum_{ci,kh,kw} wpk[ci][kh][kw][co] * in[b,ci,d*SH+kh-PH,t*SW+kw-PW]
 // out address = b*ob + co*oc + d*orow + t ; positions t >= out_len[b] are written as 0 (if out_len)
 // stat_sums (double[64]) += per-channel sum / sum of squares of what was written (if non-null), and with it
-// piv_sums (double[64]) += the same of what was written minus the channel's bias (the BatchNorm pivot, see bn2d_finalize)
+// piv_sums (double[64]) += the same of what was written minus the channel's bias (the BatchNorm pivot, see bn.cu)
 template <int KH, int KW, int SH, int SW>
 __global__ void __launch_bounds__(256) conv_fwd_kernel(const float* __restrict__ in, int Cin, int Hin, int Win,
                                                        const float* __restrict__ wpk, const float* __restrict__ bias,
@@ -162,44 +162,7 @@ __global__ void pack_bwd_data_kernel(int parity, const float* __restrict__ w2, f
   wT[i] = w2[(((size_t)co * CO + ci) * 21 + kh) * 11 + kw];
 }
 
-// ---- BatchNorm2d pieces -----------------------------------------------------------------------
-// The statistics come from raw sums, E[z^2] - E[z]^2, which cancel when a channel's mean is large against its spread;
-// the conv bias is what usually puts it there, so the conv epilogues also sum z - K and (z - K)^2 with the pivot
-// K = the channel's bias (piv, known before the conv runs), and a channel whose E[z^2] exceeds BN2D_RAW_MAX_CANCEL var
-// takes mean = K + S1/n, var = S2/n - (S1/n)^2 from those.  Channels below the threshold keep the raw result bit for
-// bit (as the sequence-wise BatchNorm of bn.cu does); there the raw variance is within a few 1e-7 of float64.
-constexpr double BN2D_RAW_MAX_CANCEL = 16.0;
-__global__ void bn2d_finalize_kernel(double count, const double* __restrict__ sums, const double* __restrict__ piv_sums,
-                                     const float* __restrict__ piv, const float* __restrict__ gamma,
-                                     const float* __restrict__ beta, float* __restrict__ rmean,
-                                     float* __restrict__ rvar, int training, float momentum, float eps,
-                                     float* __restrict__ mean_invstd /*[2][32]*/) {
-  int c = threadIdx.x;
-  if (c >= CO) return;
-  float mean, var;
-  if (training) {
-    double m = sums[c] / count, v = sums[CO + c] / count - m * m;
-    if (v < 0.0) v = 0.0;
-    const double ms = piv_sums[c] / count;      // mean - K
-    double vs = piv_sums[CO + c] / count - ms * ms;
-    if (vs < 0.0) vs = 0.0;
-    if (!(sums[CO + c] / count <= BN2D_RAW_MAX_CANCEL * vs)) {   // the raw sums cancel: take the pivoted ones
-      m = (double)piv[c] + ms;
-      v = vs;
-    }
-    mean = (float)m;
-    var = (float)v;
-    double unb = count > 1.0 ? v * count / (count - 1.0) : v;
-    rmean[c] = (1.f - momentum) * rmean[c] + momentum * mean;
-    rvar[c] = (1.f - momentum) * rvar[c] + momentum * (float)unb;
-  } else {
-    mean = rmean[c];
-    var = rvar[c];
-  }
-  mean_invstd[c] = mean;
-  mean_invstd[CO + c] = rsqrtf(var + eps);
-}
-
+// ---- BatchNorm2d pieces (the statistics are finalized by bn.cu's bn_finalize) ---------------------
 // a = mask(clamp(gamma*(z-mean)*invstd+beta, 0, 20)) over (B,32,D,T)
 __global__ void bn_act_kernel(int B, int D, int T, const float* __restrict__ z, const float* __restrict__ mi,
                               const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -344,12 +307,6 @@ __global__ void ordered_sum_kernel(int n, const float* __restrict__ part, float*
     __syncthreads();
   }
   if (threadIdx.x == 0) out[blockIdx.x] = red[0];
-}
-
-__global__ void bn_bwd_params2d_kernel(const double* __restrict__ sums, float* __restrict__ dgamma,
-                                       float* __restrict__ dbeta) {
-  int c = threadIdx.x;
-  if (c < CO) { dbeta[c] = (float)sums[c]; dgamma[c] = (float)sums[CO + c]; }
 }
 
 // ---- weight gradients -------------------------------------------------------------------------
@@ -552,8 +509,9 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
   int rc = launch_conv<41, 11, 2, 2>(x, B, 1, F, T, W.wpk1, b1, z1, D1, Tp, (size_t)CO * D1 * Tp, (size_t)D1 * Tp,
                                      (size_t)Tp, 20, 5, out_len, training ? W.sums : nullptr, piv1, st);
   if (rc) return rc;
-  DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D1 * Tp, W.sums, W.sums + 128, b1, g1, be1, rm1, rv1,
-             training, momentum, eps, stats);
+  rc = bn_finalize(CO, (double)B * D1 * Tp, W.sums, W.sums + 128, b1, BN2D_RAW_MAX_CANCEL, rm1, rv1, training,
+                   momentum, eps, stats, st);
+  if (rc) return rc;
   DS2_LAUNCH(bn_act_kernel, 132 * 8, 256, 0, st, B, D1, Tp, z1, stats, g1, be1, out_len, a1);
   if (tensor_core_mode()) {
     // conv2 on wgmma: channels-last copy of a1, packed taps, implicit GEMM with the kw taps folded into N
@@ -569,8 +527,9 @@ int ds2_conv_frontend_fwd(int B, int T, const float* x, const int32_t* out_len, 
                                    (size_t)Tp, 10, 5, out_len, training ? W.sums + 64 : nullptr, piv2, st);
   }
   if (rc) return rc;
-  DS2_LAUNCH(bn2d_finalize_kernel, 1, 32, 0, st, (double)B * D2 * Tp, W.sums + 64, W.sums + 192, b2, g2, be2, rm2,
-             rv2, training, momentum, eps, stats + 64);
+  rc = bn_finalize(CO, (double)B * D2 * Tp, W.sums + 64, W.sums + 192, b2, BN2D_RAW_MAX_CANCEL, rm2, rv2, training,
+                   momentum, eps, stats + 64, st);
+  if (rc) return rc;
   DS2_LAUNCH(bn_act_transpose_kernel, dim3(cdiv(Tp, 32), cdiv(CO * D2, 32), B), dim3(32, 8), 0, st, B, D2, Tp, z2,
              stats + 64, g2, be2, out_len, y);
   return DS2_OK;
@@ -600,7 +559,7 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
   // ---- stage 2: BN2 + Hardtanh + mask backward (dy arrives time-major)
   DS2_LAUNCH(bn_bwd_reduce_kernel<true>, dim3(cdiv(Tp, 32), cdiv(CO * D2, 32), B), dim3(32, 8), 0, st, B, D2, Tp, z2,
              stats + 64, g2, be2, out_len, dy, W.du2, s2);
-  DS2_LAUNCH(bn_bwd_params2d_kernel, 1, 32, 0, st, s2, dg2, dbe2);
+  if (int rc = bn_bwd_params(CO, s2, dg2, dbe2, st)) return rc;
   DS2_LAUNCH(bn_bwd_apply_kernel, dim3(cdiv(D2 * Tp, 256), CO, B), 256, 0, st, B, D2, Tp, 1.0 / ((double)B * D2 * Tp),
              z2, stats + 64, g2, out_len, s2, W.du2, W.db_part);
   DS2_LAUNCH(ordered_sum_kernel, CO, 256, 0, st, B * cdiv(D2 * Tp, 256), W.db_part, db2);
@@ -654,7 +613,8 @@ int ds2_conv_frontend_bwd(int B, int T, const float* x, const int32_t* out_len, 
   // ---- stage 1: BN1 + Hardtanh + mask backward (natural layout, in place over da1)
   DS2_LAUNCH(bn_bwd_reduce_kernel<false>, dim3(cdiv(Tp, 32), cdiv(CO * D1, 32), B), dim3(32, 8), 0, st, B, D1, Tp,
              z1, stats, g1, be1, out_len, W.da1, W.da1, s1);
-  DS2_LAUNCH(bn_bwd_params2d_kernel, 1, 32, 0, st, s1, dg1, dbe1);
+  rc = bn_bwd_params(CO, s1, dg1, dbe1, st);
+  if (rc) return rc;
   DS2_LAUNCH(bn_bwd_apply_kernel, dim3(cdiv(D1 * Tp, 256), CO, B), 256, 0, st, B, D1, Tp, 1.0 / ((double)B * D1 * Tp),
              z1, stats, g1, out_len, s1, W.da1, W.db_part);
   DS2_LAUNCH(ordered_sum_kernel, CO, 256, 0, st, B * cdiv(D1 * Tp, 256), W.db_part, db1);

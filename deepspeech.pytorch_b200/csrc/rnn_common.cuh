@@ -16,7 +16,8 @@ struct SeqArgs {
   float* hseq;   // (D,T,B,H) per-direction outputs, zero at masked steps
   float* aux;    // (D,T,B,H) LSTM cell states / GRU W_hn h + b_hn (-> dGh_n after bwd); null for tanh
   const float* w_hh[2];   // the layer's (G*H,H) recurrent weights
-  float* w_hhT[2];        // bwd: (H,G*H) workspace for the fp32 W_hh^T, filled by the sweep that reads it
+  float* w_hhT[2];        // bwd: (H,G*H) workspace for the fp32 W_hh^T of the streaming and FFMA backward sweeps,
+                          // each of which transposes w_hh into it itself (the resident ones read fp16 only)
   const float* b_ih[2];
   const float* b_hh[2];
   const float* h0;        // (D,B,H) or null

@@ -589,11 +589,6 @@ static size_t fwd_smem_bytes(int NB) {
          (2 * STAGES + 2) * sizeof(uint64_t) + 64 + tc::acc_image_bytes(NB);
 }
 
-__global__ void f32_to_f16_kernel(size_t n, const float* __restrict__ in, __half* __restrict__ out) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (size_t)gridDim.x * blockDim.x;
-  for (; i < n; i += stride) out[i] = __float2half_rn(in[i]);
-}
-
 static size_t res_smem_bytes(int NB, int H) {
   using namespace rp;
   size_t NBp = NB + 1;
@@ -632,10 +627,11 @@ static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chu
   p.box3 = chunks % 4 == 0;
   const int rows = (a.T + (state ? 2 : 0)) * a.B;
   for (int d = 0; d < a.D; ++d) {
-    DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hh[d], w.w16 + (size_t)d * wn);
-    int rc = unit_major
-                 ? make_tmap_f16(&p.tmW[d], w.w16 + (size_t)d * wn, 3, a.H, G, a.H, (size_t)a.H * a.H, (size_t)a.H, 64, 4, UT)
-                 : make_tmap_f16(&p.tmW[d], w.w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
+    int rc = f32_to_f16_rows(G * a.H, a.H, a.w_hh[d], a.H, w.w16 + (size_t)d * wn, a.H, nullptr, st);
+    if (rc) return rc;
+    rc = unit_major
+             ? make_tmap_f16(&p.tmW[d], w.w16 + (size_t)d * wn, 3, a.H, G, a.H, (size_t)a.H * a.H, (size_t)a.H, 64, 4, UT)
+             : make_tmap_f16(&p.tmW[d], w.w16 + (size_t)d * wn, 3, a.H, a.H, G, (size_t)a.H, (size_t)a.H * a.H, 64, UT, G);
     if (rc) return rc;
     __half* hbase = p.h16 + (size_t)d * a.T * BH - (state ? BH : 0);
     rc = make_tmap_f16(&p.tmV[d], hbase, 2, a.H, rows, 1, (size_t)a.H, 0, 64, a.B, 1);
@@ -646,8 +642,9 @@ static int f16_weight_maps(const SeqArgs& a, PersistParams& p, void* ws, int chu
     }
     if (state) {   // forward: the step before t = 0; reverse: the step after t = T - 1
       __half* slot = d == 0 ? p.h16 - BH : p.h16 + (size_t)a.D * a.T * BH;
-      if (a.h0) DS2_LAUNCH(f32_to_f16_kernel, 132, 256, 0, st, BH, a.h0 + (size_t)d * BH, slot);
+      if (a.h0) rc = f32_to_f16_rows(a.B, a.H, a.h0 + (size_t)d * BH, a.H, slot, a.H, nullptr, st);
       else DS2_CHECK_CUDA(cudaMemsetAsync(slot, 0, BH * sizeof(__half), st));
+      if (rc) return rc;
     }
   }
   return DS2_OK;
@@ -1941,7 +1938,7 @@ enum class Prep {
   FWD_F32,   // maps over the fp32 W_hh and hseq: the 16-unit streaming forward
   FWD_F16,   // fp16 W_hh in the workspace (f16_weight_maps): the resident and the split-K forward
   BWD_F32,   // the fp32 W_hh^T and its maps (bwd_f32_maps): the 16-unit and the split-K streaming backward
-  BWD_F16,   // fp16 W_hh^T, max |dY[t]| and the resident backward's workspace: the resident split-K backward
+  BWD_F16,   // the fp16 W_hh^T only, max |dY[t]| and the resident backward's workspace: the resident split-K backward
 };
 
 // A sweep variant as the selection returns it
@@ -2145,9 +2142,9 @@ static int bwd_f32_maps(const SeqArgs& a, PersistParams& p, int rows, cudaStream
 }
 
 // The resident split-K backward: its workspace, the bias-gradient and fp16 gate-gradient outputs, the fp16 W_hh^T
-// (the forward pass's copy when there is one, else converted from the fp32 transpose), the maps over it and over the
-// fp16 gate gradients, and max |dY[t]| per time step (the step-0 scale, and part of every later step's scale: spiky
-// upstream gradients).  *ctl_bytes: the control block and gmax, which are zeroed.
+// (the forward pass's copy when there is one, else made here by the same one-pass conversion), the maps over it and
+// over the fp16 gate gradients, and max |dY[t]| per time step (the step-0 scale, and part of every later step's scale:
+// spiky upstream gradients).  *ctl_bytes: the control block and gmax, which are zeroed.
 static int prepare_res_bwd(const SweepChoice& c, const SeqArgs& a, void* ws, PersistParams& p, cudaStream_t st,
                            size_t* ctl_bytes) {
   using namespace rp;
@@ -2170,8 +2167,8 @@ static int prepare_res_bwd(const SweepChoice& c, const SeqArgs& a, void* ws, Per
   for (int d = 0; d < a.D; ++d) {
     const __half* wsrc = static_cast<const __half*>(a.w_hhT16[d]);
     if (!cached) {
-      if (int rc = transpose(GH, a.H, a.w_hh[d], a.w_hhT[d], st)) return rc;
-      DS2_LAUNCH(f32_to_f16_kernel, 132 * 4, 256, 0, st, wn, a.w_hhT[d], w.wT16 + (size_t)d * wn);
+      if (int rc = f32_to_f16_transpose(GH, a.H, a.w_hh[d], a.H, nullptr, 0, w.wT16 + (size_t)d * wn, GH, nullptr, st))
+        return rc;
       wsrc = w.wT16 + (size_t)d * wn;
     }
     int rc = make_tmap_f16(&p.tmW[d], wsrc, 2, GH, a.H, 1, (size_t)GH, 0, 64, UT * CL, 1);

@@ -2,7 +2,7 @@
 
 A training forward in a tensor-core mode leaves an fp16 W_hh^T in its reserve for the backward sweep; a backward on a
 reserve the library did not see filled converts the weights itself (include/ds2_b200.h).  The forward's copy is
-f32_to_f16_transpose(W_hh) and the backward's own is f32_to_f16(transpose(W_hh)): the same fp16 values, so both
+f32_to_f16_transpose(W_hh) and the backward's own is the same call on the same W_hh: the same fp16 values, so both
 backwards must give the same bits.  One shape per backward sweep variant (tests/test_gpu_sweep_selection.py) and one
 that falls back to the FFMA step kernels.  Only the resident split-K variants read the fp16 W_hh^T; the streaming,
 16-unit and FFMA backwards make the fp32 transpose either way, so for those shapes the two backwards take the same
